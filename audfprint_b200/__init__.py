@@ -1,4 +1,4 @@
-"""audfprint_b200 — Blackwell-native (sm_100a) landmark audio-fingerprint engine
+"""audfprint_b200 — H100-native (sm_90a) landmark audio-fingerprint engine
 behind the Analyzer / HashTable / Matcher API of dpwe/audfprint.
 
 Only the one hot path of SURVEY.md §8 lives here: csrc/ (CUDA kernels + C ABI,

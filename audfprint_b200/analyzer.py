@@ -1,5 +1,5 @@
 """Analyzer — drop-in mirror of audfprint_analyze.Analyzer whose arithmetic
-runs in libafp.so (sm_100a CUDA) through the C ABI of include/afp.h.
+runs in libafp.so (sm_90a CUDA) through the C ABI of include/afp.h.
 
 Same attribute names, method names, argument meaning and error behaviour as the
 reference class (audfprint_analyze.py:115-457); the module-level helpers

@@ -1,4 +1,4 @@
-// Internal declarations shared by the libafp translation units (sm_100a only).
+// Internal declarations shared by the libafp translation units (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -62,7 +62,7 @@ struct TableDev {
 
 struct afp_ctx {
   int device = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   cudaStream_t stream = nullptr;
   bool own_stream = false;
   std::string err;

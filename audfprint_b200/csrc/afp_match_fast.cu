@@ -6,9 +6,8 @@
 // <= 1024, a few thousand track ids hit more than once.  Queries outside its capacities are
 // handed to the general kernel through a work list, so the pair is exact for every input.
 //
-// Why it is faster (profiles/r02_k4_match_r01final.txt: the general kernel moves 19x its
-// algorithmic bytes and spends its time on ~4 shared-memory atomics + ~90 bytes of HBM scratch per
-// probed table entry): a 10 s query touches ~80k table entries but only a few thousand track ids
+// Why it is faster (the general kernel spends ~4 shared-memory atomics + ~90 bytes of HBM scratch
+// per probed table entry): a 10 s query touches ~80k table entries but only a few thousand track ids
 // more than once, and only those can matter -
 //   * an id hit by ONE (bucket, slot) record has raw count m = the number of query rows that
 //     probe that bucket (<= shifts, and <= threshcount or it is treated as a multi-record id), so
@@ -23,8 +22,8 @@
 //     (set slot, dtime) of members to a short list; the exact raw counts are then a histogram
 //     of that list;
 //   * the top-K members by (weight desc, id desc) come from a histogram select on the float
-//     image of the weight (monotone), then a bitonic sort of the few hundred survivors (a full
-//     sort of the ~6000 members cost 45 % of the first version of this kernel);
+//     image of the weight (monotone), then a bitonic sort of the few hundred survivors (cheaper than
+//     a full sort of the ~6000 members);
 //     single-record ids are provably out when  min(m_max, threshcount) / min(hashesperid) <
 //     K-th member weight; otherwise pass 3 re-reads only the bucket groups whose multiplicity
 //     could reach that weight, gathers hashesperid for their non-member ids and admits the

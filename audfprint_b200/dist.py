@@ -6,7 +6,7 @@ pickling results back.  The same shape is used here:
 
 * fingerprinting: file i -> rank i % world; NO data-path collective (results are
   per-file and gathered as host objects only if the caller asks for them);
-* matching, table replicated (419 MB << 180 GB): query j -> rank j % world; no
+* matching, table replicated (419 MB << 80 GB): query j -> rank j % world; no
   collective;
 * matching, table sharded by track-id range (SURVEY.md §8e, BASELINE configs[4]):
   every rank sees every query, computes the candidate list and result rows of

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — audio-seconds fingerprinted per second (BASELINE.json metric).
 
-  python bench.py --gpus N --steps K --warmup W            # this framework (CUDA, sm_100a)
+  python bench.py --gpus N --steps K --warmup W            # this framework (CUDA, sm_90a)
   python bench.py --impl reference --gpus N --steps K ...  # CPU arm: the oracle port of the
                                                            # reference path on all host cores
 
@@ -15,6 +15,9 @@ Prints ONE JSON line (rank 0).  `value` has the PCM already resident in HBM;
 `e2e` goes through Analyzer.fingerprint_packed with pinned HOST buffers, the
 host->device copy of the PCM and the device->host read of the hashes inside the
 timed region.
+
+  --dump-outputs DIR  after the timed steps, write the hashes of the last timed step as .npy
+                      files (see dump_outputs), so that two builds can be compared output for output
 """
 from __future__ import annotations
 
@@ -83,12 +86,12 @@ _TRACKS = None      # set before the CPU pool is forked: workers inherit the PCM
 
 
 def reference_dir():
-    """A checkout of the reference (dpwe/audfprint) if one is reachable: $AFP_REFERENCE,
-    baseline/_ref, /root/reference.  It is pure Python and is NOT part of this repo, so on the
-    GPU box there is normally none and the CPU arm is the oracle port (`kind: "port"`)."""
-    for d in (os.environ.get("AFP_REFERENCE"), os.path.join(ROOT, "baseline", "_ref"), "/root/reference"):
-        if d and os.path.isfile(os.path.join(d, "audfprint_analyze.py")):
-            return d
+    """The checkout of the reference (dpwe/audfprint) that $AFP_REFERENCE names, if any.  It is
+    pure Python and is NOT part of this repo; without it the CPU arm is the oracle port
+    (`kind: "port"`)."""
+    d = os.environ.get("AFP_REFERENCE")
+    if d and os.path.isfile(os.path.join(d, "audfprint_analyze.py")):
+        return d
     return None
 
 
@@ -314,7 +317,7 @@ def bench_match(a, an, ctx, tracks, rows, roff, queries, cores, want_cpu, stream
     res = m.match_batch(ht, (qrows, qoff))
     warm_up(lambda: m.match_batch(ht, (qrows, qoff)))
     # --- match only, host hashes in / rows out (includes H2D of the query hashes, D2H of rows)
-    steps = 5
+    steps = a.steps
     torch.cuda.synchronize()
     t0 = time.perf_counter()
     for _ in range(steps):
@@ -447,7 +450,7 @@ def bench_match_sharded(a, an, rows, roff, qpool, rank, world):
         for qb in batches:
             full += m.match_batch(ht, qb, sort=False)
     # ---- replicated table, queries sharded j % world (no collective): the fast layout when
-    # the table fits one GPU (419 MB << 180 GB), SURVEY.md 8e
+    # the table fits one GPU (419 MB << 80 GB), SURVEY.md 8e
     mine = afd.shard_indices(nq, rank, world)
     my_rows = np.ascontiguousarray(np.concatenate([qh[i] for i in mine])) if len(mine) else np.zeros((0, 2), np.int32)
     my_off = np.zeros(len(mine) + 1, np.int64)
@@ -479,7 +482,7 @@ def bench_match_sharded(a, an, rows, roff, qpool, rank, world):
     dbatches = [(torch.from_numpy(qb[0]).cuda(), qb[1]) for qb in batches]   # query hashes resident, like the N=1 `value`
     for k in range(24):         # collective calls: the same count on every rank; ~0.4 s of GPU work
         afd.match_sharded_batch(m, ht, dbatches[k % len(dbatches)], row_cap=16, fetch=False)
-    steps = 3
+    steps = a.steps
     dist.barrier()
     torch.cuda.synchronize()
     t0 = time.perf_counter()
@@ -665,7 +668,7 @@ def bench_ingest(a, rank, local_rank, world, cores, pool):
                "gpu_launches": int(launches),
                "split_ms_per_step": {"fingerprint_kernels": fp_ms / a.steps, "store_and_host": ms_total / a.steps - fp_ms / a.steps},
                "roofline": {"kernel": "afp_stft_kernel<int16> (K1)", "bound": "hbm", "unit": "GB/s", "peak": peak,
-                            "peak_source": which, "algorithmic_bytes_per_launch": k1_bytes, "traffic": None,
+                            "peak_source": which, "algorithmic_bytes_per_launch": k1_bytes,
                             "launch_ms": k1_ms / a.steps, "achieved": k1_bytes / (k1_ms / a.steps * 1e-3) / 1e9,
                             "frac": k1_bytes / (k1_ms / a.steps * 1e-3) / 1e9 / peak},
                "table": {"tracks": ntracks, "hashes_stored_or_dropped": nh, "bucket_fill": full, "dropped_fraction": dropped},
@@ -677,21 +680,58 @@ def bench_ingest(a, rank, local_rank, world, cores, pool):
 
 
 def measured_peaks():
+    """HBM bandwidth the roofline fractions divide by: a measured value from MEASURED_PEAKS.json
+    ({"hbm_gbs": ...}) when one is present, else the H100 SXM data-sheet figure (3.35 TB/s)."""
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured"
     except Exception:
-        return 6650.0, "fallback"
+        return 3350.0, "H100 SXM data sheet"
+
+
+DUMP_BYTES = 64 << 20
+
+
+def fetch_last_hashes(ctx, nfiles):
+    """(rows int32 (U,2), row_offsets int64 (nfiles+1)) of the last fingerprint call on `ctx`,
+    as Analyzer.fingerprint_packed would have returned them, without running it again."""
+    import ctypes as C
+    roff = np.empty(nfiles + 1, np.int64)
+    ctx.check(ctx.lib.afp_fetch_hashes(ctx.h, None, 1, roff.ctypes.data_as(C.POINTER(C.c_int64))))
+    rows = np.empty((int(roff[-1]), 2), np.int32)
+    ctx.check(ctx.lib.afp_fetch_hashes(ctx.h, rows.ctypes.data, 1, None))
+    return rows, roff
+
+
+def dump_outputs(out_dir, rows, roff):
+    """Write hashes.npy ((time, hash) rows), row_offsets.npy (rows of file i are
+    hashes[row_offsets[i]:row_offsets[i+1]]) and files.npy (which files of the batch these
+    are), all float64.  When the whole batch would exceed DUMP_BYTES, a fixed, seeded sample
+    of whole files is written."""
+    nfiles = len(roff) - 1
+    counts = np.diff(roff)
+    files = np.arange(nfiles)
+    per_file = 2 * 8 * counts + 2 * 8                      # rows + offset + file index, float64
+    budget = DUMP_BYTES - 8                                # the leading 0 of row_offsets
+    if per_file.sum() > budget:
+        order = np.random.default_rng(0).permutation(nfiles)
+        n = int(np.searchsorted(np.cumsum(per_file[order]), budget, side="right"))
+        files = np.sort(order[:max(n, 1)])
+    out_rows = np.concatenate([rows[roff[i]:roff[i + 1]] for i in files]) if len(files) else rows[:0]
+    out_off = np.concatenate([[0], np.cumsum(counts[files])])
+    os.makedirs(out_dir, exist_ok=True)
+    for name, arr in (("hashes", out_rows), ("row_offsets", out_off), ("files", files)):
+        np.save(os.path.join(out_dir, name + ".npy"), np.asarray(arr, np.float64))
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--steps", type=int, default=None, help="timed steps (default 10; 12 with --config 3)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--files", type=int, default=1024, help="files per GPU per step")
-    ap.add_argument("--seconds", type=float, default=30.0)
+    ap.add_argument("--seconds", type=float, default=None, help="seconds per file (default 30; 180 with --config 3)")
     ap.add_argument("--cpu-sample", type=int, default=512, help="files in the CPU-baseline sample")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true",
@@ -703,16 +743,21 @@ def main():
     ap.add_argument("--e2e-files", type=int, default=256, help="--config 3: tracks per device call of the host-PCM leg")
     ap.add_argument("--match-batch", type=int, default=10000, help="queries per device call of the sharded match")
     ap.add_argument("--config", type=int, default=1, choices=[1, 2, 3, 4],
-                    help="BASELINE.json configs[]: 1 batch fingerprint (default; the driver's line), 2 match 10k "
+                    help="BASELINE.json configs[]: 1 batch fingerprint (default), 2 match 10k "
                          "queries on 1 GPU, 3 ingest 180 s tracks incl. store, 4 sharded-table match of 100k queries")
     ap.add_argument("--match-cpu-sample", type=int, default=1024,
                     help="queries in the CPU baseline / parity sample of the match leg (~3 s on 16 cores)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="--config 1: write the hashes of the last timed step to DIR (see dump_outputs)")
     a = ap.parse_args()
     if a.match_queries is None:
         a.match_queries = 100000 if a.config == 4 else 10000
-    if a.config == 3:
-        a.seconds = 180.0 if a.seconds == 30.0 else a.seconds
-        a.steps = 12 if a.steps == 10 else a.steps
+    if a.seconds is None:
+        a.seconds = 180.0 if a.config == 3 else 30.0
+    if a.steps is None:
+        a.steps = 12 if a.config == 3 else 10
+    if a.dump_outputs and (a.config != 1 or a.impl != "ours"):
+        ap.error("--dump-outputs writes the fingerprint workload of --config 1")
 
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -838,6 +883,8 @@ def main():
     clocks = sampler.stop()
     ctx.set_profiling(False)
     stages /= a.steps
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, *fetch_last_hashes(ctx, a.files))
 
     # ---- end to end: pinned host PCM in, hashes + offsets out, every step --------------------
     rows, roff = an.fingerprint_packed(dev_pcm, offs, sample_lengths=lens)
@@ -960,12 +1007,6 @@ def main():
         k1_bytes = a.files * (2 * nsamp + 8 * 256 * T + 8 * T)      # int16 PCM in, FP64 logs + nyq out
         k1_ms = float(stages[1])
         achieved = k1_bytes / (k1_ms * 1e-3) / 1e9
-        traffic = None
-        try:
-            with open(os.path.join(ROOT, "profiles", "k1_traffic.json")) as f:
-                traffic = json.load(f).get("dram_bytes_per_launch")
-        except Exception:
-            pass
         out = {"metric": METRIC, "value": audio_s * world * a.steps / (ms_total * 1e-3), "unit": UNIT,
                "n_gpus": world, "steps": a.steps, "warmup": max(a.warmup, 3), "ms_per_step": ms_total / a.steps,
                "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f64",
@@ -978,9 +1019,7 @@ def main():
                "gpu_launches": int(launches),
                "roofline": {"kernel": "afp_stft_kernel<int16> (K1: frame+window+512-pt real FFT+log|.|, FP64)",
                             "bound": "hbm", "achieved": achieved, "peak": peak, "peak_source": which,
-                            "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
-                            "traffic_source": "dram__bytes_read+write of one launch, ncu --set full capture "
-                                              "profiles/r01_v5_k1_stft.txt (K1 is unchanged since)",
+                            "unit": "GB/s", "frac": achieved / peak,
                             "algorithmic_bytes_per_launch": k1_bytes, "launch_ms": k1_ms},
                "stages_ms": {"h2d": float(stages[0]), "k1_stft_log": float(stages[1]),
                              "stats": float(stages[2]), "k2_peaks": float(stages[3]),
@@ -991,7 +1030,7 @@ def main():
             # BASELINE configs[2] / configs[4]: the match leg is the headline line, the fingerprint
             # numbers of the same run ride along
             line = dict(match)
-            line.update({"n_gpus": world, "steps": 3 if world > 1 else 5, "warmup": 2, "higher_is_better": True,
+            line.update({"n_gpus": world, "steps": a.steps, "warmup": 2, "higher_is_better": True,
                          "scaling": "strong" if world > 1 else "weak", "vs_baseline": None, "dtype": "u32",
                          "data": "synthetic", "clocks": clocks, "gpu_launches": 2,
                          "config": {"workload": ("match %d x 10 s noisy synthetic queries (4 shifts) against a "

@@ -1,5 +1,5 @@
 /*
- * afp.h — C ABI of libafp.so, the sm_100a landmark-fingerprint engine.
+ * afp.h — C ABI of libafp.so, the sm_90a (H100) landmark-fingerprint engine.
  *
  * This is the drop-in boundary for the ONE hot path SURVEY.md §8 scopes.  The
  * reference (dpwe/audfprint @ cb03ba99) is pure Python and has no FFI of its

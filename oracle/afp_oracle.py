@@ -13,11 +13,11 @@ Rules of use (see the task's parity section):
 
 Pinning: the reference ships no numeric known-answer tests for this path
 (SURVEY.md §4, §8c).  The oracle is therefore pinned against OUTPUTS OF THE LIVE
-REFERENCE, imported from /root/reference in the build container by
+REFERENCE, imported from a checkout of it by
 `oracle/make_golden.py`, committed as `tests/golden/*.npz`;
 `tests/test_oracle_golden.py` checks this module against them bit-for-bit.
 
-Third-party arithmetic the reference leans on (not under /root/reference,
+Third-party arithmetic the reference leans on (not part of the reference,
 un-pinned in requirements.txt:1-2): numpy (pocketfft `rfft`, `log`, `exp`,
 `mean`) and `scipy.signal.lfilter`.  The oracle calls the same numpy routines
 and restates lfilter's direct-form-II-transposed recurrence explicitly.

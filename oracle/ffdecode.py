@@ -1,4 +1,4 @@
-"""TEST INFRASTRUCTURE (build container only) - decode the reference's bundled
+"""TEST INFRASTRUCTURE (golden generation only) - decode the reference's bundled
 tests/data/*.mp3 the way the reference's own reader does.
 
 The reference reads audio by piping `ffmpeg -i FILE -f s16le -ac 1 -ar 11025 -`

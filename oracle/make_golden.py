@@ -1,8 +1,8 @@
-"""Generate tests/golden/*.npz by running the LIVE reference (read-only at
-/root/reference) on the deterministic cases of tests/cases.py.
+"""Generate tests/golden/*.npz by running the LIVE reference on the
+deterministic cases of tests/cases.py.
 
-Run in the build container only (the GPU box has no /root/reference):
-    python oracle/make_golden.py
+Needs a checkout of the reference (dpwe/audfprint) named by $AFP_REFERENCE:
+    AFP_REFERENCE=<checkout> python oracle/make_golden.py
 
 Only OUTPUT ARRAYS of the reference are stored; no reference source is copied.
 The reference's file reader is replaced by an in-memory PCM provider because
@@ -18,7 +18,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-REF = os.environ.get("AFP_REFERENCE", "/root/reference")
+REF = os.environ["AFP_REFERENCE"]
 sys.path.insert(0, REF)
 
 import audfprint_analyze as ref_an      # noqa: E402  (the reference)

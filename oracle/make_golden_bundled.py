@@ -1,5 +1,5 @@
 """Golden vectors from the reference's OWN bundled test material
-(/root/reference/tests/data: Nine_Lives/*.mp3 + query.mp3), i.e. what the
+(tests/data of the reference: Nine_Lives/*.mp3 + query.mp3), i.e. what the
 reference's Makefile exercises (`make test_onecore`: new / add / match at
 --density 100, Makefile:12-29), produced by the LIVE reference.
 
@@ -10,12 +10,12 @@ the FFmpeg libraries vendored with OpenCV, with the parameters of the
 reference's `ffmpeg -f s16le -ac 1 -ar 11025` pipe (audio_read.py:196-203), and
 the live reference runs on that PCM with its reader replaced by the decoder.
 
-Run in the build container only (the GPU box has no /root/reference):
-    python oracle/make_golden_bundled.py
+Needs a checkout of the reference (dpwe/audfprint) named by $AFP_REFERENCE:
+    AFP_REFERENCE=<checkout> python oracle/make_golden_bundled.py
 Stored in tests/golden/bundled.npz: reference OUTPUTS (hashes, table rows,
 match rows, report lines) and the decoded int16 PCM of the query and of
-PCM_TRACKS (the input the GPU parity tests need; the GPU box has neither the
-MP3s nor /root/reference).  No reference source is copied.
+PCM_TRACKS (the input the GPU parity tests need, so that they need neither the
+MP3s nor the reference).  No reference source is copied.
 """
 from __future__ import annotations
 
@@ -28,7 +28,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-REF = os.environ.get("AFP_REFERENCE", "/root/reference")
+REF = os.environ["AFP_REFERENCE"]
 sys.path.insert(0, REF)
 
 import audfprint_analyze as ref_an      # noqa: E402  (the reference)

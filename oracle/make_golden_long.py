@@ -3,7 +3,8 @@
 stored times alias (180 s > 2^12 frames = 95 s) built by the reference's own `store`, queried by
 the reference's own `match_hashes`.
 
-Run in the build container only:   python oracle/make_golden_long.py
+Needs a checkout of the reference (dpwe/audfprint) named by $AFP_REFERENCE:
+    AFP_REFERENCE=<checkout> python oracle/make_golden_long.py
 Stores only OUTPUT arrays of the reference in tests/golden/long.npz.
 """
 from __future__ import annotations
@@ -16,7 +17,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-REF = os.environ.get("AFP_REFERENCE", "/root/reference")
+REF = os.environ["AFP_REFERENCE"]
 sys.path.insert(0, REF)
 
 import audfprint_analyze as ref_an      # noqa: E402

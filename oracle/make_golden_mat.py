@@ -3,7 +3,8 @@
 reference's loader indexes (HT_params struct, HashTable depth x buckets, cell array of names);
 tests/golden/matlab_db_arrays.npz holds the attributes of the reference object after loading it.
 
-Run in the build container only:  python oracle/make_golden_mat.py
+Needs a checkout of the reference (dpwe/audfprint) named by $AFP_REFERENCE:
+    AFP_REFERENCE=<checkout> python oracle/make_golden_mat.py
 """
 from __future__ import annotations
 
@@ -15,7 +16,7 @@ import scipy.io
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.environ.get("AFP_REFERENCE", "/root/reference"))
+sys.path.insert(0, os.environ["AFP_REFERENCE"])
 
 import hash_table as ref_ht             # noqa: E402  (the reference)
 

@@ -2,8 +2,8 @@
 hashesfor), produced by the LIVE reference Matcher (audfprint_match.py:149-352) on the
 databases and queries already stored in tests/golden/match.npz.
 
-Run in the build container only (the GPU box has no /root/reference):
-    python oracle/make_golden_options.py
+Needs a checkout of the reference (dpwe/audfprint) named by $AFP_REFERENCE:
+    AFP_REFERENCE=<checkout> python oracle/make_golden_options.py
 Only OUTPUT ARRAYS of the reference are stored; no reference source is copied.
 """
 from __future__ import annotations
@@ -15,7 +15,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.environ.get("AFP_REFERENCE", "/root/reference"))
+sys.path.insert(0, os.environ["AFP_REFERENCE"])
 
 import audfprint_match as ref_ma        # noqa: E402  (the reference)
 import hash_table as ref_ht             # noqa: E402

@@ -1,5 +1,5 @@
 """GPU: the CUDA path on the reference's OWN bundled test material (the Nine_Lives excerpts
-and query.mp3 of /root/reference/tests/data - what `make test` of the reference runs,
+and query.mp3 of the reference's tests/data - what `make test` of the reference runs,
 Makefile:12-29), against what the LIVE reference produced on the same decoded PCM
 (tests/golden/bundled.npz, oracle/make_golden_bundled.py).  BASELINE.json north_star:
 "match results bit-identical to the reference on the bundled tests/data queries".

@@ -1,18 +1,11 @@
-"""CPU: the oracle against what the LIVE reference produced on its own bundled test
-material (/root/reference/tests/data: Nine_Lives/*.mp3 and query.mp3, the files of the
-reference's `make test`), stored in tests/golden/bundled.npz by
-oracle/make_golden_bundled.py.  The MP3s were decoded with FFmpeg's libraries at the
-parameters of the reference's `ffmpeg -f s16le -ac 1 -ar 11025` pipe (oracle/ffdecode.py).
-
-The first group runs anywhere (committed PCM of the query and of four tracks, reference
-outputs for all thirteen).  The second group needs the reference checkout and the vendored
-FFmpeg libraries (build container only): it re-decodes the MP3s, checks the nine tracks whose
-PCM is not committed, and runs the UNMODIFIED reference command line (`new`, `add`, `match`:
-Makefile:19-29) on the decoded audio to confirm the stored report lines."""
+"""CPU: the oracle against what the reference produced on its own bundled test material
+(tests/data of dpwe/audfprint: Nine_Lives/*.mp3 and query.mp3, the files of the reference's
+`make test`), stored in tests/golden/bundled.npz by oracle/make_golden_bundled.py.  The MP3s
+were decoded with FFmpeg's libraries at the parameters of the reference's
+`ffmpeg -f s16le -ac 1 -ar 11025` pipe (oracle/ffdecode.py); the golden file holds the PCM of
+the query and of four tracks, and the reference's outputs for all thirteen."""
 import os
 import random
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -20,8 +13,6 @@ import pytest
 from oracle import afp_oracle as orc
 from tests.conftest import GOLDEN, expand_table
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.environ.get("AFP_REFERENCE", "/root/reference")
 PCM_TRACKS = (0, 4, 8, 12)
 DENSITIES = (100.0, 20.0)
 # Matcher settings of oracle/make_golden_bundled.py on top of the command line's defaults
@@ -154,83 +145,3 @@ def test_mirror_report_lines_from_the_reference_rows(gb):
                 assert mt.file_match_to_msgs(an, Table, qname) == [str(x) for x in gb[key + "/msgs_terse"]], key
             checked += 1
     assert checked > 40
-
-
-# ---- build container only: the MP3s themselves and the live reference ------------------------
-def _have_decoder():
-    try:
-        from oracle import ffdecode
-        ffdecode._load()
-        return True
-    except Exception:
-        return False
-
-
-live = pytest.mark.skipif(not (os.path.isfile(os.path.join(REF, "tests", "data", "query.mp3")) and _have_decoder()),
-                          reason="needs the reference checkout and the vendored FFmpeg libraries")
-
-
-def _crc(pcm):
-    return int(np.bitwise_xor.reduce(pcm.astype(np.int64) * (np.arange(len(pcm)) % 8191 + 1)))
-
-
-@live
-def test_decoding_is_reproducible_and_oracle_holds_on_all_thirteen(gb):
-    from oracle import ffdecode
-    data = os.path.join(REF, "tests", "data")
-    names = [str(n) for n in gb["names"]] + [str(gb["query_name"])]
-    for i, name in enumerate(names):
-        pcm = ffdecode.decode(os.path.join(data, name))
-        assert len(pcm) == gb["pcm_lengths"][i] and _crc(pcm) == gb["pcm_crc"][i], name
-        if i in PCM_TRACKS:
-            assert np.array_equal(pcm, gb["track%d/pcm" % i])
-        if i < 13:
-            for dens in DENSITIES:
-                want = gb["d%d/track%d/hashes" % (int(dens), i)]
-                assert np.array_equal(orc.fingerprint(to_float(pcm), density=dens), want), (name, dens)
-    assert np.array_equal(ffdecode.decode(os.path.join(data, "query.mp3")), gb["query/pcm"])
-
-
-CLI_DRIVER = r'''
-import os, sys
-ROOT, REF = sys.argv[1], sys.argv[2]
-sys.path.insert(0, ROOT)
-from tests.test_reference_cli_cpu import DRIVER
-pre = DRIVER.split("sys.path.insert(0, REF)")[0]          # the docopt stand-in
-sys.argv = [sys.argv[0], ROOT, REF, "ref", sys.argv[3]]
-exec(pre)
-sys.path.insert(0, REF)
-import numpy as np
-import audio_read
-from oracle import ffdecode
-audio_read.audio_read = ffdecode.audio_read               # where the ffmpeg pipe stands
-import audfprint                                          # the reference's CLI, unmodified
-for argv in argv_sets:
-    audfprint.main(["audfprint"] + argv)
-'''
-
-
-@live
-def test_reference_command_line_on_the_bundled_files(gb, tmp_path):
-    """`make test_onecore` of the reference (Makefile:19-29) with the decoder in the place of
-    the ffmpeg pipe: the report line is the one stored in the golden file."""
-    data = os.path.join(REF, "tests", "data")
-    db = str(tmp_path / "fpdbase.pklz")
-    files = sorted(os.listdir(os.path.join(data, "Nine_Lives")))
-    first = [os.path.join("Nine_Lives", f) for f in files if f.startswith("0")]
-    rest = [os.path.join("Nine_Lives", f) for f in files if f.startswith("1")]
-    text = ""
-    for argv in (["new", "--dbase", db, "--density", "100"] + first,
-                 ["add", "--dbase", db, "--density", "100"] + rest,
-                 ["match", "--dbase", db, "--density", "100", "query.mp3"],
-                 ["match", "--dbase", db, "--density", "100", "--find-time-range", "--exact-count",
-                  "--max-matches", "5", "--sortbytime", "query.mp3"]):
-        out = subprocess.run([sys.executable, "-c", CLI_DRIVER, ROOT, REF, repr([argv])],
-                             capture_output=True, text=True, timeout=600, cwd=data)
-        assert out.returncode == 0, out.stdout + out.stderr
-        text += out.stdout
-    lines = text.splitlines()
-    assert str(gb["d100/query_s4/default/msgs"][0]) in lines
-    assert str(gb["d100/query_s4/exact_range_time/msgs"][0]) in lines
-    nh = int(np.sum(gb["d100/db/hashesperid"]))
-    assert any(ln.startswith("Saved fprints for 13 files ( %d hashes)" % nh) for ln in lines)

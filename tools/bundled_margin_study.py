@@ -45,6 +45,7 @@ def main():
         orc.stft_complex = exact
         out.append({"eps_of_largest_bin": eps, "fingerprints": total, "changed": int(flips)})
         print(out[-1])
+    os.makedirs(os.path.join(ROOT, "profiles"), exist_ok=True)
     with open(os.path.join(ROOT, "profiles", "r02_bundled_margin_study.json"), "w") as f:
         json.dump({"what": __doc__.strip().split("\n\n")[0], "results": out}, f, indent=1)
 
