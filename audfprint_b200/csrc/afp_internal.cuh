@@ -80,6 +80,7 @@ struct afp_ctx {
   // analyzer configuration
   afp_analyzer_params ap{};
   bool analyzer_set = false;
+  bool peaks_carveout_set = false;   // K2's shared-memory carveout has been raised on this device
   DevBuf d_window;   // 2 x 512 doubles: window, then window * 2^-15 (int16 PCM)
   DevBuf d_gauss;    // AFP_GAUSS_N doubles
   DevBuf d_window_f; // float copies for the FP32 spectrogram mode

@@ -11,7 +11,7 @@
 // The time recursion is strictly sequential inside an item, so the unit of
 // parallelism is ONE WARP PER ITEM (one warp per CTA): lane l owns bins
 // 8l..8l+7 (threshold, filter state and the current column live in registers), the column stream arrives through a TMA bulk-copy ring in shared
-// memory (3 chunks of 4 columns in flight per warp), neighbour compares use warp
+// memory (2 chunks of 4 columns per warp), neighbour compares use warp
 // shuffles, the per-column top-N selection uses redux.sync (warp-wide integer
 // max on the bit pattern of the positive doubles), and thousands of items run
 // concurrently.  All arithmetic that feeds a comparison is done with explicit
@@ -24,8 +24,21 @@ namespace {
 
 constexpr unsigned FULL = 0xffffffffu;
 constexpr int CH = 4;      // columns per TMA chunk (8 KB)
-constexpr int NST = 3;     // chunks in flight per warp (24 KB ring)
+constexpr int NST = 2;     // chunks in flight per warp (16 KB ring)
 constexpr int PFB = 8;     // prefetch distance (columns) of the backward pass
+
+// K2 is one warp per item and every item lasts about T column steps, so the kernel takes as many
+// item-durations as it has waves: the whole default batch (1024 items) has to be resident at once.
+// 10 CTAs per SM (1320 on a 132-SM H100 SXM, 1140 on a 114-SM H100 PCIe) leave 233,472 / 10 B of
+// shared memory per CTA, of which the runtime reserves 1 KB.
+constexpr int K2_CTAS_PER_SM = 10;
+constexpr size_t K2_SMEM_BUDGET = 233472 / K2_CTAS_PER_SM - 1024;
+constexpr size_t k2_static_smem(size_t rsize) {
+  return sizeof(double) * AFP_GAUSS_PAD + 128 /* sCol alignment */ + NST * CH * AFP_NBINS * rsize +
+         NST * sizeof(unsigned long long);
+}
+static_assert(k2_static_smem(sizeof(double)) <= K2_SMEM_BUDGET,
+              "K2's shared memory would fit fewer than 10 CTAs per SM: a 1024-item batch would run in two waves");
 
 struct PeakArgs {
   const ItemDesc* items;
@@ -57,11 +70,22 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 }
 
 // thr = max(thr, val * E[bin - pos]) for the 8 bins of this lane
-// (audfprint_analyze.py:225-227 / :193-196)
+// (audfprint_analyze.py:225-227 / :193-196).
+// A threshold starts at 0 and is only ever raised by max() or scaled by a_dec > 0, so it is
+// never NaN: compare-and-select then makes the same decisions as fmax(), without its NaN fix-up.
+// The 8 entries are consecutive in the table; in its padded layout those from the next group
+// of 8 on sit one element further, so two base addresses serve all 8 loads.
 __device__ __forceinline__ void bump(double (&thr)[8], const double* sE, int lane, int pos, double val) {
   const int k0 = AFP_NBINS - pos + 8 * lane;
+  const uint32_t e0 = smem_u32(sE + gidx(k0)), e1 = e0 + 8;
+  const int split = 8 - (k0 & 7);   // gidx(k0 + j) == gidx(k0) + j + (j >= split)
 #pragma unroll
-  for (int j = 0; j < 8; ++j) thr[j] = fmax(thr[j], __dmul_rn(val, sE[gidx(k0 + j)]));
+  for (int j = 0; j < 8; ++j) {
+    double e;
+    asm volatile("ld.shared.f64 %0, [%1];" : "=d"(e) : "r"((j >= split ? e1 : e0) + 8 * j) : "memory");
+    const double p = __dmul_rn(val, e);
+    thr[j] = p > thr[j] ? p : thr[j];
+  }
 }
 
 __device__ __forceinline__ double pick(const double (&v)[8], int j) {
@@ -153,11 +177,8 @@ struct ColRing {
           : "memory");
     }
   }
-  // read column t; with `consume`, the chunk is recycled after its last column
-  __device__ __forceinline__ void load(int t, double (&x)[8], bool consume) const {
-    const int chunk = t / CH;
-    if (t % CH == 0 || !consume) wait(chunk);
-    const R* col = buf + ((chunk % NST) * CH + t % CH) * AFP_NBINS;
+  // this lane's 8 values of one column (shared or global memory)
+  __device__ __forceinline__ void read(const R* col, double (&x)[8]) const {
     if (sizeof(R) == 8) {
       const double2* p = reinterpret_cast<const double2*>(col) + 4 * lane;
 #pragma unroll
@@ -172,7 +193,15 @@ struct ColRing {
       x[0] = u.x; x[1] = u.y; x[2] = u.z; x[3] = u.w;
       x[4] = v.x; x[5] = v.y; x[6] = v.z; x[7] = v.w;
     }
-    if (consume && (t % CH == CH - 1 || t == T - 1)) {
+  }
+  // column t straight from global memory, bypassing the ring
+  __device__ __forceinline__ void peek(int t, double (&x)[8]) const { read(src + (size_t)t * AFP_NBINS, x); }
+  // column t from the ring; the chunk is recycled after its last column
+  __device__ __forceinline__ void load(int t, double (&x)[8]) const {
+    const int chunk = t / CH;
+    if (t % CH == 0) wait(chunk);
+    read(buf + ((chunk % NST) * CH + t % CH) * AFP_NBINS, x);
+    if (t % CH == CH - 1 || t == T - 1) {
       __syncwarp();
       if (lane == 0 && (chunk + NST) * CH < T) issue(chunk + NST);
     }
@@ -214,14 +243,15 @@ __global__ void __launch_bounds__(32) afp_peaks_kernel(PeakArgs a) {
   double thr[8], z[8], s[8], sn[8], l[8];
 
   // ---- initial threshold: spread of the per-bin max over the first 10 columns
-  // (audfprint_analyze.py:204-206); the ring holds columns 0..11, nothing is consumed yet
+  // (audfprint_analyze.py:204-206), read from global memory while the ring fills with columns
+  // 0..NST*CH-1 for the forward pass (the ring is smaller than 10 columns)
   {
     double mx[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) { z[j] = 0.0; mx[j] = -INFINITY; }
     const int n0 = min(10, T);
     for (int t = 0; t < n0; ++t) {
-      ring.load(t, l, false);
+      ring.peek(t, l);
       hpf_step(l, z, s, lf, mean, pole);
 #pragma unroll
       for (int j = 0; j < 8; ++j) mx[j] = fmax(mx[j], s[j]);
@@ -234,13 +264,13 @@ __global__ void __launch_bounds__(32) afp_peaks_kernel(PeakArgs a) {
   // the threshold) before the threshold-dependent decisions of column t.
 #pragma unroll
   for (int j = 0; j < 8; ++j) z[j] = 0.0;
-  ring.load(0, l, true);
+  ring.load(0, l);
   hpf_step(l, z, s, lf, mean, pole);
   unsigned lm = locmax_mask(s, lane);
   for (int t = 0; t < T; ++t) {
     unsigned lmn = 0;
     if (t + 1 < T) {
-      ring.load(t + 1, l, true);
+      ring.load(t + 1, l);
       hpf_step(l, z, sn, lf, mean, pole);
       lmn = locmax_mask(sn, lane);
     }
@@ -467,6 +497,14 @@ int afp_launch_peaks(afp_ctx* c, int item0, int nitems) {
   a.pk_cnt = c->d_pk_cnt.as<uint8_t>();
   a.item_scols = c->d_item_scols.as<int32_t>();
   a.item_npeaks = c->d_item_npeaks.as<int32_t>();
+  if (!c->peaks_carveout_set) {
+    // the whole per-SM shared memory for K2, so that K2_CTAS_PER_SM items fit on every SM
+    AFP_CUDA(c, cudaFuncSetAttribute(afp_peaks_kernel<double>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                     cudaSharedmemCarveoutMaxShared));
+    AFP_CUDA(c, cudaFuncSetAttribute(afp_peaks_kernel<float>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                     cudaSharedmemCarveoutMaxShared));
+    c->peaks_carveout_set = true;
+  }
   if (c->ap.spectrogram_fp32) afp_peaks_kernel<float><<<nitems, 32, 0, c->stream>>>(a);
   else afp_peaks_kernel<double><<<nitems, 32, 0, c->stream>>>(a);
   AFP_CUDA(c, cudaGetLastError());
