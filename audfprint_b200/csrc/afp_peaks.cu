@@ -19,6 +19,7 @@
 // of the reference, so given the same spectrogram the decisions are bit-exact.
 #include <math.h>
 #include "afp_internal.cuh"
+#include "afp_tma.cuh"
 
 namespace {
 
@@ -64,10 +65,6 @@ __device__ __forceinline__ int bin_of(int lane, int j) { return 8 * lane + j; }
 __device__ __forceinline__ int lane_of(int pos) { return pos >> 3; }
 __device__ __forceinline__ int reg_of(int pos) { return pos & 7; }
 __device__ __forceinline__ int gidx(int k) { return k + (k >> 3); }   // padded table index
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-  return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
 
 // thr = max(thr, val * E[bin - pos]) for the 8 bins of this lane
 // (audfprint_analyze.py:225-227 / :193-196).
@@ -156,27 +153,9 @@ struct ColRing {
   __device__ __forceinline__ void issue(int chunk) const {   // lane 0 only
     const int c0 = chunk * CH;
     const uint32_t bytes = (uint32_t)min(CH, T - c0) * AFP_NBINS * sizeof(R);
-    unsigned long long* b = bar + (chunk % NST);
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(b)), "r"(bytes) : "memory");
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                     smem_u32(buf + (chunk % NST) * CH * AFP_NBINS)),
-                 "l"(src + (size_t)c0 * AFP_NBINS), "r"(bytes), "r"(smem_u32(b))
-                 : "memory");
+    bulk_copy_g2s(buf + (chunk % NST) * CH * AFP_NBINS, src + (size_t)c0 * AFP_NBINS, bytes, bar + (chunk % NST));
   }
-  __device__ __forceinline__ void wait(int chunk) const {
-    const uint32_t parity = (chunk / NST) & 1;
-    uint32_t done = 0;
-    while (!done) {
-      asm volatile(
-          "{\n\t.reg .pred p;\n\t"
-          "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-          "selp.u32 %0, 1, 0, p;\n\t}"
-          : "=r"(done)
-          : "r"(smem_u32(bar + (chunk % NST))), "r"(parity)
-          : "memory");
-    }
-  }
+  __device__ __forceinline__ void wait(int chunk) const { mbar_wait(bar + (chunk % NST), (chunk / NST) & 1); }
   // this lane's 8 values of one column (shared or global memory)
   __device__ __forceinline__ void read(const R* col, double (&x)[8]) const {
     if (sizeof(R) == 8) {
@@ -233,8 +212,7 @@ __global__ void __launch_bounds__(32) afp_peaks_kernel(PeakArgs a) {
   }
   ColRing<R> ring{sCol, sBar, reinterpret_cast<const R*>(a.logs) + base * AFP_NBINS, T, lane};
   if (lane == 0) {
-    for (int i = 0; i < NST; ++i) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(sBar + i)));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_init<NST>(sBar);
     for (int c = 0; c < NST && c * CH < T; ++c) ring.issue(c);
   }
   __syncwarp();

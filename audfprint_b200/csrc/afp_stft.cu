@@ -21,47 +21,25 @@
 // way the reference's float64 NumPy path does; an FP32 spectrogram flips a
 // decision roughly once per 10^5 frames (DESIGN.md "Precision").  The kernel is
 // therefore bound by the FP64 pipe (64 lanes/clk/SM), not by HBM; the log is a
-// table-driven FP64 routine (10 FP64 ops instead of libdevice's ~30).
+// table-driven FP64 routine (10 FP64 ops instead of libdevice's ~30).  The opt-in
+// FP32 spectrogram mode is the same kernel over R = float; K1Traits<R> holds what
+// differs between the two precisions.
 #include <math.h>
 #include <algorithm>
 #include "afp_fft.cuh"
 #include "afp_internal.cuh"
+#include "afp_tma.cuh"
 
 namespace {
 
 constexpr int FT = AFP_FRAMES_PER_TILE;   // 16 frames per tile
 constexpr int XS = 17;                    // padded row stride of the 16x16 exchange
-constexpr int XF = 16 * XS;               // 272 doubles per frame per component
+constexpr int XF = 16 * XS;               // 272 values per frame per component
 constexpr int K1_THREADS = 256;
 constexpr int LOGTAB = 64;                // log table entries (6 mantissa bits) ...
 constexpr int LOGCOPIES = 8;              // ... each stored 8 times, copy j in the 16-byte bank group j:
                                           // lane (l & 7) reads copy (l & 7), so the random lookups of a
                                           // quarter-warp never collide (4 wavefronts per LDS.128, always)
-
-struct StftArgs {
-  const void* pcm;
-  const ItemDesc* items;
-  const int32_t* tile_item;   // [ntiles] item of every tile (built by afp_tile_table_kernel)
-  int nitems;
-  int tile_begin, tile_end;   // tile range of this launch (a chunk of the batch)
-  const double* window;   // 512 (pre-scaled by 2^-15 for int16 PCM)
-  const double2* tw256;   // [p][r] = W256^(r*p), (cos, -sin)
-  const double2* w512;    // 256: (cos, -sin)(2 pi k / 512)
-  const double2* logtab;  // [64][8]: (c_i, -0.5*log(c_i)), 8 identical copies interleaved
-  double* logs;           // [frames][256]
-  double* nyq;            // [frames]
-  double* tile_stats;     // [tiles][3]
-  double* mag;            // optional [frames][257]
-  // FP32 spectrogram mode (opt-in, NOT bit-identical downstream; see DESIGN.md)
-  const float* window_f;  // 512 (pre-scaled by 2^-15 for int16 PCM)
-  const float2* tw256_f;  // [p][r]
-  const float2* w512_f;   // 256
-  float* logs_f;          // [frames][256]
-};
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-  return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
 
 // np.pad(..., mode='reflect') index map (edge sample not repeated), any number
 // of bounces (stft.py:88; SURVEY.md A.1).
@@ -109,19 +87,106 @@ __device__ __forceinline__ double half_log_quarter(double v, const double2* s_lo
 template <typename PcmT> struct PcmTraits;
 template <> struct PcmTraits<int16_t> {
   static constexpr int NBUF = 2;
+};
+template <> struct PcmTraits<float> {
+  static constexpr int NBUF = 1;   // 2 x 17 KB would not leave room for two CTAs per SM
+};
+
+// What differs between the two spectrogram precisions of K1.  load2 converts two PCM samples
+// (int16 unscaled: the window carries the 2^-15); log_pair / log1 give 0.5*log(0.25*v) of
+// v = 4|X|^2; hbits maps a positive v to an int that orders like it, HMIN_NONE being the value
+// of a warp without a frame; log_lower_bound turns the warp's minimum hbits into a lower bound
+// of its smallest log.
+template <typename R> struct K1Traits;
+
+// FP64 (default): table-driven log, bit-exact downstream.
+template <> struct K1Traits<double> {
+  using R2 = double2;
+  static constexpr int MIN_CTAS = 2;                    // per SM: 2 x 256 threads x <= 128 registers
+  static constexpr int LOGTAB_N = LOGTAB * LOGCOPIES;   // log table entries staged in shared memory
+  static constexpr int HMIN_NONE = 0x7ff00000;          // high word of +inf
   __device__ static __forceinline__ void load2(const int16_t* p, double& a, double& b) {
     const uint32_t w = *reinterpret_cast<const uint32_t*>(p);
     a = int_to_double((int)(short)(w & 0xffffu));
     b = int_to_double((int)w >> 16);
   }
-};
-template <> struct PcmTraits<float> {
-  static constexpr int NBUF = 1;   // 2 x 17 KB would not leave room for two CTAs per SM
   __device__ static __forceinline__ void load2(const float* p, double& a, double& b) {
     const float2 w = *reinterpret_cast<const float2*>(p);
     a = (double)w.x;
     b = (double)w.y;
   }
+  // the high word alone: positive doubles order like their bits
+  __device__ static __forceinline__ int hbits(double v) { return __double2hiint(v); }
+  __device__ static __forceinline__ void log_pair(double ssa, double ssb, const double2* tab, double& la,
+                                                  double& lb) {
+    la = half_log_quarter(ssa, tab);
+    lb = half_log_quarter(ssb, tab);
+    if (is_special(ssa) || is_special(ssb)) {   // digital silence etc.: rare, off the hot path
+      la = half_log_quarter_slow(ssa);
+      lb = half_log_quarter_slow(ssb);
+    }
+  }
+  __device__ static __forceinline__ double log1(double ss, const double2* tab) {
+    double lg = half_log_quarter(ss, tab);
+    if (is_special(ss)) lg = half_log_quarter_slow(ss);
+    return lg;
+  }
+  // the log of the high word with the low word zeroed: the statistics pass only asks "is
+  // anything below the floor?"; a false alarm just takes its exact path
+  __device__ static __forceinline__ double log_lower_bound(int hmin, const double2* tab) {
+    const double v_lo = __hiloint2double(hmin, 0);
+    return hmin >= HMIN_NONE ? INFINITY : (hmin < 0x00100000 ? -INFINITY : half_log_quarter(v_lo, tab));
+  }
+};
+
+// FP32 (Analyzer.precision = 'fp32', opt-in): FFT, |.|^2 and log (MUFU) in single precision,
+// float log-spectrogram out: half the output bytes, twice the FP32 lane rate, ~80 registers ->
+// three CTAs per SM.  Downstream decisions then see values that differ from the reference's
+// by ~1e-7 relative, so hashes are NOT guaranteed bit-identical (measured in bench.py).
+template <> struct K1Traits<float> {
+  using R2 = float2;
+  static constexpr int MIN_CTAS = 3;                    // per SM: 3 x 256 threads x <= 80 registers
+  static constexpr int LOGTAB_N = 0;
+  static constexpr int HMIN_NONE = 0x7f800000;          // bits of +inf
+  __device__ static __forceinline__ void load2(const int16_t* p, float& a, float& b) {
+    const uint32_t w = *reinterpret_cast<const uint32_t*>(p);
+    a = (float)(short)(w & 0xffffu);
+    b = (float)((int)w >> 16);
+  }
+  __device__ static __forceinline__ void load2(const float* p, float& a, float& b) {
+    const float2 w = *reinterpret_cast<const float2*>(p);
+    a = w.x;
+    b = w.y;
+  }
+  __device__ static __forceinline__ int hbits(float v) { return __float_as_int(v); }
+  __device__ static __forceinline__ void log_pair(float ssa, float ssb, const double2*, float& la, float& lb) {
+    la = 0.5f * __logf(0.25f * ssa);
+    lb = 0.5f * __logf(0.25f * ssb);
+  }
+  __device__ static __forceinline__ float log1(float ss, const double2*) { return 0.5f * __logf(0.25f * ss); }
+  // the exact minimum's log, less a margin for __logf's error so that it stays a lower bound
+  __device__ static __forceinline__ double log_lower_bound(int hmin, const double2*) {
+    return hmin >= HMIN_NONE ? INFINITY
+           : (hmin < 0x00800000 ? -INFINITY : (double)(0.5f * __logf(0.25f * __int_as_float(hmin))) - 1e-6);
+  }
+};
+
+template <typename R>
+struct StftArgs {
+  using R2 = typename K1Traits<R>::R2;
+  const void* pcm;
+  const ItemDesc* items;
+  const int32_t* tile_item;   // [ntiles] item of every tile (built by afp_tile_table_kernel)
+  int nitems;
+  int tile_begin, tile_end;   // tile range of this launch (a chunk of the batch)
+  const R* window;        // 512 (pre-scaled by 2^-15 for int16 PCM)
+  const R2* tw256;        // [p][r] = W256^(r*p), (cos, -sin)
+  const R2* w512;         // 256: (cos, -sin)(2 pi k / 512)
+  const double2* logtab;  // [64][8]: (c_i, -0.5*log(c_i)), 8 identical copies interleaved (FP64 only)
+  R* logs;                // [frames][256]
+  double* nyq;            // [frames]
+  double* tile_stats;     // [tiles][3]
+  double* mag;            // optional [frames][257]
 };
 
 struct TileInfo {
@@ -136,7 +201,7 @@ struct TileInfo {
 };
 
 template <typename PcmT>
-__device__ __forceinline__ TileInfo make_tile(const StftArgs& a, const ItemDesc& it, int tile) {
+__device__ __forceinline__ TileInfo make_tile(const PcmT* pcm, const ItemDesc& it, int tile) {
   TileInfo ti;
   const int t0 = (tile - it.tile_base) * FT;
   ti.frame0 = it.frame_base + t0;
@@ -150,32 +215,17 @@ __device__ __forceinline__ TileInfo make_tile(const StftArgs& a, const ItemDesc&
   const int64_t run_n = (int64_t)(ti.nft + 1) * AFP_N_HOP;
   const int64_t lo = ti.j0 < 0 ? -ti.j0 : 0;
   const int64_t hi = (ti.j0 + run_n <= it.nsamples ? run_n : it.nsamples - ti.j0) & ~(int64_t)(GR - 1);
-  const bool aligned = (reinterpret_cast<uintptr_t>(reinterpret_cast<const PcmT*>(a.pcm) + ti.src) & 15) == 0;
+  const bool aligned = (reinterpret_cast<uintptr_t>(pcm + ti.src) & 15) == 0;
   ti.tma = (aligned && hi > lo) ? (int)((lo << 16) | (hi - lo)) : 0;   // lo is 0 or 256: a granule multiple
   return ti;
 }
 
 // Stage the PCM run of a tile: TMA bulk copy (one thread) or reflected loads (all).
 template <typename PcmT>
-__device__ __forceinline__ void stage_tile(const StftArgs& a, const TileInfo& ti, PcmT* dst,
-                                           unsigned long long* bar) {
-  const PcmT* pcm = reinterpret_cast<const PcmT*>(a.pcm);
+__device__ __forceinline__ void stage_tile(const PcmT* pcm, const TileInfo& ti, PcmT* dst, unsigned long long* bar) {
   const int nsamp = (ti.nft + 1) * AFP_N_HOP;
   const int t_first = ti.tma >> 16, t_count = ti.tma & 0xffff;
-  if (t_count) {
-    if (threadIdx.x == 0) {
-      const uint32_t bytes = t_count * sizeof(PcmT);
-      // order earlier generic-proxy accesses of this buffer before the async-proxy write
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
-                   : "memory");
-      asm volatile(
-          "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-              smem_u32(dst + t_first)),
-          "l"(pcm + ti.src + t_first), "r"(bytes), "r"(smem_u32(bar))
-          : "memory");
-    }
-  }
+  if (t_count && threadIdx.x == 0) bulk_copy_g2s(dst + t_first, pcm + ti.src + t_first, t_count * sizeof(PcmT), bar);
   if (t_count != nsamp) {   // samples outside the bulk copy: [0, t_first) and [t_first + t_count, nsamp)
     const PcmT* item0 = pcm + (ti.src - ti.j0);
     for (int i = threadIdx.x; i < nsamp - t_count; i += K1_THREADS) {
@@ -185,46 +235,45 @@ __device__ __forceinline__ void stage_tile(const StftArgs& a, const TileInfo& ti
   }
 }
 
-__device__ __forceinline__ void wait_bar(unsigned long long* bar, uint32_t parity) {
-  uint32_t done = 0;
-  while (!done) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-  }
+// Shared memory of one K1 CTA; the kernel carves it up in this order.
+template <typename R, typename PcmT>
+constexpr size_t k1_smem_bytes() {
+  return 512 * sizeof(R) + 2 * 256 * sizeof(typename K1Traits<R>::R2) + K1Traits<R>::LOGTAB_N * sizeof(double2) +
+         2 * FT * XF * sizeof(R) + 24 * sizeof(double) + 2 * sizeof(unsigned long long) +
+         PcmTraits<PcmT>::NBUF * (FT + 1) * AFP_N_HOP * sizeof(PcmT);
 }
 
-template <typename PcmT, bool WRITE_MAG>
-__global__ void __launch_bounds__(K1_THREADS, 2) afp_stft_kernel(StftArgs a) {
+// `a` is __grid_constant__: its fields are read from the parameter bank where they are used.
+// Passed by value, a struct this small is copied into registers at entry, and its pointers
+// then stay live across the whole persistent loop and spill.
+template <typename R, typename PcmT, bool WRITE_MAG>
+__global__ void __launch_bounds__(K1_THREADS, K1Traits<R>::MIN_CTAS)
+    afp_stft_kernel(const __grid_constant__ StftArgs<R> a) {
+  using Tr = K1Traits<R>;
+  using R2 = typename Tr::R2;
   constexpr int NBUF = PcmTraits<PcmT>::NBUF;
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  double* s_win = reinterpret_cast<double*>(smem_raw);                 // 512
-  double2* s_tw256 = reinterpret_cast<double2*>(s_win + 512);          // 256, [p][r]
-  double2* s_w512 = s_tw256 + 256;                                     // 256
-  double2* s_logtab_all = s_w512 + 256;                                // LOGTAB * LOGCOPIES
-  double* s_xr = reinterpret_cast<double*>(s_logtab_all + LOGTAB * LOGCOPIES);   // FT * XF
-  double* s_xi = s_xr + FT * XF;                                       // FT * XF
-  double* s_red = s_xi + FT * XF;                                      // 3 * 8
+  R* s_win = reinterpret_cast<R*>(smem_raw);                           // 512
+  R2* s_tw256 = reinterpret_cast<R2*>(s_win + 512);                    // 256, [p][r]
+  R2* s_w512 = s_tw256 + 256;                                          // 256
+  double2* s_logtab_all = reinterpret_cast<double2*>(s_w512 + 256);    // Tr::LOGTAB_N
+  R* s_xr = reinterpret_cast<R*>(s_logtab_all + Tr::LOGTAB_N);         // FT * XF
+  R* s_xi = s_xr + FT * XF;                                            // FT * XF
+  double* s_red = reinterpret_cast<double*>(s_xi + FT * XF);           // 3 * 8
   unsigned long long* s_bar = reinterpret_cast<unsigned long long*>(s_red + 24);   // 2
   PcmT* s_pcm = reinterpret_cast<PcmT*>(s_bar + 2);                    // NBUF * (FT+1)*256, 16 B aligned
   constexpr int PCM_BUF = (FT + 1) * AFP_N_HOP;
+  const PcmT* pcm = reinterpret_cast<const PcmT*>(a.pcm);
 
   const int tid = threadIdx.x;
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(s_bar)));
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(s_bar + 1)));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
+  if (tid == 0) mbar_init<2>(s_bar);
   for (int i = tid; i < 512; i += K1_THREADS) s_win[i] = a.window[i];
   for (int i = tid; i < 256; i += K1_THREADS) {
     s_tw256[i] = a.tw256[i];
     s_w512[i] = a.w512[i];
   }
-  for (int i = tid; i < LOGTAB * LOGCOPIES; i += K1_THREADS) s_logtab_all[i] = a.logtab[i];
+  if constexpr (Tr::LOGTAB_N > 0)
+    for (int i = tid; i < Tr::LOGTAB_N; i += K1_THREADS) s_logtab_all[i] = a.logtab[i];
   __syncthreads();
 
   const int g = tid >> 4;   // frame within the tile
@@ -239,48 +288,48 @@ __global__ void __launch_bounds__(K1_THREADS, 2) afp_stft_kernel(StftArgs a) {
   const int G = gridDim.x;
   // Tile descriptors are fetched two tiles ahead so that their (dependent) global
   // loads never sit on the critical path: item index at distance 3, ItemDesc at 2.
-  TileInfo cur = make_tile<PcmT>(a, a.items[a.tile_item[tile]], tile);
+  TileInfo cur = make_tile(pcm, a.items[a.tile_item[tile]], tile);
   TileInfo nxt = cur;
-  if (tile + G < a.tile_end) nxt = make_tile<PcmT>(a, a.items[a.tile_item[tile + G]], tile + G);
+  if (tile + G < a.tile_end) nxt = make_tile(pcm, a.items[a.tile_item[tile + G]], tile + G);
   int item_nn = (tile + 2 * G < a.tile_end) ? a.tile_item[tile + 2 * G] : 0;
-  stage_tile<PcmT>(a, cur, s_pcm, s_bar);
+  stage_tile(pcm, cur, s_pcm, s_bar);
   int buf = 0;
 
   for (; tile < a.tile_end; tile += G) {
     const int next = tile + G;
     // prefetch the next tile into the other buffer (free since the end-of-iteration barrier)
-    if (NBUF == 2 && next < a.tile_end) stage_tile<PcmT>(a, nxt, s_pcm + (buf ^ 1) * PCM_BUF, s_bar + (buf ^ 1));
+    if (NBUF == 2 && next < a.tile_end) stage_tile(pcm, nxt, s_pcm + (buf ^ 1) * PCM_BUF, s_bar + (buf ^ 1));
     ItemDesc desc_nn = a.items[item_nn];                                   // consumed at the end of the iteration
     const int item_n3 = (tile + 3 * G < a.tile_end) ? a.tile_item[tile + 3 * G] : 0;   // consumed next iteration
     if (cur.tma & 0xffff) {
-      wait_bar(s_bar + buf, (phases >> buf) & 1u);
+      mbar_wait(s_bar + buf, (phases >> buf) & 1u);
       phases ^= 1u << buf;
     }
     if ((cur.tma & 0xffff) != (cur.nft + 1) * AFP_N_HOP) __syncthreads();   // scalar-staged samples are visible
 
     const bool active = g < cur.nft;
     const int64_t frame = cur.frame0 + g;
-    double vmax = 0.0, vsum = 0.0;
-    int hmin = 0x7ff00000;   // min over the high words of 4|X|^2 (positive doubles order like their bits)
-    double zr[16], zi[16];
+    R vmax = 0, vsum = 0;
+    int hmin = Tr::HMIN_NONE;   // min of hbits(4|X|^2)
+    R zr[16], zi[16];
     if (active) {
       // step A: z[16q + r] = (x[2n] w[2n], x[2n+1] w[2n+1]), n = 16q + r
       const PcmT* fr = s_pcm + buf * PCM_BUF + g * AFP_N_HOP;
 #pragma unroll
       for (int q = 0; q < 16; ++q) {
         const int i0 = 2 * (16 * q + r);
-        const double2 w = *reinterpret_cast<const double2*>(s_win + i0);
-        double x0, x1;
-        PcmTraits<PcmT>::load2(fr + i0, x0, x1);
+        const R2 w = *reinterpret_cast<const R2*>(s_win + i0);
+        R x0, x1;
+        Tr::load2(fr + i0, x0, x1);
         zr[q] = x0 * w.x;
         zi[q] = x1 * w.y;
       }
       afp_fft16(zr, zi);
-      double* xr = s_xr + g * XF;
-      double* xi = s_xi + g * XF;
+      R* xr = s_xr + g * XF;
+      R* xi = s_xi + g * XF;
 #pragma unroll
       for (int p = 0; p < 16; ++p) {
-        const double2 w = s_tw256[p * 16 + r];
+        const R2 w = s_tw256[p * 16 + r];
         xr[p * XS + r] = zr[p] * w.x - zi[p] * w.y;
         xi[p * XS + r] = zr[p] * w.y + zi[p] * w.x;
       }
@@ -288,8 +337,8 @@ __global__ void __launch_bounds__(K1_THREADS, 2) afp_stft_kernel(StftArgs a) {
     __syncwarp();
     if (active) {
       // step B: thread p = r transforms column p: Z[p + 16 s]
-      const double* xr = s_xr + g * XF + r * XS;
-      const double* xi = s_xi + g * XF + r * XS;
+      const R* xr = s_xr + g * XF + r * XS;
+      const R* xi = s_xi + g * XF + r * XS;
 #pragma unroll
       for (int q = 0; q < 16; ++q) {
         zr[q] = xr[q];
@@ -302,71 +351,62 @@ __global__ void __launch_bounds__(K1_THREADS, 2) afp_stft_kernel(StftArgs a) {
     //   2Xe = Z[k] + conj(Zp), 2Xo = -i (Z[k] - conj(Zp)), P = W512^k * 2Xo
     //   4|X[k]|^2 = |2Xe + P|^2,  4|X[256-k]|^2 = |2Xe - P|^2
     {
-      double* out = a.logs + frame * AFP_NBINS;
+      R* out = a.logs + frame * AFP_NBINS;
 #pragma unroll
       for (int s = 0; s < 8; ++s) {
-        double c = __shfl_sync(0xffffffffu, zr[15 - s], src_lane);
-        double d = __shfl_sync(0xffffffffu, zi[15 - s], src_lane);
+        R c = __shfl_sync(0xffffffffu, zr[15 - s], src_lane);
+        R d = __shfl_sync(0xffffffffu, zi[15 - s], src_lane);
         if (r == 0) {
           c = zr[(16 - s) & 15];
           d = zi[(16 - s) & 15];
         }
         if (active) {
           const int k = r + 16 * s;
-          const double2 w = s_w512[k];
-          const double er = zr[s] + c, ei = zi[s] - d, orr = zi[s] + d, oi = c - zr[s];
-          const double pr = w.x * orr - w.y * oi, pi = w.x * oi + w.y * orr;
-          const double ar = er + pr, ai = ei + pi, br = er - pr, bi = ei - pi;
-          const double ssa = ar * ar + ai * ai;   // 4 |X[k]|^2
-          const double ssb = br * br + bi * bi;   // 4 |X[256-k]|^2
-          double la = half_log_quarter(ssa, s_logtab);
-          double lb = half_log_quarter(ssb, s_logtab);
-          if (is_special(ssa) || is_special(ssb)) {   // digital silence etc.: rare, off the hot path
-            la = half_log_quarter_slow(ssa);
-            lb = half_log_quarter_slow(ssb);
-          }
+          const R2 w = s_w512[k];
+          const R er = zr[s] + c, ei = zi[s] - d, orr = zi[s] + d, oi = c - zr[s];
+          const R pr = w.x * orr - w.y * oi, pi = w.x * oi + w.y * orr;
+          const R ar = er + pr, ai = ei + pi, br = er - pr, bi = ei - pi;
+          const R ssa = ar * ar + ai * ai;   // 4 |X[k]|^2
+          const R ssb = br * br + bi * bi;   // 4 |X[256-k]|^2
+          R la, lb;
+          Tr::log_pair(ssa, ssb, s_logtab, la, lb);
           out[k] = la;
           if (k != 0) out[256 - k] = lb; else a.nyq[frame] = lb;   // k == 0 pairs with the Nyquist bin
           if (WRITE_MAG) {
-            a.mag[frame * 257 + k] = sqrt(0.25 * ssa);
-            a.mag[frame * 257 + 256 - k] = sqrt(0.25 * ssb);
+            a.mag[frame * 257 + k] = sqrt(R(0.25) * ssa);
+            a.mag[frame * 257 + 256 - k] = sqrt(R(0.25) * ssb);
           }
           vmax = fmax(vmax, fmax(ssa, ssb));
-          hmin = min(hmin, min(__double2hiint(ssa), __double2hiint(ssb)));
+          hmin = min(hmin, min(Tr::hbits(ssa), Tr::hbits(ssb)));
           vsum += la + lb;
         }
       }
       if (active && r == 0) {   // bin 128 pairs with itself
-        const double2 w = s_w512[128];
-        const double er = 2.0 * zr[8], orr = 2.0 * zi[8];   // ei = 0, oi = 0
-        const double ar = er + w.x * orr, ai = w.y * orr;
-        const double ss = ar * ar + ai * ai;
-        double lg = half_log_quarter(ss, s_logtab);
-        if (is_special(ss)) lg = half_log_quarter_slow(ss);
+        const R2 w = s_w512[128];
+        const R er = R(2) * zr[8], orr = R(2) * zi[8];   // ei = 0, oi = 0
+        const R ar = er + w.x * orr, ai = w.y * orr;
+        const R ss = ar * ar + ai * ai;
+        const R lg = Tr::log1(ss, s_logtab);
         out[128] = lg;
-        if (WRITE_MAG) a.mag[frame * 257 + 128] = sqrt(0.25 * ss);
+        if (WRITE_MAG) a.mag[frame * 257 + 128] = sqrt(R(0.25) * ss);
         vmax = fmax(vmax, ss);
-        hmin = min(hmin, __double2hiint(ss));
+        hmin = min(hmin, Tr::hbits(ss));
         vsum += lg;
       }
     }
-    // deterministic CTA reduction of (max |S|^2, min log, sum log)
-    // a LOWER bound of the smallest log: the high word alone (low word zeroed).  The
-    // statistics pass only asks "is anything below the floor?"; a false alarm just takes its
-    // exact path.
+    // deterministic CTA reduction of (max |S|^2, min log, sum log), in FP64 for both precisions
     hmin = __reduce_min_sync(0xffffffffu, hmin);
-    const double v_lo = __hiloint2double(hmin, 0);
-    double vmin = hmin >= 0x7ff00000 ? INFINITY      // this warp had no frame in the tile
-                  : (hmin < 0x00100000 ? -INFINITY : half_log_quarter(v_lo, s_logtab));
+    const double vmin = Tr::log_lower_bound(hmin, s_logtab);   // +inf: this warp had no frame in the tile
+    double dmax = vmax, dsum = vsum;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
-      vmax = fmax(vmax, __shfl_xor_sync(0xffffffffu, vmax, o));
-      vsum += __shfl_xor_sync(0xffffffffu, vsum, o);
+      dmax = fmax(dmax, __shfl_xor_sync(0xffffffffu, dmax, o));
+      dsum += __shfl_xor_sync(0xffffffffu, dsum, o);
     }
     if (lane == 0) {
-      s_red[(tid >> 5) * 3 + 0] = vmax;
+      s_red[(tid >> 5) * 3 + 0] = dmax;
       s_red[(tid >> 5) * 3 + 1] = vmin;
-      s_red[(tid >> 5) * 3 + 2] = vsum;
+      s_red[(tid >> 5) * 3 + 2] = dsum;
     }
     __syncthreads();   // also: every thread is done with s_pcm[buf]
     if (tid == 0) {
@@ -383,201 +423,10 @@ __global__ void __launch_bounds__(K1_THREADS, 2) afp_stft_kernel(StftArgs a) {
     }
     if (NBUF == 2) buf ^= 1;
     cur = nxt;
-    if (tile + 2 * G < a.tile_end) nxt = make_tile<PcmT>(a, desc_nn, tile + 2 * G);
+    if (tile + 2 * G < a.tile_end) nxt = make_tile(pcm, desc_nn, tile + 2 * G);
     item_nn = item_n3;
-    if (NBUF == 1 && next < a.tile_end) stage_tile<PcmT>(a, cur, s_pcm, s_bar);
+    if (NBUF == 1 && next < a.tile_end) stage_tile(pcm, cur, s_pcm, s_bar);
   }
-}
-
-
-// ---- FP32 variant of K1 (Analyzer.precision = 'fp32') -----------------------------------
-// Same decomposition, single precision throughout (FFT, |.|^2, log via MUFU), float
-// log-spectrogram out: half the output bytes, twice the FP32 lane rate, ~80 registers ->
-// three CTAs per SM.  Downstream decisions then see values that differ from the reference's
-// by ~1e-7 relative, so hashes are NOT guaranteed bit-identical (measured in bench.py).
-template <typename PcmT> struct PcmF32;
-template <> struct PcmF32<int16_t> {
-  __device__ static __forceinline__ void load2(const int16_t* p, float& a, float& b) {
-    const uint32_t w = *reinterpret_cast<const uint32_t*>(p);
-    a = (float)(short)(w & 0xffffu);
-    b = (float)((int)w >> 16);
-  }
-};
-template <> struct PcmF32<float> {
-  __device__ static __forceinline__ void load2(const float* p, float& a, float& b) {
-    const float2 w = *reinterpret_cast<const float2*>(p);
-    a = w.x;
-    b = w.y;
-  }
-};
-
-template <typename PcmT, bool WRITE_MAG>
-__global__ void __launch_bounds__(K1_THREADS, 3) afp_stft_f32_kernel(StftArgs a) {
-  constexpr int NBUF = PcmTraits<PcmT>::NBUF;
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  float* s_win = reinterpret_cast<float*>(smem_raw);                   // 512
-  float2* s_tw256 = reinterpret_cast<float2*>(s_win + 512);            // 256, [p][r]
-  float2* s_w512 = s_tw256 + 256;                                      // 256
-  float* s_xr = reinterpret_cast<float*>(s_w512 + 256);                // FT * XF
-  float* s_xi = s_xr + FT * XF;                                        // FT * XF
-  double* s_red = reinterpret_cast<double*>(s_xi + FT * XF);           // 3 * 8
-  unsigned long long* s_bar = reinterpret_cast<unsigned long long*>(s_red + 24);   // 2
-  PcmT* s_pcm = reinterpret_cast<PcmT*>(s_bar + 2);                    // NBUF * (FT+1)*256
-  constexpr int PCM_BUF = (FT + 1) * AFP_N_HOP;
-
-  const int tid = threadIdx.x;
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(s_bar)));
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(s_bar + 1)));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  for (int i = tid; i < 512; i += K1_THREADS) s_win[i] = a.window_f[i];
-  for (int i = tid; i < 256; i += K1_THREADS) {
-    s_tw256[i] = a.tw256_f[i];
-    s_w512[i] = a.w512_f[i];
-  }
-  __syncthreads();
-
-  const int g = tid >> 4, r = tid & 15, lane = tid & 31;
-  const int src_lane = (lane & 16) | ((16 - r) & 15);
-  uint32_t phases = 0u;
-
-  int tile = a.tile_begin + blockIdx.x;
-  if (tile >= a.tile_end) return;
-  const int G = gridDim.x;
-  TileInfo cur = make_tile<PcmT>(a, a.items[a.tile_item[tile]], tile);
-  TileInfo nxt = cur;
-  if (tile + G < a.tile_end) nxt = make_tile<PcmT>(a, a.items[a.tile_item[tile + G]], tile + G);
-  int item_nn = (tile + 2 * G < a.tile_end) ? a.tile_item[tile + 2 * G] : 0;
-  stage_tile<PcmT>(a, cur, s_pcm, s_bar);
-  int buf = 0;
-
-  for (; tile < a.tile_end; tile += G) {
-    const int next = tile + G;
-    if (NBUF == 2 && next < a.tile_end) stage_tile<PcmT>(a, nxt, s_pcm + (buf ^ 1) * PCM_BUF, s_bar + (buf ^ 1));
-    ItemDesc desc_nn = a.items[item_nn];
-    const int item_n3 = (tile + 3 * G < a.tile_end) ? a.tile_item[tile + 3 * G] : 0;
-    if (cur.tma & 0xffff) {
-      wait_bar(s_bar + buf, (phases >> buf) & 1u);
-      phases ^= 1u << buf;
-    }
-    if ((cur.tma & 0xffff) != (cur.nft + 1) * AFP_N_HOP) __syncthreads();
-    const bool active = g < cur.nft;
-    const int64_t frame = cur.frame0 + g;
-    float vmax = 0.0f, vsum = 0.0f;
-    int hmin = 0x7f800000;
-    float zr[16], zi[16];
-    if (active) {
-      const PcmT* fr = s_pcm + buf * PCM_BUF + g * AFP_N_HOP;
-#pragma unroll
-      for (int q = 0; q < 16; ++q) {
-        const int i0 = 2 * (16 * q + r);
-        const float2 w = *reinterpret_cast<const float2*>(s_win + i0);
-        float x0, x1;
-        PcmF32<PcmT>::load2(fr + i0, x0, x1);
-        zr[q] = x0 * w.x;
-        zi[q] = x1 * w.y;
-      }
-      afp_fft16(zr, zi);
-      float* xr = s_xr + g * XF;
-      float* xi = s_xi + g * XF;
-#pragma unroll
-      for (int p = 0; p < 16; ++p) {
-        const float2 w = s_tw256[p * 16 + r];
-        xr[p * XS + r] = zr[p] * w.x - zi[p] * w.y;
-        xi[p * XS + r] = zr[p] * w.y + zi[p] * w.x;
-      }
-    }
-    __syncwarp();
-    if (active) {
-      const float* xr = s_xr + g * XF + r * XS;
-      const float* xi = s_xi + g * XF + r * XS;
-#pragma unroll
-      for (int q = 0; q < 16; ++q) {
-        zr[q] = xr[q];
-        zi[q] = xi[q];
-      }
-      afp_fft16(zr, zi);
-    }
-    {
-      float* out = a.logs_f + frame * AFP_NBINS;
-#pragma unroll
-      for (int s = 0; s < 8; ++s) {
-        float c = __shfl_sync(0xffffffffu, zr[15 - s], src_lane);
-        float d = __shfl_sync(0xffffffffu, zi[15 - s], src_lane);
-        if (r == 0) {
-          c = zr[(16 - s) & 15];
-          d = zi[(16 - s) & 15];
-        }
-        if (active) {
-          const int k = r + 16 * s;
-          const float2 w = s_w512[k];
-          const float er = zr[s] + c, ei = zi[s] - d, orr = zi[s] + d, oi = c - zr[s];
-          const float pr = w.x * orr - w.y * oi, pi = w.x * oi + w.y * orr;
-          const float ar = er + pr, ai = ei + pi, br = er - pr, bi = ei - pi;
-          const float ssa = ar * ar + ai * ai, ssb = br * br + bi * bi;     // 4|X|^2
-          const float la = 0.5f * __logf(0.25f * ssa), lb = 0.5f * __logf(0.25f * ssb);
-          out[k] = la;
-          if (k != 0) out[256 - k] = lb; else a.nyq[frame] = (double)lb;
-          if (WRITE_MAG) {
-            a.mag[frame * 257 + k] = (double)sqrtf(0.25f * ssa);
-            a.mag[frame * 257 + 256 - k] = (double)sqrtf(0.25f * ssb);
-          }
-          vmax = fmaxf(vmax, fmaxf(ssa, ssb));
-          hmin = min(hmin, min(__float_as_int(ssa), __float_as_int(ssb)));
-          vsum += la + lb;
-        }
-      }
-      if (active && r == 0) {
-        const float2 w = s_w512[128];
-        const float er = 2.0f * zr[8], orr = 2.0f * zi[8];
-        const float ar = er + w.x * orr, ai = w.y * orr;
-        const float ss = ar * ar + ai * ai;
-        const float lg = 0.5f * __logf(0.25f * ss);
-        out[128] = lg;
-        if (WRITE_MAG) a.mag[frame * 257 + 128] = (double)sqrtf(0.25f * ss);
-        vmax = fmaxf(vmax, ss);
-        hmin = min(hmin, __float_as_int(ss));
-        vsum += lg;
-      }
-    }
-    hmin = __reduce_min_sync(0xffffffffu, hmin);
-    double vmin = hmin >= 0x7f800000 ? INFINITY
-                  : (hmin < 0x00800000 ? -INFINITY : (double)(0.5f * __logf(0.25f * __int_as_float(hmin))) - 1e-6);
-    double dmax = (double)vmax, dsum = (double)vsum;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      dmax = fmax(dmax, __shfl_xor_sync(0xffffffffu, dmax, o));
-      dsum += __shfl_xor_sync(0xffffffffu, dsum, o);
-    }
-    if (lane == 0) {
-      s_red[(tid >> 5) * 3 + 0] = dmax;
-      s_red[(tid >> 5) * 3 + 1] = vmin;
-      s_red[(tid >> 5) * 3 + 2] = dsum;
-    }
-    __syncthreads();
-    if (tid == 0) {
-      double m = 0.0, mn = INFINITY, sm = 0.0;
-#pragma unroll
-      for (int w = 0; w < K1_THREADS / 32; ++w) {
-        m = fmax(m, s_red[w * 3 + 0]);
-        mn = fmin(mn, s_red[w * 3 + 1]);
-        sm += s_red[w * 3 + 2];
-      }
-      a.tile_stats[(size_t)tile * 3 + 0] = 0.25 * m;
-      a.tile_stats[(size_t)tile * 3 + 1] = mn;
-      a.tile_stats[(size_t)tile * 3 + 2] = sm;
-    }
-    if (NBUF == 2) buf ^= 1;
-    cur = nxt;
-    if (tile + 2 * G < a.tile_end) nxt = make_tile<PcmT>(a, desc_nn, tile + 2 * G);
-    item_nn = item_n3;
-    if (NBUF == 1 && next < a.tile_end) stage_tile<PcmT>(a, cur, s_pcm, s_bar);
-  }
-}
-
-constexpr size_t k1_f32_smem_bytes(size_t pcm_elem, int nbuf) {
-  return 512 * 4 + 256 * 8 * 2 + 2 * FT * XF * 4 + 24 * 8 + 16 + nbuf * (FT + 1) * 256 * pcm_elem;
 }
 
 // tile -> item table (one thread per item)
@@ -587,11 +436,6 @@ __global__ void afp_tile_table_kernel(const ItemDesc* items, int nitems, int32_t
   const ItemDesc it = items[i];
   const int nt = (it.nframes + FT - 1) / FT;
   for (int k = 0; k < nt; ++k) tile_item[it.tile_base + k] = i;
-}
-
-constexpr size_t k1_smem_bytes(size_t pcm_elem, int nbuf) {
-  return 512 * 8 + 256 * 16 * 2 + LOGTAB * LOGCOPIES * 16 + 2 * FT * XF * 8 + 24 * 8 + 16 +
-         nbuf * (FT + 1) * 256 * pcm_elem;
 }
 
 // ---- per-item statistics: floor, mean (audfprint_analyze.py:283-286) ----------
@@ -697,58 +541,55 @@ int afp_launch_tile_table(afp_ctx* c) {
   return AFP_OK;
 }
 
-int afp_launch_stft(afp_ctx* c, const void* pcm, int dtype, double* mag_out, int64_t tile0, int64_t ntiles) {
-  if (ntiles <= 0) return AFP_OK;
-  StftArgs a;
+namespace {
+
+// One K1 instantiation: num_sms x its CTAs per SM, at most one CTA per tile.
+template <typename R, typename PcmT, bool WRITE_MAG>
+cudaError_t launch_k1(const StftArgs<R>& a, int num_sms, int64_t ntiles, cudaStream_t stream) {
+  constexpr size_t smem = k1_smem_bytes<R, PcmT>();
+  const int nctas = (int)std::min<int64_t>(ntiles, (int64_t)num_sms * K1Traits<R>::MIN_CTAS);
+  const cudaError_t e =
+      cudaFuncSetAttribute(afp_stft_kernel<R, PcmT, WRITE_MAG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e == cudaSuccess) afp_stft_kernel<R, PcmT, WRITE_MAG><<<nctas, K1_THREADS, smem, stream>>>(a);
+  return e;
+}
+
+// window: 2 x 512 (the second pre-scaled by 2^-15 for int16 PCM); twid: tw256, then W512
+template <typename R>
+cudaError_t launch_stft(afp_ctx* c, const DevBuf& window, const DevBuf& twid, const void* pcm, int dtype,
+                        double* mag_out, int64_t tile0, int64_t ntiles) {
+  using R2 = typename K1Traits<R>::R2;
+  StftArgs<R> a;
   a.pcm = pcm;
   a.items = c->d_items.as<ItemDesc>();
   a.tile_item = c->d_tile_item.as<int32_t>();
   a.nitems = c->nitems;
   a.tile_begin = (int)tile0;
   a.tile_end = (int)(tile0 + ntiles);
-  a.window = c->d_window.as<double>() + (dtype == AFP_PCM_I16 ? AFP_N_FFT : 0);
-  a.tw256 = c->d_twid.as<double2>();
-  a.w512 = c->d_twid.as<double2>() + 256;
+  a.window = window.as<R>() + (dtype == AFP_PCM_I16 ? AFP_N_FFT : 0);
+  a.tw256 = twid.as<R2>();
+  a.w512 = twid.as<R2>() + 256;
   a.logtab = c->d_twid.as<double2>() + 512;
-  a.logs = c->d_logs.as<double>();
+  a.logs = c->d_logs.as<R>();
   a.nyq = c->d_nyq.as<double>();
   a.tile_stats = c->d_tile_stats.as<double>();
   a.mag = mag_out;
-  a.window_f = c->d_window_f.as<float>() + (dtype == AFP_PCM_I16 ? AFP_N_FFT : 0);
-  a.tw256_f = c->d_twid_f.as<float2>();
-  a.w512_f = c->d_twid_f.as<float2>() + 256;
-  a.logs_f = c->d_logs.as<float>();
-  const bool f32 = c->ap.spectrogram_fp32 != 0;
-  const int nctas = (int)std::min<int64_t>(ntiles, (int64_t)c->num_sms * (f32 ? 3 : 2));
-  const dim3 grid((unsigned)nctas), block(K1_THREADS);
-  cudaError_t e;
-#define LAUNCH_F32(T, M)                                                                              \
-  do {                                                                                                \
-    const size_t smem = k1_f32_smem_bytes(sizeof(T), PcmTraits<T>::NBUF);                             \
-    e = cudaFuncSetAttribute(afp_stft_f32_kernel<T, M>, cudaFuncAttributeMaxDynamicSharedMemorySize,  \
-                             (int)smem);                                                              \
-    if (e == cudaSuccess) afp_stft_f32_kernel<T, M><<<grid, block, smem, c->stream>>>(a);             \
-  } while (0)
-#define LAUNCH(T, M)                                                                              \
-  do {                                                                                            \
-    const size_t smem = k1_smem_bytes(sizeof(T), PcmTraits<T>::NBUF);                             \
-    e = cudaFuncSetAttribute(afp_stft_kernel<T, M>, cudaFuncAttributeMaxDynamicSharedMemorySize,  \
-                             (int)smem);                                                          \
-    if (e == cudaSuccess) afp_stft_kernel<T, M><<<grid, block, smem, c->stream>>>(a);             \
-  } while (0)
-  if (f32) {
-    if (dtype == AFP_PCM_I16) {
-      if (mag_out) LAUNCH_F32(int16_t, true); else LAUNCH_F32(int16_t, false);
-    } else {
-      if (mag_out) LAUNCH_F32(float, true); else LAUNCH_F32(float, false);
-    }
-  } else if (dtype == AFP_PCM_I16) {
-    if (mag_out) LAUNCH(int16_t, true); else LAUNCH(int16_t, false);
-  } else {
-    if (mag_out) LAUNCH(float, true); else LAUNCH(float, false);
-  }
-#undef LAUNCH
-#undef LAUNCH_F32
+  const int n = c->num_sms;
+  if (dtype == AFP_PCM_I16)
+    return mag_out ? launch_k1<R, int16_t, true>(a, n, ntiles, c->stream)
+                   : launch_k1<R, int16_t, false>(a, n, ntiles, c->stream);
+  return mag_out ? launch_k1<R, float, true>(a, n, ntiles, c->stream)
+                 : launch_k1<R, float, false>(a, n, ntiles, c->stream);
+}
+
+}  // namespace
+
+int afp_launch_stft(afp_ctx* c, const void* pcm, int dtype, double* mag_out, int64_t tile0, int64_t ntiles) {
+  if (ntiles <= 0) return AFP_OK;
+  const cudaError_t e =
+      c->ap.spectrogram_fp32
+          ? launch_stft<float>(c, c->d_window_f, c->d_twid_f, pcm, dtype, mag_out, tile0, ntiles)
+          : launch_stft<double>(c, c->d_window, c->d_twid, pcm, dtype, mag_out, tile0, ntiles);
   AFP_CUDA(c, e);
   AFP_CUDA(c, cudaGetLastError());
   c->launches++;
