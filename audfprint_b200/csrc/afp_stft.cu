@@ -66,6 +66,12 @@ __device__ __forceinline__ bool is_special(double v) {
   return (unsigned)(__double2hiint(v) - 0x00100000) >= 0x7fe00000u;
 }
 
+// The coefficients of 0.5*log1p(r) and ln2/2.  They live in constant memory so that the DFMAs
+// take them as c[][] operands: as literals, every one without a zero low word is rebuilt in
+// registers at each of the nine inlined log call sites.
+__constant__ double k1_log_c64[8] = {0.5 / 7.0, -0.5 / 6.0, 0.5 / 5.0, -0.5 / 4.0,
+                                     0.5 / 3.0, -0.5 / 2.0, 0.5,       0.34657359027997264};
+
 // s_logtab_lane = table base + (lane & 7): this lane's private copy (stride LOGCOPIES).
 __device__ __forceinline__ double half_log_quarter(double v, const double2* s_logtab_lane) {
   const int hi = __double2hiint(v);
@@ -73,15 +79,15 @@ __device__ __forceinline__ double half_log_quarter(double v, const double2* s_lo
   const double m = __hiloint2double((hi & 0x000fffff) | 0x3ff00000, lo);
   const double2 ct = s_logtab_lane[((hi >> 14) & (LOGTAB - 1)) * LOGCOPIES];
   const double r = fma(m, ct.x, -1.0);
-  double p = 0.5 / 7.0;
-  p = fma(p, r, -0.5 / 6.0);
-  p = fma(p, r, 0.5 / 5.0);
-  p = fma(p, r, -0.5 / 4.0);
-  p = fma(p, r, 0.5 / 3.0);
-  p = fma(p, r, -0.5 / 2.0);
-  p = fma(p, r, 0.5);
+  double p = k1_log_c64[0];
+  p = fma(p, r, k1_log_c64[1]);
+  p = fma(p, r, k1_log_c64[2]);
+  p = fma(p, r, k1_log_c64[3]);
+  p = fma(p, r, k1_log_c64[4]);
+  p = fma(p, r, k1_log_c64[5]);
+  p = fma(p, r, k1_log_c64[6]);
   const double ed = int_to_double((hi >> 20) - 1025);
-  return fma(ed, 0.34657359027997264, ct.y) + p * r;   // ln2/2
+  return fma(ed, k1_log_c64[7], ct.y) + p * r;   // ln2/2
 }
 
 template <typename PcmT> struct PcmTraits;
