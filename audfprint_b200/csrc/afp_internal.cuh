@@ -172,7 +172,6 @@ int afp_compact_peaks(afp_ctx* c, int shift);
 int afp_spread_peaks_impl(afp_ctx* c, const double* vector, int32_t n, const double* table, double width,
                           const double* base, double* out);
 int afp_launch_scan_i32_to_i64(afp_ctx* c, const int32_t* in, int64_t* out, int64_t n);
-cudaError_t afp_launch_match_fast(const void* match_args, int nctas, cudaStream_t stream);   // afp_match_fast.cu
 extern "C" int afp_table_stats(afp_ctx* c);
 int afp_finish_match_rows(afp_ctx* c, int nqueries, int row_cap, int64_t* total_out);
 int afp_scan_large(afp_ctx* c, const int32_t* in, int64_t* out, int64_t n);   // afp_store.cu

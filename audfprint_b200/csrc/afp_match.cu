@@ -10,6 +10,9 @@
 // dtime histogram cleared over the touched range); the per-track raw counts are
 // built in shared memory, segment by segment.  Results do not depend on hit
 // order, so hits and records are appended with (shared-memory) atomics.
+// Once the candidates are ranked and their hits routed, the candidate stage
+// (quick filter, dtime histograms, modes) is the fast kernel's, from
+// afp_match_common.cuh.
 //
 // Tie rule (documented deviation, see oracle/afp_oracle.py::rank_candidates):
 // the reference reverses an unstable argsort, so the order of equal weighted
@@ -19,6 +22,31 @@
 #include "afp_match_common.cuh"
 
 namespace {
+
+constexpr int GCAP = 1024;        // radix select stops once the undecided set is this small
+constexpr int QCAP = 16384;       // query rows sorted in shared memory to merge probes of one bucket (128 KB)
+constexpr int CSEG = 32768;       // track ids counted per pass in shared memory (u32 counters, the same 128 KB)
+constexpr int64_t HITS_MAX = (int64_t)1 << 30;   // per-query hit capacity (rows * depth): int indexing
+constexpr int HSET_BITS = 11;     // candidate hash set: 2048 entries for <= KCAP = 1024 keys
+constexpr int HSET = 1 << HSET_BITS;
+
+struct Shared {
+  ModeScratch ms;
+  unsigned long long a_w[KCAP + GCAP];   // gathered keys, sorted descending: the top-K' candidates
+  unsigned a_id[KCAP + GCAP];
+  unsigned a_raw[KCAP];
+  int loff[KCAP];        // start of candidate j's dt list
+  int cur[KCAP];         // fill cursor of candidate j's dt list
+  unsigned char pass[KCAP];
+  int rhist[256];        // radix-select digit histogram
+  int wsum[NW];
+  unsigned long long kw[NW];
+  unsigned kid[NW];
+  unsigned nhits, ndist, nabove, ngather, nrec;
+  int sel_digit, sel_need, sel_m;
+  int segoff[514];       // record range of every id segment (nids < 2^24 -> <= 512 segments)
+  int segcur[512];
+};
 
 // raw count of a selected id from its weight: w = raw / hpi correctly rounded, so
 // rint(w * hpi) == raw exactly (raw < 2^21).  hashesperid == 0 (w = inf) falls back to a scan.
@@ -70,17 +98,9 @@ __global__ void __launch_bounds__(MT) afp_match_kernel(MatchArgs a) {
                               (uint32_t)a.q[2 * (q0 + i)]
                         : ~0ull;
       __syncthreads();
-      for (int k = 2; k <= n2; k <<= 1)          // bitonic sort, ascending (bucket, time)
-        for (int j = k >> 1; j > 0; j >>= 1) {
-          for (int i = tid; i < n2; i += MT) {
-            const int l = i ^ j;
-            if (l > i) {
-              const unsigned long long x = s_q[i], y = s_q[l];
-              if ((x > y) == ((i & k) == 0)) { s_q[i] = y; s_q[l] = x; }
-            }
-          }
-          __syncthreads();
-        }
+      bitonic_sort(                              // ascending (bucket, time)
+          n2, [&](int i, int l, int k) { return (s_q[i] > s_q[l]) == ((i & k) == 0); },
+          [&](int i, int l) { const unsigned long long x = s_q[i]; s_q[i] = s_q[l]; s_q[l] = x; });
     }
     for (int r = warp; r < nq; r += NW) {
       uint32_t b;
@@ -222,7 +242,6 @@ __global__ void __launch_bounds__(MT) afp_match_kernel(MatchArgs a) {
     // candidate depth: min(#ids above threshold, search_depth) (:142-144); a table shard
     // publishes its full local top-search_depth list instead (dist.merge_sharded_results)
     const int maxdepth = a.publish ? min(ndist, a.sdepth) : min(nabove, a.sdepth);
-    int32_t* qrows = a.rows + (size_t)qi * a.row_cap * 7;
 
     if (maxdepth > 0 && maxdepth <= KCAP) {
       // ---- fast path: the top-`maxdepth` distinct ids by (weight desc, id desc) via an
@@ -301,42 +320,24 @@ __global__ void __launch_bounds__(MT) afp_match_kernel(MatchArgs a) {
       while (n2 < ng) n2 <<= 1;
       for (int i = ng + tid; i < n2; i += MT) { sh.a_w[i] = 0ull; sh.a_id[i] = 0u; }
       __syncthreads();
-      for (int k = 2; k <= n2; k <<= 1)          // bitonic sort, descending
-        for (int j = k >> 1; j > 0; j >>= 1) {
-          for (int i = tid; i < n2; i += MT) {
-            const int l = i ^ j;
-            if (l > i) {
-              const bool desc = (i & k) == 0;
-              const bool gt = key_gt(sh.a_w[i], sh.a_id[i], sh.a_w[l], sh.a_id[l]);
-              if (gt != desc) {
-                const unsigned long long tw = sh.a_w[i]; sh.a_w[i] = sh.a_w[l]; sh.a_w[l] = tw;
-                const unsigned ti = sh.a_id[i]; sh.a_id[i] = sh.a_id[l]; sh.a_id[l] = ti;
-              }
-            }
-          }
-          __syncthreads();
-        }
+      bitonic_sort(                              // descending
+          n2, [&](int i, int l, int k) { return key_gt(sh.a_w[i], sh.a_id[i], sh.a_w[l], sh.a_id[l]) != ((i & k) == 0); },
+          [&](int i, int l) {
+            const unsigned long long tw = sh.a_w[i]; sh.a_w[i] = sh.a_w[l]; sh.a_w[l] = tw;
+            const unsigned ti = sh.a_id[i]; sh.a_id[i] = sh.a_id[l]; sh.a_id[l] = ti;
+          });
       const int ncand = maxdepth;               // entries 0..maxdepth-1 of the sorted list, rank = index
+      const CandArrays cands{sh.a_id, sh.a_raw, sh.loff, sh.cur, sh.pass};
       {
-        unsigned raw = 0;
+        unsigned id = 0, raw = 0;
+        unsigned long long wb = 0ull;
         if (tid < ncand) {
-          raw = raw_of(a, sh.a_w[tid], sh.a_id[tid], dlist, rawl, ndist);
+          id = sh.a_id[tid];
+          wb = sh.a_w[tid];
+          raw = raw_of(a, wb, id, dlist, rawl, ndist);
           sh.a_raw[tid] = raw;
-          if (a.publish) {
-            double* c3 = a.cand + ((size_t)qi * a.sdepth + tid) * 3;
-            c3[0] = (double)sh.a_id[tid];
-            c3[1] = (double)raw;
-            c3[2] = __longlong_as_double((long long)sh.a_w[tid]);
-          }
         }
-        const bool rowable = tid < ncand && raw > (uint32_t)a.thresh;   // only these can yield rows (:291)
-        const int lraw = rowable ? (int)raw : 0;
-        const int lend = block_scan_incl(lraw, sh.wsum);
-        if (tid < ncand) {
-          sh.loff[tid] = lend - lraw;
-          sh.cur[tid] = 0;
-          sh.pass[tid] = 0;
-        }
+        const bool rowable = candidates_begin(a, qi, ncand, id, raw, wb, cands, sh.wsum);
         // id -> candidate slot: open-addressing hash set in the (now free) upper halves of the
         // sort arrays, so that routing the hits costs no global access
         unsigned* hkey = reinterpret_cast<unsigned*>(sh.a_w + KCAP);              // HSET entries
@@ -344,8 +345,8 @@ __global__ void __launch_bounds__(MT) afp_match_kernel(MatchArgs a) {
         for (int i = tid; i < HSET; i += MT) hkey[i] = 0u;
         __syncthreads();
         if (rowable) {
-          const unsigned key = sh.a_id[tid] + 1u;
-          unsigned h = (sh.a_id[tid] * 2654435761u) >> (32 - HSET_BITS);
+          const unsigned key = id + 1u;
+          unsigned h = (id * 2654435761u) >> (32 - HSET_BITS);
           while (atomicCAS(&hkey[h], 0u, key) != 0u) h = (h + 1u) & (HSET - 1);
           hval[h] = (unsigned short)tid;
         }
@@ -375,42 +376,7 @@ __global__ void __launch_bounds__(MT) afp_match_kernel(MatchArgs a) {
         }
       }
       __syncthreads();
-      // ---- quick filter, one warp per candidate: a row needs a dtime bin > threshcount (:291)
-      for (int j = warp; j < ncand; j += NW) {
-        const int n = (int)sh.a_raw[j];
-        if (n <= a.thresh) continue;       // warp-uniform
-        const uint32_t* L = dts + sh.loff[j];
-        int best = 0;
-        for (int i = lane; i < n; i += 32) {
-          const uint32_t me = L[i];
-          int c = 0;
-          for (int k = 0; k < n; ++k) c += (L[k] == me) ? 1 : 0;
-          best = max(best, c);
-        }
-        best = __reduce_max_sync(0xffffffffu, best);
-        if (lane == 0) sh.pass[j] = best > a.thresh;
-      }
-      __syncthreads();
-      // ---- full mode search of the surviving candidates, in rank order
-      for (int j = 0; j < ncand; ++j) {
-        if (!sh.pass[j]) continue;          // uniform
-        const int n = (int)sh.a_raw[j];
-        const uint32_t* L = dts + sh.loff[j];
-        if (tid == 0) { sh.dmin = 0x7fffffff; sh.dmax = -1; }
-        __syncthreads();
-        int dmin = 0x7fffffff, dmax = -1;
-        for (int i = tid; i < n; i += MT) {
-          const int d = (int)L[i];
-          atomicAdd(&hist[d], 1);
-          dmin = min(dmin, d);
-          dmax = max(dmax, d);
-        }
-        dmin = __reduce_min_sync(0xffffffffu, dmin);
-        dmax = __reduce_max_sync(0xffffffffu, dmax);
-        if (lane == 0 && dmax >= 0) { atomicMin(&sh.dmin, dmin); atomicMax(&sh.dmax, dmax); }
-        __syncthreads();
-        candidate_modes(a, sh.ms, hist, filt, sh.dmin, sh.dmax, sh.a_id[j], n, j, qrows);
-      }
+      candidates_finish(a, qi, ncand, cands, dts, sh.ms, hist, filt);
     } else if (maxdepth > 0) {
       // ---- slow path (search_depth > KCAP): one pass over the distinct
       // ids and one over the hits per candidate
@@ -448,32 +414,13 @@ __global__ void __launch_bounds__(MT) afp_match_kernel(MatchArgs a) {
           if (tid == 0) { c3[0] = (double)bid; c3[1] = (double)raw; c3[2] = __longlong_as_double((long long)bw); }
         }
         if (raw <= a.thresh) continue;      // cannot yield a row (:291), but keeps its rank
-        if (tid == 0) { sh.dmin = 0x7fffffff; sh.dmax = -1; }
-        __syncthreads();
-        int dmin = 0x7fffffff, dmax = -1;
-        for (int i = tid; i < nhits; i += MT) {
-          const uint2 h = hits[i];
-          if (h.x == bid) {
-            atomicAdd(&hist[h.y], 1);
-            dmin = min(dmin, (int)h.y);
-            dmax = max(dmax, (int)h.y);
-          }
-        }
-        dmin = __reduce_min_sync(0xffffffffu, dmin);
-        dmax = __reduce_max_sync(0xffffffffu, dmax);
-        if (lane == 0 && dmax >= 0) { atomicMin(&sh.dmin, dmin); atomicMax(&sh.dmax, dmax); }
-        __syncthreads();
-        candidate_modes(a, sh.ms, hist, filt, sh.dmin, sh.dmax, bid, raw, rank, qrows);
+        candidate_modes(   // over the whole hit list, filtered by id
+            a, sh.ms, hist, filt, qi, nhits,
+            [&](int i, int& d) { const uint2 h = hits[i]; d = (int)h.y; return h.x == bid; }, bid, raw, rank);
       }
     }
     __syncthreads();
-    if (tid == 0) {
-      a.row_cnt[qi] = sh.ms.nrows;
-      if (a.publish) {
-        a.cand_cnt[2 * qi] = maxdepth;
-        a.cand_cnt[2 * qi + 1] = nabove;
-      }
-    }
+    if (tid == 0) query_done(a, qi, sh.ms.nrows, maxdepth, nabove);
     __syncthreads();
   }
 }
@@ -880,7 +827,7 @@ int afp_match_batch(afp_ctx* c, const int32_t* q_rows, int q_on_host, int32_t nq
     a.qlist = c->d_mqlist.as<int32_t>() + 4;
     a.fstat = a.qlist + nqueries;
     AFP_CUDA(c, cudaMemsetAsync(a.nlist, 0, sizeof(int), c->stream));
-    AFP_CUDA(c, afp_launch_match_fast(&a, nctas, c->stream));
+    AFP_CUDA(c, afp_launch_match_fast(a, nctas, c->stream));
     c->launches++;
     c->match_fast_ran = true;
   }

@@ -1,21 +1,12 @@
 // Pieces shared by the two matching kernels (afp_match.cu: general path, afp_match_fast.cu:
-// fast path): launch geometry, kernel arguments, candidate order, block-wide helpers and the
-// per-candidate time-offset histogram mode search (audfprint_match.py:284-311).
+// fast path): kernel arguments and the fast kernel's launcher, launch geometry, candidate order,
+// block-wide helpers (scan, bitonic sort, arg-max) and the candidate stage that follows the
+// ranking in both kernels - publish and dt-list offsets of the top-K, quick filter, per-candidate
+// dtime histogram and its mode search (audfprint_match.py:284-311), end-of-query counts.  Each
+// kernel finds its ranked candidates and routes their hits to the dt lists in its own way.
 #pragma once
 #include <math.h>
 #include "afp_internal.cuh"
-
-namespace {
-
-constexpr int MT = 1024;          // threads per matching CTA (one CTA per SM, persistent over the queries)
-constexpr int NW = MT / 32;
-constexpr int KCAP = 1024;        // candidate depth handled by the fast path (search_depth <= KCAP)
-constexpr int GCAP = 1024;        // radix select stops once the undecided set is this small
-constexpr int QCAP = 16384;       // query rows sorted in shared memory to merge probes of one bucket (128 KB)
-constexpr int CSEG = 32768;       // track ids counted per pass in shared memory (u32 counters, the same 128 KB)
-constexpr int64_t HITS_MAX = (int64_t)1 << 30;   // per-query hit capacity (rows * depth): int indexing
-constexpr int HSET_BITS = 11;     // candidate hash set: 2048 entries for <= KCAP = 1024 keys
-constexpr int HSET = 1 << HSET_BITS;
 
 struct MatchArgs {
   const int32_t* q;        // [sum nq][2]
@@ -54,6 +45,15 @@ struct MatchArgs {
   int bm_exact;                           // nids <= bitmap bits: the repeat bitmap is indexed by the id itself
 };
 
+// The fast kernel over every query (afp_match_fast.cu); it appends the ones it hands over to a.qlist.
+cudaError_t afp_launch_match_fast(const MatchArgs& a, int nctas, cudaStream_t stream);
+
+namespace {
+
+constexpr int MT = 1024;          // threads per matching CTA (one CTA per SM, persistent over the queries)
+constexpr int NW = MT / 32;
+constexpr int KCAP = 1024;        // candidate depth handled by the fast path (search_depth <= KCAP)
+
 // candidate order: (weighted count desc, id desc); keys are (bits of the positive double, id)
 __device__ __forceinline__ bool key_gt(unsigned long long w1, unsigned i1, unsigned long long w2, unsigned i2) {
   return w1 > w2 || (w1 == w2 && i1 > i2);
@@ -63,25 +63,17 @@ __device__ __forceinline__ bool key_gt(unsigned long long w1, unsigned i1, unsig
 struct ModeScratch {
   int val[NW], idx[NW];
   int nrows;
+  int dmin, dmax;
 };
 
-struct Shared {
-  ModeScratch ms;
-  unsigned long long a_w[KCAP + GCAP];   // gathered keys, sorted descending: the top-K' candidates
-  unsigned a_id[KCAP + GCAP];
-  unsigned a_raw[KCAP];
-  int loff[KCAP];        // start of candidate j's dt list
-  int cur[KCAP];         // fill cursor of candidate j's dt list
-  unsigned char pass[KCAP];
-  int rhist[256];        // radix-select digit histogram
-  int wsum[NW];
-  unsigned long long kw[NW];
-  unsigned kid[NW];
-  unsigned nhits, ndist, nabove, ngather, nrec;
-  int dmin, dmax;
-  int sel_digit, sel_need, sel_m;
-  int segoff[514];       // record range of every id segment (nids < 2^24 -> <= 512 segments)
-  int segcur[512];
+// The ranked candidates of one query in shared memory, index = rank: id, raw count, and the
+// start, fill cursor and quick-filter verdict of each candidate's dt list.
+struct CandArrays {
+  const unsigned* id;
+  const unsigned* raw;
+  int* loff;
+  int* cur;
+  unsigned char* pass;
 };
 
 // 96-bit composite key (weight bits, id), 12 digits of 8 bits from the top
@@ -127,6 +119,20 @@ __device__ __forceinline__ int block_scan_incl(int v, int* wsum) {
   return v + (warp ? wsum[warp - 1] : 0);
 }
 
+// Block-wide bitonic network over n2 entries (a power of two): entries i < l of a stage whose
+// sorted runs are k long are exchanged by swap(i, l) when out_of_order(i, l, k).
+template <class OutOfOrder, class Swap>
+__device__ __forceinline__ void bitonic_sort(int n2, OutOfOrder out_of_order, Swap swap) {
+  for (int k = 2; k <= n2; k <<= 1)
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int i = threadIdx.x; i < n2; i += MT) {
+        const int l = i ^ j;
+        if (l > i && out_of_order(i, l, k)) swap(i, l);
+      }
+      __syncthreads();
+    }
+}
+
 // (value desc, index asc) arg-max over f[lo..hi] == np.argmax (first max)
 __device__ inline void block_argmax(const int32_t* f, int lo, int hi, ModeScratch& sh, int& best_v, int& best_i) {
   const int tid = threadIdx.x;
@@ -150,11 +156,31 @@ __device__ inline void block_argmax(const int32_t* f, int lo, int hi, ModeScratc
     if (sh.val[w] > best_v || (sh.val[w] == best_v && sh.idx[w] < best_i)) { best_v = sh.val[w]; best_i = sh.idx[w]; }
 }
 
-// Histogram-mode search of one candidate (audfprint_match.py:284-311) given lo/hi of its
-// (already filled) dense histogram; emits rows, restores hist to zero.
-__device__ inline void candidate_modes(const MatchArgs& a, ModeScratch& sh, int32_t* hist, int32_t* filt, int lo, int hi,
-                                unsigned id, int raw, int rank, int32_t* qrows) {
+// One candidate of query qi: its dense dtime histogram from n entries - dt(i, d) stores entry i's
+// dtime in d and says whether the entry belongs to the candidate - then the histogram-mode search
+// (audfprint_match.py:284-311).  Emits rows, restores hist to zero.
+template <class Dt>
+__device__ inline void candidate_modes(const MatchArgs& a, ModeScratch& sh, int32_t* hist, int32_t* filt, int qi, int n,
+                                       Dt dt, unsigned id, int raw, int rank) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  if (tid == 0) { sh.dmin = 0x7fffffff; sh.dmax = -1; }
+  __syncthreads();
+  {
+    int dmin = 0x7fffffff, dmax = -1;
+    for (int i = tid; i < n; i += MT) {
+      int d;
+      if (dt(i, d)) {
+        atomicAdd(&hist[d], 1);
+        dmin = min(dmin, d);
+        dmax = max(dmax, d);
+      }
+    }
+    dmin = __reduce_min_sync(0xffffffffu, dmin);
+    dmax = __reduce_max_sync(0xffffffffu, dmax);
+    if (lane == 0 && dmax >= 0) { atomicMin(&sh.dmin, dmin); atomicMax(&sh.dmax, dmax); }
+  }
+  __syncthreads();
+  const int lo = sh.dmin, hi = sh.dmax;
   // keep_local_maxes (:70-75, locmax :51-67); zero-extended ends are equivalent
   for (int i = lo + tid; i <= hi; i += MT) {
     const int v = __ldcg(hist + i), l = __ldcg(hist + i - 1), r = __ldcg(hist + i + 1);
@@ -178,7 +204,7 @@ __device__ inline void candidate_modes(const MatchArgs& a, ModeScratch& sh, int3
       for (int w = 0; w < NW; ++w) count += sh.val[w];
       const int nr = sh.nrows;
       if (nr < a.row_cap) {
-        int32_t* row = qrows + (size_t)nr * 7;
+        int32_t* row = a.rows + ((size_t)qi * a.row_cap + nr) * 7;
         row[0] = (int32_t)id; row[1] = count; row[2] = bi - a.bias; row[3] = raw;
         row[4] = rank; row[5] = 0; row[6] = 0;                      // :300-301
       }
@@ -195,6 +221,67 @@ __device__ inline void candidate_modes(const MatchArgs& a, ModeScratch& sh, int3
   __syncthreads();
   for (int i = lo + tid; i <= hi; i += MT) hist[i] = 0;              // restore the scratch
   __syncthreads();
+}
+
+// Start of the candidate stage: thread `tid` < ncand holds rank tid's (id, raw, weight bits).
+// Publishes the ranked list in shard mode and lays out the dt lists of the candidates that can
+// yield rows (raw > threshcount, :291) back to back; returns whether rank tid is one of them.
+__device__ __forceinline__ bool candidates_begin(const MatchArgs& a, int qi, int ncand, unsigned id, unsigned raw,
+                                                 unsigned long long wb, const CandArrays& c, int* wsum) {
+  const int tid = threadIdx.x;
+  const bool rowable = tid < ncand && raw > (unsigned)a.thresh;
+  const int lraw = rowable ? (int)raw : 0;
+  const int lend = block_scan_incl(lraw, wsum);
+  if (tid < ncand) {
+    if (a.publish) {
+      double* c3 = a.cand + ((size_t)qi * a.sdepth + tid) * 3;
+      c3[0] = (double)id;
+      c3[1] = (double)raw;
+      c3[2] = __longlong_as_double((long long)wb);
+    }
+    c.loff[tid] = lend - lraw;
+    c.cur[tid] = 0;
+    c.pass[tid] = 0;
+  }
+  return rowable;
+}
+
+// End of the candidate stage, once the caller has routed the hits to the dt lists: quick filter,
+// then the full mode search of the surviving candidates in rank order.
+__device__ __forceinline__ void candidates_finish(const MatchArgs& a, int qi, int ncand, const CandArrays& c,
+                                                  const uint32_t* dts, ModeScratch& ms, int32_t* hist, int32_t* filt) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  // quick filter, one warp per candidate: a row needs a dtime bin > threshcount (:291)
+  for (int j = warp; j < ncand; j += NW) {
+    const int n = (int)c.raw[j];
+    if (n <= a.thresh) continue;       // warp-uniform
+    const uint32_t* L = dts + c.loff[j];
+    int best = 0;
+    for (int i = lane; i < n; i += 32) {
+      const uint32_t me = L[i];
+      int cnt = 0;
+      for (int k = 0; k < n; ++k) cnt += (L[k] == me) ? 1 : 0;
+      best = max(best, cnt);
+    }
+    best = __reduce_max_sync(0xffffffffu, best);
+    if (lane == 0) c.pass[j] = best > a.thresh;
+  }
+  __syncthreads();
+  for (int j = 0; j < ncand; ++j) {
+    if (!c.pass[j]) continue;          // uniform
+    const int n = (int)c.raw[j];
+    const uint32_t* L = dts + c.loff[j];
+    candidate_modes(a, ms, hist, filt, qi, n, [&](int i, int& d) { d = (int)L[i]; return true; }, c.id[j], n, j);
+  }
+}
+
+// a query's row count and, in shard mode, its candidate counts (one thread)
+__device__ __forceinline__ void query_done(const MatchArgs& a, int qi, int nrows, int ncand, int nabove) {
+  a.row_cnt[qi] = nrows;
+  if (a.publish) {
+    a.cand_cnt[2 * qi] = ncand;
+    a.cand_cnt[2 * qi + 1] = nabove;
+  }
 }
 
 }  // namespace

@@ -28,8 +28,9 @@
 //     K-th member weight; otherwise pass 3 re-reads only the bucket groups whose multiplicity
 //     could reach that weight, gathers hashesperid for their non-member ids and admits the
 //     few that do outrank the K-th member;
-//   * the hits of the row-capable candidates are routed from the member list and go through the
-//     same quick filter / histogram mode search as in the general kernel.
+//   * the hits of the row-capable candidates are routed from the member list; the candidate stage
+//     around that routing (dt-list offsets, quick filter, histogram mode search) is the general
+//     kernel's, from afp_match_common.cuh.
 // Per probed entry: 4 B read from HBM, 4 B again from L2, one atomicOr, one set lookup.
 #include "afp_match_common.cuh"
 
@@ -81,7 +82,6 @@ struct FastShared {
   int wcount[NW];          // hits in every warp's segment of the member-hit list
   unsigned nmem, nmh, nx, nabove, ndist, mmax, ngath;
   int overflow;
-  int dmin, dmax;
   int cut_bin, cut_above;
 };
 
@@ -304,26 +304,23 @@ __device__ void scan_chunk(const MatchArgs& a, FastShared& fs, unsigned char* sm
   if (PASS == 2 && lane == 0) fs.wcount[warp] = min(wcount, wcap);
 }
 
-// descending bitonic sort of (sw, sid) with sraw carried along; n2 a power of two <= SCAP
-__device__ void rank_sort(unsigned char* smem, int n2) {
+// descending sort of the first n <= SCAP entries of (sw, sid) with sraw carried along: padded
+// with zero keys to a power of two, then a bitonic sort
+__device__ void rank_sort(unsigned char* smem, int n) {
   unsigned* sid = reinterpret_cast<unsigned*>(smem + OFF_SID);
   unsigned* sraw = reinterpret_cast<unsigned*>(smem + OFF_SRAW);
   unsigned long long* sw = reinterpret_cast<unsigned long long*>(smem + OFF_SW);
-  for (int k = 2; k <= n2; k <<= 1)
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int i = threadIdx.x; i < n2; i += MT) {
-        const int l = i ^ j;
-        if (l > i) {
-          const bool desc = (i & k) == 0;
-          if (key_gt(sw[i], sid[i], sw[l], sid[l]) != desc) {
-            const unsigned long long tw = sw[i]; sw[i] = sw[l]; sw[l] = tw;
-            const unsigned ti = sid[i]; sid[i] = sid[l]; sid[l] = ti;
-            const unsigned tr = sraw[i]; sraw[i] = sraw[l]; sraw[l] = tr;
-          }
-        }
-      }
-      __syncthreads();
-    }
+  int n2 = 2;
+  while (n2 < n) n2 <<= 1;
+  for (int i = n + threadIdx.x; i < n2; i += MT) { sid[i] = 0u; sraw[i] = 0u; sw[i] = 0ull; }
+  __syncthreads();
+  bitonic_sort(
+      n2, [&](int i, int l, int k) { return key_gt(sw[i], sid[i], sw[l], sid[l]) != ((i & k) == 0); },
+      [&](int i, int l) {
+        const unsigned long long tw = sw[i]; sw[i] = sw[l]; sw[l] = tw;
+        const unsigned ti = sid[i]; sid[i] = sid[l]; sid[l] = ti;
+        const unsigned tr = sraw[i]; sraw[i] = sraw[l]; sraw[l] = tr;
+      });
 }
 
 __global__ void __launch_bounds__(MT) afp_match_fast_kernel(MatchArgs a) {
@@ -353,7 +350,6 @@ __global__ void __launch_bounds__(MT) afp_match_fast_kernel(MatchArgs a) {
   for (int qi = blockIdx.x; qi < a.nqueries; qi += gridDim.x) {
     const int64_t q0 = a.qoff[qi];
     const int nq = (int)(a.qoff[qi + 1] - q0);
-    int32_t* qrows = a.rows + (size_t)qi * a.row_cap * 7;
     __syncthreads();                               // the previous query is completely done
     if (tid == 0) {
       fs.nmem = 0; fs.nmh = 0; fs.nx = 0; fs.nabove = 0; fs.ndist = 0; fs.mmax = 0; fs.ngath = 0;
@@ -499,11 +495,7 @@ __global__ void __launch_bounds__(MT) afp_match_fast_kernel(MatchArgs a) {
           if (M > SCAP - XCAP) handover = FS_TIES;   // one weight bin holds thousands of members
         }
         if (!handover && K > 0) {
-          int n2 = 2;
-          while (n2 < M) n2 <<= 1;
-          for (int i = M + tid; i < n2; i += MT) { sid[i] = 0u; sraw[i] = 0u; sw[i] = 0ull; }
-          __syncthreads();
-          rank_sort(smem, n2);
+          rank_sort(smem, M);
           // ---- can a single-record id outrank the K-th member?  Its weight is m / hashesperid
           // with m <= min(m_max, threshcount).
           const unsigned long long wk = K <= M ? sw[K - 1] : 0ull;
@@ -521,12 +513,8 @@ __global__ void __launch_bounds__(MT) afp_match_fast_kernel(MatchArgs a) {
             const int X = (int)fs.nx;
             __syncthreads();
             if (!handover && X > 0) {
-              int n3 = 2;
-              while (n3 < M + X) n3 <<= 1;
-              for (int i = M + X + tid; i < n3; i += MT) { sid[i] = 0u; sraw[i] = 0u; sw[i] = 0ull; }
-              __syncthreads();
-              rank_sort(smem, n3);
               M += X;
+              rank_sort(smem, M);
             }
             if (!handover && K > M) handover = FS_INCONSISTENT;   // cannot happen
           }
@@ -534,24 +522,11 @@ __global__ void __launch_bounds__(MT) afp_match_fast_kernel(MatchArgs a) {
       }
       if (!handover && K > 0) {
         // ---- the top-K: publish, dt-list offsets of the row-capable candidates ---------------
-        const int ncand = K;
+        const CandArrays cands{sid, sraw, loff, cur, pass};
         unsigned id = 0, raw = 0;
         unsigned long long wb = 0ull;
-        if (tid < ncand) { id = sid[tid]; raw = sraw[tid]; wb = sw[tid]; }
-        const bool rowable = tid < ncand && raw > (unsigned)a.thresh;      // only these can yield rows (:291)
-        const int lraw = rowable ? (int)raw : 0;
-        const int lend = block_scan_incl(lraw, fs.wsum);   // (barrier: every rank entry is read)
-        if (tid < ncand) {
-          if (a.publish) {
-            double* c3 = a.cand + ((size_t)qi * a.sdepth + tid) * 3;
-            c3[0] = (double)id;
-            c3[1] = (double)raw;
-            c3[2] = __longlong_as_double((long long)wb);
-          }
-          loff[tid] = lend - lraw;
-          cur[tid] = 0;
-          pass[tid] = 0;
-        }
+        if (tid < K) { id = sid[tid]; raw = sraw[tid]; wb = sw[tid]; }
+        const bool rowable = candidates_begin(a, qi, K, id, raw, wb, cands, fs.wsum);
         for (int i = tid; i < MSLOTS; i += MT) map16[i] = 0xffffu;
         __syncthreads();
         if (rowable) map16[set_find(mkeys, id)] = (unsigned short)tid;     // raw > threshcount: a member
@@ -574,42 +549,7 @@ __global__ void __launch_bounds__(MT) afp_match_fast_kernel(MatchArgs a) {
           }
         }
         __syncthreads();
-        // ---- quick filter, one warp per candidate: a row needs a dtime bin > threshcount (:291)
-        for (int j = warp; j < ncand; j += NW) {
-          const int n = (int)sraw[j];
-          if (n <= a.thresh) continue;       // warp-uniform
-          const uint32_t* L = dts + loff[j];
-          int best = 0;
-          for (int i = lane; i < n; i += 32) {
-            const uint32_t me = L[i];
-            int c = 0;
-            for (int k = 0; k < n; ++k) c += (L[k] == me) ? 1 : 0;
-            best = max(best, c);
-          }
-          best = __reduce_max_sync(0xffffffffu, best);
-          if (lane == 0) pass[j] = best > a.thresh;
-        }
-        __syncthreads();
-        // ---- full mode search of the surviving candidates, in rank order --------------------
-        for (int j = 0; j < ncand; ++j) {
-          if (!pass[j]) continue;          // uniform
-          const int n = (int)sraw[j];
-          const uint32_t* L = dts + loff[j];
-          if (tid == 0) { fs.dmin = 0x7fffffff; fs.dmax = -1; }
-          __syncthreads();
-          int dmin = 0x7fffffff, dmax = -1;
-          for (int i = tid; i < n; i += MT) {
-            const int d = (int)L[i];
-            atomicAdd(&hist[d], 1);
-            dmin = min(dmin, d);
-            dmax = max(dmax, d);
-          }
-          dmin = __reduce_min_sync(0xffffffffu, dmin);
-          dmax = __reduce_max_sync(0xffffffffu, dmax);
-          if (lane == 0 && dmax >= 0) { atomicMin(&fs.dmin, dmin); atomicMax(&fs.dmax, dmax); }
-          __syncthreads();
-          candidate_modes(a, fs.ms, hist, filt, fs.dmin, fs.dmax, sid[j], n, j, qrows);
-        }
+        candidates_finish(a, qi, K, cands, dts, fs.ms, hist, filt);
       }
     }
     __syncthreads();
@@ -617,25 +557,15 @@ __global__ void __launch_bounds__(MT) afp_match_fast_kernel(MatchArgs a) {
       int32_t* st = a.fstat + (size_t)qi * 8;
       st[0] = handover; st[1] = (int)fs.nmem; st[2] = (int)fs.nmh; st[3] = (int)fs.nx;
       st[4] = K; st[5] = nabove; st[6] = (int)fs.mmax; st[7] = (int)fs.ndist;
-      if (handover) {
-        a.qlist[atomicAdd(a.nlist, 1)] = qi;       // the general kernel takes this query
-      } else {
-        a.row_cnt[qi] = fs.ms.nrows;
-        if (a.publish) {
-          a.cand_cnt[2 * qi] = K;
-          a.cand_cnt[2 * qi + 1] = nabove;
-        }
-      }
+      if (handover) a.qlist[atomicAdd(a.nlist, 1)] = qi;       // the general kernel takes this query
+      else query_done(a, qi, fs.ms.nrows, K, nabove);
     }
   }
 }
 
 }  // namespace
 
-size_t afp_match_fast_smem() { return FAST_SMEM; }
-
-cudaError_t afp_launch_match_fast(const void* args, int nctas, cudaStream_t stream) {
-  const MatchArgs& a = *static_cast<const MatchArgs*>(args);
+cudaError_t afp_launch_match_fast(const MatchArgs& a, int nctas, cudaStream_t stream) {
   cudaError_t e = cudaFuncSetAttribute(afp_match_fast_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FAST_SMEM);
   if (e != cudaSuccess) return e;
   afp_match_fast_kernel<<<nctas, MT, FAST_SMEM, stream>>>(a);
