@@ -70,6 +70,10 @@ _SIGS = {
     "afp_table_download": (C.c_int, [_P, _P, _P]),
     "afp_mt_randint_replay": (C.c_int, [_P, _P, C.c_int64, _P]),
     "afp_table_restrict_ids": (C.c_int, [_P, C.c_int64, C.c_int64]),
+    "afp_table_remove_ids": (C.c_int, [_P, _I64P, C.c_int64, _I64P]),
+    "afp_table_retrieve_ids": (C.c_int, [_P, _I64P, C.c_int64, _I64P]),
+    "afp_fetch_retrieved": (C.c_int, [_P, _P, C.c_int, _I64P]),
+    "afp_table_pruning_bound": (C.c_int, [_P, C.POINTER(C.c_uint32)]),
     "afp_get_hits": (C.c_int, [_P, _P, C.c_int64, C.c_int, _I64P]),
     "afp_fetch_hits": (C.c_int, [_P, _P, C.c_int]),
     "afp_match_batch": (C.c_int, [_P, _P, C.c_int, C.c_int32, _I64P, C.POINTER(MatcherParams), _I64P]),

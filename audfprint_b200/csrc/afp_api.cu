@@ -77,7 +77,10 @@ void afp_destroy(afp_ctx* c) {
                     &c->d_hit_off, &c->d_hits, &c->d_st_off, &c->d_st_ids, &c->d_st_eval, &c->d_st_seq, &c->d_st_ovf,
                     &c->d_st_cnt, &c->d_st_seg, &c->d_st_heavy, &c->d_st_part, &c->d_st_scan, &c->d_st_obkt,
                     &c->d_st_opos, &c->d_st_oval, &c->d_st_slot, &c->d_st_last, &c->d_mfast, &c->d_mqlist, &c->d_mscratch, &c->d_mrows, &c->d_mrow_cnt,
-                    &c->d_mrow_off, &c->d_mrows_packed, &c->d_mcand, &c->d_mcand_cnt};
+                    &c->d_mrow_off, &c->d_mrows_packed, &c->d_mcand, &c->d_mcand_cnt,
+                    &c->d_ed_ids, &c->d_ed_bits, &c->d_ed_slot, &c->d_ed_cnt, &c->d_ed_off, &c->d_ed_key,
+                    &c->d_ed_key2, &c->d_ed_val, &c->d_ed_val2, &c->d_ed_cub, &c->d_ed_uoff, &c->d_ed_req,
+                    &c->d_ed_rows};
   for (DevBuf* b : bufs) b->release();
   if (c->copy_stream) {
     cudaStreamDestroy(c->copy_stream);

@@ -129,6 +129,12 @@ struct afp_ctx {
   DevBuf d_st_off, d_st_ids, d_st_eval, d_st_seq, d_st_ovf, d_st_cnt, d_st_seg, d_st_heavy, d_st_part, d_st_scan;
   DevBuf d_st_obkt, d_st_opos, d_st_oval, d_st_slot, d_st_last;
   int64_t store_novf = 0;
+  // device-side HashTable.remove / retrieve for a list of ids (afp_table_edit.cu)
+  DevBuf d_ed_ids, d_ed_bits, d_ed_slot, d_ed_cnt, d_ed_off, d_ed_key, d_ed_key2, d_ed_val, d_ed_val2, d_ed_cub;
+  DevBuf d_ed_uoff, d_ed_req, d_ed_rows;
+  int64_t rt_total = -1;              // rows of the last afp_table_retrieve_ids; -1 = none
+  int rt_src = 0;                     // where they are: 0 d_ed_val, 1 d_ed_val2, 2 d_ed_rows
+  std::vector<int64_t> h_rt_off;      // [n+1] row offsets per requested id
   DevBuf d_mfast, d_mqlist;    // fast path: member-hit lists; [count + pad][query list] handed to the general kernel
   int64_t match_general = 0;   // queries of the last batch the general kernel processed
   int match_general_h = 0;

@@ -614,6 +614,13 @@ int afp_table_stats(afp_ctx* c) {
   return AFP_OK;
 }
 
+int afp_table_pruning_bound(afp_ctx* c, uint32_t* hmin) {
+  if (!c || !hmin) return AFP_ERR_INVALID;
+  if (!c->tab.loaded) AFP_FAIL(c, AFP_ERR_STATE, "no table on the device");
+  *hmin = c->tab.hmin;
+  return AFP_OK;
+}
+
 int afp_table_restrict_ids(afp_ctx* c, int64_t id_lo, int64_t id_hi) {
   if (!c) return AFP_ERR_INVALID;
   if (!c->tab.loaded) AFP_FAIL(c, AFP_ERR_STATE, "no table uploaded");

@@ -8,7 +8,9 @@ source of truth; `get_hits` (the hot method, 92 % of the reference's match
 time) runs on the GPU against a lazily refreshed device copy.  `store` exists
 twice: per track on the host, and batched on the device (`store_batch`,
 SURVEY.md §8f-1: the device copy then leads and the host arrays refresh from it
-when read); `merge` and `remove` are host bookkeeping.  All of them reproduce the
+when read).  `remove` and `retrieve` also exist batched on the device (`remove_batch`,
+`retrieve_batch`), which the per-name forms use while the device copy leads; `merge` is
+host bookkeeping.  All of them reproduce the
 reference's results exactly, including its draws from the global `random` /
 `np.random` generators on bucket overflow.
 """
@@ -382,7 +384,10 @@ class HashTable(object):
         return len(self.names) - 1
 
     def remove(self, name):
-        """Drop every entry of `name` (hash_table.py:347-367)."""
+        """Drop every entry of `name` (hash_table.py:347-367).  When the device copy is the
+        current one (after store_batch) the removal runs there (remove_batch)."""
+        if getattr(self, "_dev_newer", False):
+            return self.remove_batch([name])
         id_ = self.name_to_id(name)
         mine = (self.table >> np.uint32(self.maxtimebits)) == id_ + 1
         removed = 0
@@ -400,7 +405,10 @@ class HashTable(object):
         print("Removed", name, "(", removed, "hashes).")
 
     def retrieve(self, name):
-        """(time, hash) pairs stored for `name` (hash_table.py:369-385)."""
+        """(time, hash) pairs stored for `name` (hash_table.py:369-385), read from the device copy
+        when that is the current one (retrieve_batch)."""
+        if getattr(self, "_dev_newer", False):
+            return self.retrieve_batch([name])[0]
         id_ = self.name_to_id(name)
         tmask = (1 << self.maxtimebits) - 1
         valid = np.arange(self.depth)[None, :] < np.minimum(self.depth, self.counts)[:, None]
@@ -410,6 +418,94 @@ class HashTable(object):
         out[:, 0] = self.table[hs, slots] & tmask
         out[:, 1] = hs
         return out
+
+    # ---- batched remove / retrieve on the device table ---------------------------------------
+    def remove_batch(self, names):
+        """HashTable.remove (hash_table.py:346-364) for a list of tracks (names or ids) in ONE pass
+        over the device table.  Leaves table, counts, names and hashesperid as `for n in names:
+        self.remove(n)` does and prints the same lines, but checks the whole list first: an unknown
+        name, an id outside [0, len(names)) or a track named twice raises ValueError before
+        anything changes.  Afterwards the DEVICE copy is the current one (as after store_batch)."""
+        self._check_device_edit("remove_batch")
+        ids = self._ids_of(names, distinct=True)
+        if len(ids) == 0:
+            return
+        ctx = self._sync_device()
+        removed = np.zeros(len(ids), np.int64)
+        ctx.check(ctx.lib.afp_table_remove_ids(ctx.h, ids.ctypes.data_as(C.POINTER(C.c_int64)), len(ids),
+                                               removed.ctypes.data_as(C.POINTER(C.c_int64))))
+        hpi = self.__dict__["_hashesperid"]
+        for i in ids:
+            self.names[i] = None
+            hpi[i] = 0
+        self._touch()
+        self._dev_newer = True
+        ctx.table_key = self._dev_key = self._stamp()      # the device copy IS this version
+        ctx.table_owner = weakref.ref(self)
+        for name, n in zip(names, removed):
+            print("Removed", name, "(", int(n), "hashes).")
+
+    def retrieve_batch(self, names):
+        """HashTable.retrieve (hash_table.py:369-385) for a list of tracks (names or ids, repeats
+        allowed) in ONE pass over the device table: a list of int32 (n, 2) [time, hash] arrays,
+        each equal to retrieve(name).  An unknown name or an id outside [0, len(names)) raises
+        ValueError."""
+        self._check_device_edit("retrieve_batch")
+        ids = self._ids_of(names, distinct=False)
+        if len(ids) == 0:
+            return []
+        ctx = self._sync_device()
+        total = C.c_int64(0)
+        ctx.check(ctx.lib.afp_table_retrieve_ids(ctx.h, ids.ctypes.data_as(C.POINTER(C.c_int64)), len(ids),
+                                                 C.byref(total)))
+        rows = np.empty((int(total.value), 2), np.int32)
+        off = np.empty(len(ids) + 1, np.int64)
+        ctx.check(ctx.lib.afp_fetch_retrieved(ctx.h, rows.ctypes.data if len(rows) else None, 1,
+                                              off.ctypes.data_as(C.POINTER(C.c_int64))))
+        return [rows[off[k]:off[k + 1]] for k in range(len(ids))]
+
+    def _check_device_edit(self, what):
+        # a shard stamp left behind after another table took the device is no shard: _sync_device
+        # uploads the whole table again
+        if self._shard is not None and _lib.context(self.device).table_key == self._stamp(self._shard):
+            raise AfpStateError("the device copy is a shard (restrict_device_ids): cannot %s on it" % what)
+        if getattr(self, "_store_pending", False):
+            raise AfpStateError("%s: a store_batch_begin was not finished" % what)
+
+    def _ids_of(self, names, distinct):
+        """Ids of existing tracks, given by name or by integer id (name_to_id without adding).  A few
+        names are searched in the list (names.index: milliseconds each at a million tracks); more
+        go through one dict of all names built per call (a few hundred milliseconds at a million)."""
+        nids = len(self.names)
+        known = None
+        if sum(isinstance(n, (str, bytes)) for n in names) > 16:
+            try:        # walked backwards, so a name listed twice keeps its first id (names.index)
+                known = dict(zip(reversed(self.names), range(nids - 1, -1, -1)))
+            except TypeError:                 # a Matlab database marks removed tracks with []
+                known = {}
+                for i, n in enumerate(self.names):
+                    if isinstance(n, (str, bytes)) and n not in known:
+                        known[n] = i
+        ids = np.empty(len(names), np.int64)
+        for k, name in enumerate(names):
+            if isinstance(name, (str, bytes)):
+                if known is not None:
+                    i = known.get(name)
+                else:
+                    try:
+                        i = self.names.index(name)
+                    except ValueError:
+                        i = None
+                if i is None:
+                    raise ValueError("name " + str(name) + " not found")
+            else:
+                i = int(name)
+                if not 0 <= i < nids:
+                    raise ValueError("track id %d outside [0, %d)" % (i, nids))
+            ids[k] = i
+        if distinct and len(np.unique(ids)) != len(ids):
+            raise ValueError("a track is named twice")
+        return ids
 
     def list(self, print_fn=None):
         """One "<name> (<n> hashes)" line per stored track (hash_table.py:387-391)."""

@@ -53,6 +53,21 @@ def synth_query(track_pcm: np.ndarray, qseed: int, seconds: float = 10.0,
     return np.round(x * 32768.0).clip(-32768, 32767).astype(np.int16), off
 
 
+def synth_table(hashbits: int = 20, depth: int = 100, nids: int = 1_000_000, maxtimebits: int = 12,
+                seed: int = 0, overflow: int = 50):
+    """A hash table of the bench geometry with every slot filled: uniform-random ids in
+    [0, nids) and times in [0, 2^maxtimebits), counts[b] = depth + U[0, overflow) (buckets that
+    saw more inserts than they hold).  Returns (table, counts, hashesperid), hashesperid being
+    the entries each id holds."""
+    rng = np.random.default_rng(seed)
+    shape = (1 << hashbits, depth)
+    table = rng.integers(1, nids + 1, size=shape, dtype=np.uint32) << np.uint32(maxtimebits)
+    table |= rng.integers(0, 1 << maxtimebits, size=shape, dtype=np.uint32)
+    counts = (depth + rng.integers(0, overflow, size=shape[0])).astype(np.int32)
+    hpi = np.bincount((table >> np.uint32(maxtimebits)).ravel(), minlength=nids + 1)[1:].astype(np.uint32)
+    return table, counts, hpi
+
+
 def pcm_to_float(pcm: np.ndarray) -> np.ndarray:
     """int16 -> float32 in [-1, 1), exactly what the reference's reader yields
     (audio_read.py:139-145: scale 1/32768 applied to '<i2' samples)."""

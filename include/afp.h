@@ -226,6 +226,24 @@ int afp_table_download(afp_ctx* ctx, uint32_t* table, int32_t* counts);
  * random.setstate() continues where the reference would.  Host arithmetic only: this is the
  * reference's RNG, not part of the hot path. */
 int afp_mt_randint_replay(uint32_t* state625, const int32_t* count_before, int64_t n, int32_t* slot_out);
+/* HashTable.remove (hash_table.py:346-364) for n distinct ids in one pass over the device table;
+ * removed (HOST [n] or NULL) receives the entries each id had in the table.  A bucket holding an
+ * entry of one of the ids keeps its other entries below min(count, depth) in slot order, zeroes the
+ * rest of its row and takes their number as its count; other buckets are not written.  The ids'
+ * hashesperid become 0.  AFP_ERR_INVALID for an id outside [0, nids) or an id given twice.
+ * Not while a store batch is pending: its overflow entries name slots of the table as it was, so
+ * finish it (afp_table_apply_slots / afp_table_apply_patches) first. */
+int afp_table_remove_ids(afp_ctx* ctx, const int64_t* ids, int64_t n, int64_t* removed);
+/* HashTable.retrieve (hash_table.py:366-383) for n ids (repeats allowed): (time, hash) rows of the
+ * entries below min(count, depth), hash then slot order, one block per id in request order.
+ * *total_rows receives their number; afp_fetch_retrieved copies them, int32 [total][2], and the
+ * HOST int64 [n+1] offsets of every id's block. */
+int afp_table_retrieve_ids(afp_ctx* ctx, const int64_t* ids, int64_t n, int64_t* total_rows);
+int afp_fetch_retrieved(afp_ctx* ctx, int32_t* rows, int rows_on_host, int64_t* row_offsets /* HOST [n+1] */);
+/* The fast matching kernel's pruning bound of the device table: its smallest non-zero hashesperid,
+ * or 0 (no pruning) when no id has hashes or a live entry names an id whose hashesperid is 0.
+ * Recomputed by every call that changes hashesperid (upload, set_hashesperid, remove_ids). */
+int afp_table_pruning_bound(afp_ctx* ctx, uint32_t* hmin);
 /* Keep only ids in [id_lo, id_hi) of the uploaded table (sharded table,
  * SURVEY.md §8e); bucket-slot order is preserved. */
 int afp_table_restrict_ids(afp_ctx* ctx, int64_t id_lo, int64_t id_hi);
