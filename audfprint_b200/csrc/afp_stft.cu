@@ -245,7 +245,7 @@ __device__ __forceinline__ void stage_tile(const PcmT* pcm, const TileInfo& ti, 
 template <typename R, typename PcmT>
 constexpr size_t k1_smem_bytes() {
   return 512 * sizeof(R) + 2 * 256 * sizeof(typename K1Traits<R>::R2) + K1Traits<R>::LOGTAB_N * sizeof(double2) +
-         2 * FT * XF * sizeof(R) + 24 * sizeof(double) + 2 * sizeof(unsigned long long) +
+         2 * FT * XF * sizeof(R) + 2 * 24 * sizeof(double) + 2 * sizeof(unsigned long long) +
          PcmTraits<PcmT>::NBUF * (FT + 1) * AFP_N_HOP * sizeof(PcmT);
 }
 
@@ -265,8 +265,8 @@ __global__ void __launch_bounds__(K1_THREADS, K1Traits<R>::MIN_CTAS)
   double2* s_logtab_all = reinterpret_cast<double2*>(s_w512 + 256);    // Tr::LOGTAB_N
   R* s_xr = reinterpret_cast<R*>(s_logtab_all + Tr::LOGTAB_N);         // FT * XF
   R* s_xi = s_xr + FT * XF;                                            // FT * XF
-  double* s_red = reinterpret_cast<double*>(s_xi + FT * XF);           // 3 * 8
-  unsigned long long* s_bar = reinterpret_cast<unsigned long long*>(s_red + 24);   // 2
+  double* s_red = reinterpret_cast<double*>(s_xi + FT * XF);           // 2 x 3 * 8
+  unsigned long long* s_bar = reinterpret_cast<unsigned long long*>(s_red + 2 * 24);   // 2
   PcmT* s_pcm = reinterpret_cast<PcmT*>(s_bar + 2);                    // NBUF * (FT+1)*256, 16 B aligned
   constexpr int PCM_BUF = (FT + 1) * AFP_N_HOP;
   const PcmT* pcm = reinterpret_cast<const PcmT*>(a.pcm);
@@ -300,6 +300,7 @@ __global__ void __launch_bounds__(K1_THREADS, K1Traits<R>::MIN_CTAS)
   int item_nn = (tile + 2 * G < a.tile_end) ? a.tile_item[tile + 2 * G] : 0;
   stage_tile(pcm, cur, s_pcm, s_bar);
   int buf = 0;
+  int red = 0;   // NBUF == 1: which half of s_red this iteration's partials go to (NBUF == 2: buf)
 
   for (; tile < a.tile_end; tile += G) {
     const int next = tile + G;
@@ -400,7 +401,11 @@ __global__ void __launch_bounds__(K1_THREADS, K1Traits<R>::MIN_CTAS)
         vsum += lg;
       }
     }
-    // deterministic CTA reduction of (max |S|^2, min log, sum log), in FP64 for both precisions
+    // deterministic CTA reduction of (max |S|^2, min log, sum log), in FP64 for both precisions.
+    // The partials alternate between the two halves of s_red: thread 0 reads this tile's half after
+    // the barrier below, and when the next tile is wholly bulk-copied no barrier comes before the
+    // other warps write their next partials.  They go to the other half; writing this half again
+    // needs the next iteration's barrier, which thread 0 reaches only once it has read.
     hmin = __reduce_min_sync(0xffffffffu, hmin);
     const double vmin = Tr::log_lower_bound(hmin, s_logtab);   // +inf: this warp had no frame in the tile
     double dmax = vmax, dsum = vsum;
@@ -409,25 +414,26 @@ __global__ void __launch_bounds__(K1_THREADS, K1Traits<R>::MIN_CTAS)
       dmax = fmax(dmax, __shfl_xor_sync(0xffffffffu, dmax, o));
       dsum += __shfl_xor_sync(0xffffffffu, dsum, o);
     }
+    double* const s_part = s_red + 24 * (NBUF == 2 ? buf : red);
     if (lane == 0) {
-      s_red[(tid >> 5) * 3 + 0] = dmax;
-      s_red[(tid >> 5) * 3 + 1] = vmin;
-      s_red[(tid >> 5) * 3 + 2] = dsum;
+      s_part[(tid >> 5) * 3 + 0] = dmax;
+      s_part[(tid >> 5) * 3 + 1] = vmin;
+      s_part[(tid >> 5) * 3 + 2] = dsum;
     }
     __syncthreads();   // also: every thread is done with s_pcm[buf]
     if (tid == 0) {
       double m = 0.0, mn = INFINITY, sm = 0.0;
 #pragma unroll
       for (int w = 0; w < K1_THREADS / 32; ++w) {
-        m = fmax(m, s_red[w * 3 + 0]);
-        mn = fmin(mn, s_red[w * 3 + 1]);
-        sm += s_red[w * 3 + 2];
+        m = fmax(m, s_part[w * 3 + 0]);
+        mn = fmin(mn, s_part[w * 3 + 1]);
+        sm += s_part[w * 3 + 2];
       }
       a.tile_stats[(size_t)tile * 3 + 0] = 0.25 * m;
       a.tile_stats[(size_t)tile * 3 + 1] = mn;
       a.tile_stats[(size_t)tile * 3 + 2] = sm;
     }
-    if (NBUF == 2) buf ^= 1;
+    if (NBUF == 2) buf ^= 1; else red ^= 1;
     cur = nxt;
     if (tile + 2 * G < a.tile_end) nxt = make_tile(pcm, desc_nn, tile + 2 * G);
     item_nn = item_n3;
