@@ -80,7 +80,8 @@ void afp_destroy(afp_ctx* c) {
                     &c->d_mrow_off, &c->d_mrows_packed, &c->d_mcand, &c->d_mcand_cnt,
                     &c->d_ed_ids, &c->d_ed_bits, &c->d_ed_slot, &c->d_ed_cnt, &c->d_ed_off, &c->d_ed_key,
                     &c->d_ed_key2, &c->d_ed_val, &c->d_ed_val2, &c->d_ed_cub, &c->d_ed_uoff, &c->d_ed_req,
-                    &c->d_ed_rows};
+                    &c->d_ed_rows, &c->d_lg_key, &c->d_lg_cub, &c->d_lg_id, &c->d_lg_w, &c->d_lg_cand,
+                    &c->d_lg_dts, &c->d_lg_hist};
   for (DevBuf* b : bufs) b->release();
   if (c->copy_stream) {
     cudaStreamDestroy(c->copy_stream);

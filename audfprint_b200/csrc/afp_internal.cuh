@@ -146,6 +146,11 @@ struct afp_ctx {
   int64_t match_total_rows = -1;
   int32_t match_row_cap = 0;
   uint64_t match_layout = 0;   // carve-up of d_mscratch whose counters/histograms are known to be zero
+  // long-query path (afp_match_long.cu): sort keys, CUB temp, per-id counters and slots, ranking
+  // keys, candidate segments and rows, candidates' hits, per-CTA dtime histograms
+  DevBuf d_lg_key, d_lg_cub, d_lg_id, d_lg_w, d_lg_cand, d_lg_dts, d_lg_hist;
+  int lg_ctas = 0;                  // CTAs of the mode pass (one histogram pair each)
+  std::vector<int> match_long;      // queries of the last batch the long-query path finished
 };
 
 #define AFP_CUDA(ctx, call)                                                        \

@@ -701,11 +701,23 @@ int afp_match_batch(afp_ctx* c, const int32_t* q_rows, int q_on_host, int32_t nq
   AFP_CUDA(c, cudaSetDevice(c->device));
   c->match_total_rows = -1;
   c->match_nq = nqueries;
+  c->match_long.clear();
+  // A query of rows * depth >= AFP_LONG_HITS takes the long-query path (afp_match_long.cu) unless
+  // force_general is set; the rule depends on the query and the table only.  The fast and general
+  // kernels' scratch is sized over the other queries.
   int64_t maxnq = 0;
+  std::vector<int> longq;
   for (int i = 0; i < nqueries; ++i) {
     if (q_offsets[i + 1] < q_offsets[i]) AFP_FAIL(c, AFP_ERR_INVALID, "q_offsets must be non-decreasing");
-    maxnq = std::max<int64_t>(maxnq, q_offsets[i + 1] - q_offsets[i]);
+    const int64_t n = q_offsets[i + 1] - q_offsets[i];
+    if (!p->force_general && n * c->tab.depth >= AFP_LONG_HITS) {
+      if (n >= ((int64_t)1 << 31)) AFP_FAIL(c, AFP_ERR_UNSUPPORTED, "query of 2^31 rows or more");
+      longq.push_back(i);
+    } else {
+      maxnq = std::max<int64_t>(maxnq, n);
+    }
   }
+  const int nlong = (int)longq.size(), nshort = nqueries - nlong;
   const int64_t nrows_in = nqueries ? q_offsets[nqueries] : 0;
   if (nqueries && q_offsets[0] != 0) AFP_FAIL(c, AFP_ERR_INVALID, "q_offsets[0] must be 0");
   if (nrows_in > 0 && !q_rows) return AFP_ERR_INVALID;
@@ -722,19 +734,30 @@ int afp_match_batch(afp_ctx* c, const int32_t* q_rows, int q_on_host, int32_t nq
   }
   AFP_CUDA(c, cudaMemcpyAsync(c->d_qoff.p, q_offsets, sizeof(int64_t) * (size_t)(nqueries + 1),
                               cudaMemcpyHostToDevice, c->stream));
-  // largest / smallest query time (sizes the dtime histogram)
-  int h_mm[2] = {0, 0};
+  // largest / smallest query time (sizes the dtime histogram): [0, 1] over the fast / general
+  // kernels' queries, [2, 3] over the long ones (the row ranges in between are contiguous)
+  int h_mm[4] = {0, 0, 0, 0};
   AFP_CUDA(c, c->d_tmp.reserve(sizeof(int32_t) * (size_t)(nqueries + 8)));
   int* d_mm = c->d_tmp.as<int>();
-  AFP_CUDA(c, cudaMemsetAsync(d_mm, 0, 2 * sizeof(int), c->stream));
-  if (nrows_in > 0) {
-    afp_qmax_kernel<<<296, 256, 0, c->stream>>>(dq, nrows_in, d_mm, d_mm + 1);
-    AFP_CUDA(c, cudaGetLastError());
+  AFP_CUDA(c, cudaMemsetAsync(d_mm, 0, 4 * sizeof(int), c->stream));
+  auto qmax = [&](int64_t r0, int64_t r1, int* out) {
+    if (r1 <= r0) return cudaSuccess;
+    afp_qmax_kernel<<<296, 256, 0, c->stream>>>(dq + 2 * r0, r1 - r0, out, out + 1);
     c->launches++;
+    return cudaGetLastError();
+  };
+  {
+    int64_t r0 = 0;
+    for (int li : longq) {
+      AFP_CUDA(c, qmax(r0, q_offsets[li], d_mm));
+      AFP_CUDA(c, qmax(q_offsets[li], q_offsets[li + 1], d_mm + 2));
+      r0 = q_offsets[li + 1];
+    }
+    AFP_CUDA(c, qmax(r0, nrows_in, d_mm));
   }
-  AFP_CUDA(c, cudaMemcpyAsync(h_mm, d_mm, 2 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  AFP_CUDA(c, cudaMemcpyAsync(h_mm, d_mm, sizeof(h_mm), cudaMemcpyDeviceToHost, c->stream));
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));
-  if (h_mm[1] < 0) AFP_FAIL(c, AFP_ERR_INVALID, "negative query time");
+  if (h_mm[1] < 0 || h_mm[3] < 0) AFP_FAIL(c, AFP_ERR_INVALID, "negative query time");
 
   // persistent grid; a fixed CTA count keeps the scratch layout (and its zeroed state) reusable
   int nctas = c->num_sms;
@@ -761,9 +784,9 @@ int afp_match_batch(afp_ctx* c, const int32_t* q_rows, int q_on_host, int32_t nq
     AFP_FAIL(c, AFP_ERR_UNSUPPORTED, "query too large (rows * depth >= 2^30) or more than 2^24 track ids");
   const size_t per_cta = (size_t)a.hits_cap * (sizeof(uint2) + 4 * sizeof(uint32_t) + sizeof(double)) +
                          (size_t)a.hist_len * 2 * sizeof(int32_t) + 256;
-  // The scratch is per CTA and sized for the longest query of the batch (the reference has no
-  // query-length limit, hash_table.py:150-176; whole shows are matched in searching_for_ads.md):
-  // when it would not fit the memory budget the grid shrinks instead of the call failing.
+  // The scratch is per CTA and sized for the longest query the fast / general kernels run (whole
+  // shows, searching_for_ads.md, take the long-query path): when it would not fit the memory
+  // budget the grid shrinks instead of the call failing.
   {
     size_t free_b = 0, total_b = 0;
     AFP_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
@@ -817,6 +840,7 @@ int afp_match_batch(afp_ctx* c, const int32_t* q_rows, int q_on_host, int32_t nq
   a.qlist = nullptr;
   a.nlist = nullptr;
   a.fstat = nullptr;
+  a.qskip = nullptr;
   c->match_fast_ran = false;
   a.mhits = nullptr;
   a.mh_cap = 0;
@@ -824,30 +848,76 @@ int afp_match_batch(afp_ctx* c, const int32_t* q_rows, int q_on_host, int32_t nq
   a.bm_exact = c->tab.nids <= ((int64_t)1 << 20) ? 1 : 0;
   const bool fast = !p->force_general && p->threshcount >= 1 && p->search_depth >= 1 && c->tab.depth <= 65535 &&
                     a.hist_len < (1 << 30);
-  c->match_general = nqueries;
-  if (fast) {
-    a.mh_cap = (int)std::min<int64_t>(std::max<int64_t>((a.hits_cap + 31) / 32 * 32, 32768), 131072);   // 32 per-warp segments
-    AFP_CUDA(c, c->d_mfast.reserve(sizeof(uint2) * (size_t)a.mh_cap * (size_t)nctas));
-    AFP_CUDA(c, c->d_mqlist.reserve(sizeof(int32_t) * (size_t)(9 * nqueries + 4)));
-    a.mhits = c->d_mfast.as<uint2>();
+  c->match_general = nshort;
+  if (fast || nlong) {
+    // [count + pad][query list][status: 8 per query][long-query flags, bytes]
+    AFP_CUDA(c, c->d_mqlist.reserve(sizeof(int32_t) * (size_t)(9 * nqueries + 4) + (size_t)nqueries));
     a.nlist = c->d_mqlist.as<int>();
     a.qlist = c->d_mqlist.as<int32_t>() + 4;
     a.fstat = a.qlist + nqueries;
+  }
+  std::vector<int32_t> h_list;
+  std::vector<unsigned char> h_skip;
+  if (nlong) {
+    // the fast kernel skips the long queries; without it, the general kernel gets the others as its list
+    h_skip.assign(nqueries, 0);
+    for (int li : longq) h_skip[li] = 1;
+    unsigned char* d_skip = reinterpret_cast<unsigned char*>(a.fstat + 8 * (size_t)nqueries);
+    AFP_CUDA(c, cudaMemcpyAsync(d_skip, h_skip.data(), (size_t)nqueries, cudaMemcpyHostToDevice, c->stream));
+    a.qskip = d_skip;
+    if (!fast) {
+      h_list.assign(1, nshort);
+      h_list.resize(4, 0);
+      for (int i = 0; i < nqueries; ++i)
+        if (!h_skip[i]) h_list.push_back(i);
+      AFP_CUDA(c, cudaMemcpyAsync(a.nlist, h_list.data(), sizeof(int32_t) * h_list.size(), cudaMemcpyHostToDevice,
+                                  c->stream));
+    }
+  } else if (!fast) {
+    a.qlist = nullptr;
+    a.nlist = nullptr;
+    a.fstat = nullptr;
+  }
+  if (fast && nshort) {
+    a.mh_cap = (int)std::min<int64_t>(std::max<int64_t>((a.hits_cap + 31) / 32 * 32, 32768), 131072);   // 32 per-warp segments
+    AFP_CUDA(c, c->d_mfast.reserve(sizeof(uint2) * (size_t)a.mh_cap * (size_t)nctas));
+    a.mhits = c->d_mfast.as<uint2>();
     AFP_CUDA(c, cudaMemsetAsync(a.nlist, 0, sizeof(int), c->stream));
     AFP_CUDA(c, afp_launch_match_fast(a, nctas, c->stream));
     c->launches++;
     c->match_fast_ran = true;
   }
-  AFP_CUDA(c, cudaFuncSetAttribute(afp_match_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   (int)(QCAP * sizeof(unsigned long long))));
-  afp_match_kernel<<<nctas, MT, QCAP * sizeof(unsigned long long), c->stream>>>(a);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
-  if (fast)
+  if (nshort) {
+    AFP_CUDA(c, cudaFuncSetAttribute(afp_match_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)(QCAP * sizeof(unsigned long long))));
+    afp_match_kernel<<<nctas, MT, QCAP * sizeof(unsigned long long), c->stream>>>(a);
+    AFP_CUDA(c, cudaGetLastError());
+    c->launches++;
+  }
+  if (c->match_fast_ran)
     AFP_CUDA(c, cudaMemcpyAsync(&c->match_general_h, a.nlist, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  if (nlong) {
+    // ---- long queries (afp_match_long.cu): one histogram pair per CTA of the mode pass, sized
+    // over the long queries' times, zeroed here and left zeroed by the mode search
+    MatchArgs al = a;
+    al.bias = h_mm[2] + p->window + 2;
+    al.hist_len = (1 << c->tab.maxtimebits) + al.bias + p->window + 4;
+    const size_t per = (size_t)al.hist_len * 2 * sizeof(int32_t);
+    size_t free_b = 0, total_b = 0;
+    AFP_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
+    const size_t budget = std::max<size_t>((free_b + c->d_lg_hist.cap) / 2, (size_t)1 << 30);
+    c->lg_ctas = (int)std::max<size_t>(1, std::min<size_t>((size_t)c->num_sms, budget / per));
+    AFP_CUDA(c, c->d_lg_hist.reserve(per * (size_t)c->lg_ctas));
+    al.hist = c->d_lg_hist.as<int32_t>();
+    al.filt = al.hist + (size_t)al.hist_len * c->lg_ctas;
+    AFP_CUDA(c, cudaMemsetAsync(al.hist, 0, sizeof(int32_t) * (size_t)al.hist_len * c->lg_ctas, c->stream));
+    for (int li : longq)
+      if ((rc = afp_match_long(c, al, li, q_offsets[li], q_offsets[li + 1] - q_offsets[li]))) return rc;
+    c->match_long = longq;
+  }
   int64_t total = 0;
   if ((rc = afp_finish_match_rows(c, nqueries, a.row_cap, &total))) return rc;
-  if (fast) c->match_general = c->match_general_h;     // (the stream was synchronised)
+  if (c->match_fast_ran) c->match_general = c->match_general_h;     // (the stream was synchronised)
   if (total_rows) *total_rows = total;
   return AFP_OK;
 }
@@ -865,12 +935,16 @@ int afp_fetch_match_status(afp_ctx* c, int32_t* status) {
   AFP_CUDA(c, cudaSetDevice(c->device));
   if (!c->match_fast_ran) {
     for (int i = 0; i < 8 * c->match_nq; ++i) status[i] = -1;
-    return AFP_OK;
+  } else {
+    if (c->match_nq > 0)
+      AFP_CUDA(c, cudaMemcpyAsync(status, c->d_mqlist.as<int32_t>() + 4 + c->match_nq,
+                                  sizeof(int32_t) * 8 * (size_t)c->match_nq, cudaMemcpyDeviceToHost, c->stream));
+    AFP_CUDA(c, cudaStreamSynchronize(c->stream));
   }
-  if (c->match_nq > 0)
-    AFP_CUDA(c, cudaMemcpyAsync(status, c->d_mqlist.as<int32_t>() + 4 + c->match_nq, sizeof(int32_t) * 8 * (size_t)c->match_nq,
-                                cudaMemcpyDeviceToHost, c->stream));
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+  for (int qi : c->match_long) {          // finished by the long-query path
+    status[8 * (size_t)qi] = 6;
+    for (int k = 1; k < 8; ++k) status[8 * (size_t)qi + k] = 0;
+  }
   return AFP_OK;
 }
 

@@ -1,5 +1,5 @@
-// Pieces shared by the two matching kernels (afp_match.cu: general path, afp_match_fast.cu:
-// fast path): kernel arguments and the fast kernel's launcher, launch geometry, candidate order,
+// Pieces shared by the matching kernels (afp_match.cu: general path, afp_match_fast.cu: fast path;
+// afp_match_long.cu reuses the quick filter and the mode search): kernel arguments and the fast kernel's launcher, launch geometry, candidate order,
 // block-wide helpers (scan, bitonic sort, arg-max) and the candidate stage that follows the
 // ranking in both kernels - publish and dt-list offsets of the top-K, quick filter, per-candidate
 // dtime histogram and its mode search (audfprint_match.py:284-311), end-of-query counts.  Each
@@ -39,6 +39,7 @@ struct MatchArgs {
   int32_t* qlist;
   int* nlist;
   int32_t* fstat;                         // [nqueries] 0 = done by the fast kernel, else the reason it was not
+  const unsigned char* qskip;             // [nqueries] 1 = long query (afp_match_long.cu), not the fast kernel's; NULL = none
   // fast path (afp_match_fast.cu)
   uint2* mhits;     int mh_cap;           // per-CTA list of the hits of multi-record ids: (set slot, dt + bias)
   unsigned hmin;                          // smallest hashesperid of the table; 0 = unknown (no pruning)
@@ -47,6 +48,12 @@ struct MatchArgs {
 
 // The fast kernel over every query (afp_match_fast.cu); it appends the ones it hands over to a.qlist.
 cudaError_t afp_launch_match_fast(const MatchArgs& a, int nctas, cudaStream_t stream);
+// Query qi (rows q0 .. q0+nq of a.q) on the long-query path (afp_match_long.cu): writes its rows,
+// row count and, in publish mode, its candidate list.  a.hist / a.filt / a.hist_len / a.bias are
+// the mode pass's per-CTA histograms (zeroed; left zeroed), c->lg_ctas CTAs of them.
+int afp_match_long(afp_ctx* c, const MatchArgs& a, int qi, int64_t q0, int64_t nq);
+// rows * depth from which a query takes the long-query path
+constexpr int64_t AFP_LONG_HITS = (int64_t)1 << 24;
 
 namespace {
 
@@ -223,6 +230,20 @@ __device__ inline void candidate_modes(const MatchArgs& a, ModeScratch& sh, int3
   __syncthreads();
 }
 
+// Quick filter of a candidate's dt list L[0..n): the largest number of times one of the entries
+// i0, i0 + step, ... occurs in the list (the caller reduces over the threads that split it).  The
+// largest dtime bin is the maximum over all entries; a row needs it above threshcount (:291).
+__device__ __forceinline__ int max_repeat(const uint32_t* L, int n, int i0, int step) {
+  int best = 0;
+  for (int i = i0; i < n; i += step) {
+    const uint32_t me = L[i];
+    int cnt = 0;
+    for (int k = 0; k < n; ++k) cnt += (L[k] == me) ? 1 : 0;
+    best = max(best, cnt);
+  }
+  return best;
+}
+
 // Start of the candidate stage: thread `tid` < ncand holds rank tid's (id, raw, weight bits).
 // Publishes the ranked list in shard mode and lays out the dt lists of the candidates that can
 // yield rows (raw > threshcount, :291) back to back; returns whether rank tid is one of them.
@@ -255,15 +276,7 @@ __device__ __forceinline__ void candidates_finish(const MatchArgs& a, int qi, in
   for (int j = warp; j < ncand; j += NW) {
     const int n = (int)c.raw[j];
     if (n <= a.thresh) continue;       // warp-uniform
-    const uint32_t* L = dts + c.loff[j];
-    int best = 0;
-    for (int i = lane; i < n; i += 32) {
-      const uint32_t me = L[i];
-      int cnt = 0;
-      for (int k = 0; k < n; ++k) cnt += (L[k] == me) ? 1 : 0;
-      best = max(best, cnt);
-    }
-    best = __reduce_max_sync(0xffffffffu, best);
+    const int best = __reduce_max_sync(0xffffffffu, max_repeat(dts + c.loff[j], n, lane, 32));
     if (lane == 0) c.pass[j] = best > a.thresh;
   }
   __syncthreads();

@@ -348,6 +348,7 @@ __global__ void __launch_bounds__(MT) afp_match_fast_kernel(MatchArgs a) {
   };
 
   for (int qi = blockIdx.x; qi < a.nqueries; qi += gridDim.x) {
+    if (a.qskip && a.qskip[qi]) continue;          // (uniform) the long-query path takes it
     const int64_t q0 = a.qoff[qi];
     const int nq = (int)(a.qoff[qi + 1] - q0);
     __syncthreads();                               // the previous query is completely done

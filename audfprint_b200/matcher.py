@@ -78,7 +78,8 @@ class Matcher(object):
     @staticmethod
     def last_status(ht, nqueries):
         """int32 (nqueries, 8) of the last device call (afp_fetch_match_status): column 0 is 0 for the
-        fast kernel, > 0 = reason for the general kernel, -1 = the fast kernel did not run."""
+        fast kernel, 1-5 = reason for the general kernel, 6 = the long-query path (rows * depth >= 2^24,
+        whether or not the fast kernel ran), -1 = the fast kernel did not run."""
         ctx = _lib.context(ht.device)
         st = np.zeros((max(nqueries, 1), 8), np.int32)
         ctx.check(ctx.lib.afp_fetch_match_status(ctx.h, st.ctypes.data))

@@ -266,14 +266,18 @@ int afp_match_batch(afp_ctx* ctx, const int32_t* q_rows, int q_on_host, int32_t 
                     const int64_t* q_offsets, const afp_matcher_params* p,
                     int64_t* total_rows);
 int afp_fetch_match_rows(afp_ctx* ctx, int32_t* rows, int rows_on_host, int64_t* row_offsets);
-/* How many queries of the last afp_match_batch went through the general kernel (all of them
- * with force_general; otherwise the ones outside the fast kernel's capacities). */
+/* afp_match_batch sends a query of rows * depth >= 2^24 to the long-query path (grid-wide passes,
+ * memory sized by the query's actual hits, identical rows) unless force_general is set.
+ * How many queries of the last afp_match_batch went through the general kernel (all of them
+ * with force_general; otherwise the ones outside the fast kernel's capacities, never the long
+ * ones). */
 int afp_match_general_count(afp_ctx* ctx, int64_t* n);
 /* Per query of the last batch, HOST int32 [nqueries][8]:
  *   [0] 0 = the fast kernel finished it, > 0 = why it was handed to the general kernel
  *       (1 multi-record id set full, 2 member-hit list full, 3 too many single-record ids outrank
  *       the K-th member, 4 shard mode with > 2^20 ids and fewer members than search_depth,
- *       5 candidate depth > 1024), -1 = the fast kernel did not run;
+ *       5 candidate depth > 1024), 6 = the long-query path finished it (columns 1-7 are 0 then),
+ *       -1 = the fast kernel did not run;
  *   [1] multi-record ids, [2] their hits, [3] single-record ids admitted by pass 3,
  *   [4] candidate depth, [5] ids above threshcount, [6] largest bucket multiplicity, [7] distinct
  *       ids (shard mode only). */
