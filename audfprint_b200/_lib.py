@@ -59,6 +59,7 @@ _SIGS = {
     "afp_spread_peaks": (C.c_int, [_P, _P, C.c_int32, _P, C.c_double, _P, _P]),
     "afp_stft_mag": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int64, _P, C.c_int]),
     "afp_sgram": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int64, _P, C.c_int]),
+    "afp_fingerprint_from_logs": (C.c_int, [_P, _P, C.c_int, C.c_int32, _P, _P, _I64P]),
     "afp_table_upload": (C.c_int, [_P, _P, _P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int]),
     "afp_table_create": (C.c_int, [_P, C.c_int32, C.c_int32, C.c_int32]),
     "afp_table_set_hashesperid": (C.c_int, [_P, _P, C.c_int64]),

@@ -180,6 +180,41 @@ int afp_set_analyzer(afp_ctx* c, const afp_analyzer_params* p, const double* win
 
 }  // extern "C"
 
+// Size the workspace for the batch described by h_items / h_file_col_base and the totals
+// (afp_fingerprint_batch, afp_sgram, afp_fingerprint_from_logs), and upload its item table.
+static int reserve_batch(afp_ctx* c) {
+  const int32_t nfiles = c->nfiles;
+  const int64_t frames = c->total_frames, tiles = c->total_tiles, cols = c->total_cols;
+  const size_t P = (size_t)c->ap.maxpksperframe, F = (size_t)c->ap.maxpairsperpeak;
+  const size_t fr = (size_t)frames + 1;
+  AFP_CUDA(c, c->d_items.reserve(sizeof(ItemDesc) * (size_t)(c->nitems + 1)));
+  AFP_CUDA(c, c->d_file_col_base.reserve(sizeof(int64_t) * (size_t)(nfiles + 1)));
+  AFP_CUDA(c, c->d_tile_item.reserve(sizeof(int32_t) * (size_t)(tiles + 1)));
+  AFP_CUDA(c, c->d_logs.reserve(sizeof(double) * AFP_NBINS * fr));
+  AFP_CUDA(c, c->d_nyq.reserve(sizeof(double) * fr));
+  AFP_CUDA(c, c->d_tile_stats.reserve(sizeof(double) * 3 * (size_t)(tiles + 1)));
+  AFP_CUDA(c, c->d_item_stats.reserve(sizeof(ItemStats) * (size_t)(c->nitems + 1)));
+  AFP_CUDA(c, c->d_fwd_val.reserve(sizeof(double) * P * fr));
+  AFP_CUDA(c, c->d_fwd_bin.reserve(P * fr));
+  AFP_CUDA(c, c->d_fwd_cnt.reserve(fr));
+  AFP_CUDA(c, c->d_pk_bin.reserve(P * fr));
+  AFP_CUDA(c, c->d_pk_cnt.reserve(fr));
+  AFP_CUDA(c, c->d_item_scols.reserve(sizeof(int32_t) * (size_t)(c->nitems + 1)));
+  AFP_CUDA(c, c->d_item_npeaks.reserve(sizeof(int32_t) * (size_t)(c->nitems + 1)));
+  AFP_CUDA(c, c->d_lm.reserve(sizeof(uint32_t) * P * F * fr));
+  AFP_CUDA(c, c->d_col_cnt.reserve(sizeof(int32_t) * (size_t)(cols + 1)));
+  AFP_CUDA(c, c->d_file_tot.reserve(sizeof(int32_t) * (size_t)(nfiles + 1)));
+  AFP_CUDA(c, c->d_file_off.reserve(sizeof(int64_t) * (size_t)(nfiles + 1)));
+  // upper bound on the output: every hash slot distinct
+  AFP_CUDA(c, c->d_hashes.reserve(sizeof(int32_t) * 2 * (P * F * fr + 1)));
+  if (c->nitems > 0)
+    AFP_CUDA(c, cudaMemcpyAsync(c->d_items.p, c->h_items.data(), sizeof(ItemDesc) * (size_t)c->nitems,
+                                cudaMemcpyHostToDevice, c->stream));
+  AFP_CUDA(c, cudaMemcpyAsync(c->d_file_col_base.p, c->h_file_col_base.data(),
+                              sizeof(int64_t) * (size_t)(nfiles + 1), cudaMemcpyHostToDevice, c->stream));
+  return AFP_OK;
+}
+
 // Build the item table of a batch, size the workspace, stage the PCM.
 static int prepare_batch(afp_ctx* c, const void* pcm, int dtype, int on_host, int32_t nfiles,
                          const int64_t* off, const int64_t* lens, int shifts, const void** pcm_dev,
@@ -220,33 +255,8 @@ static int prepare_batch(afp_ctx* c, const void* pcm, int dtype, int on_host, in
   c->total_frames = frames;
   c->total_tiles = tiles;
   c->total_cols = cols;
-  const size_t P = (size_t)c->ap.maxpksperframe, F = (size_t)c->ap.maxpairsperpeak;
-  const size_t fr = (size_t)frames + 1;
-  AFP_CUDA(c, c->d_items.reserve(sizeof(ItemDesc) * (size_t)(c->nitems + 1)));
-  AFP_CUDA(c, c->d_file_col_base.reserve(sizeof(int64_t) * (size_t)(nfiles + 1)));
-  AFP_CUDA(c, c->d_tile_item.reserve(sizeof(int32_t) * (size_t)(tiles + 1)));
-  AFP_CUDA(c, c->d_logs.reserve(sizeof(double) * AFP_NBINS * fr));
-  AFP_CUDA(c, c->d_nyq.reserve(sizeof(double) * fr));
-  AFP_CUDA(c, c->d_tile_stats.reserve(sizeof(double) * 3 * (size_t)(tiles + 1)));
-  AFP_CUDA(c, c->d_item_stats.reserve(sizeof(ItemStats) * (size_t)(c->nitems + 1)));
-  AFP_CUDA(c, c->d_fwd_val.reserve(sizeof(double) * P * fr));
-  AFP_CUDA(c, c->d_fwd_bin.reserve(P * fr));
-  AFP_CUDA(c, c->d_fwd_cnt.reserve(fr));
-  AFP_CUDA(c, c->d_pk_bin.reserve(P * fr));
-  AFP_CUDA(c, c->d_pk_cnt.reserve(fr));
-  AFP_CUDA(c, c->d_item_scols.reserve(sizeof(int32_t) * (size_t)(c->nitems + 1)));
-  AFP_CUDA(c, c->d_item_npeaks.reserve(sizeof(int32_t) * (size_t)(c->nitems + 1)));
-  AFP_CUDA(c, c->d_lm.reserve(sizeof(uint32_t) * P * F * fr));
-  AFP_CUDA(c, c->d_col_cnt.reserve(sizeof(int32_t) * (size_t)(cols + 1)));
-  AFP_CUDA(c, c->d_file_tot.reserve(sizeof(int32_t) * (size_t)(nfiles + 1)));
-  AFP_CUDA(c, c->d_file_off.reserve(sizeof(int64_t) * (size_t)(nfiles + 1)));
-  // upper bound on the output: every hash slot distinct
-  AFP_CUDA(c, c->d_hashes.reserve(sizeof(int32_t) * 2 * (P * F * fr + 1)));
-  if (c->nitems > 0)
-    AFP_CUDA(c, cudaMemcpyAsync(c->d_items.p, c->h_items.data(), sizeof(ItemDesc) * (size_t)c->nitems,
-                                cudaMemcpyHostToDevice, c->stream));
-  AFP_CUDA(c, cudaMemcpyAsync(c->d_file_col_base.p, c->h_file_col_base.data(),
-                              sizeof(int64_t) * (size_t)(nfiles + 1), cudaMemcpyHostToDevice, c->stream));
+  int rc = reserve_batch(c);
+  if (rc) return rc;
   *pcm_dev = pcm;
   if (on_host && nfiles > 0) {
     const size_t esz = dtype == AFP_PCM_I16 ? 2 : 4;
@@ -371,6 +381,71 @@ int afp_fingerprint_batch(afp_ctx* c, const void* pcm, int pcm_dtype, int pcm_on
     AFP_CUDA(c, cudaStreamSynchronize(c->stream));
     *total_hashes = c->total_hashes;
   }
+  return AFP_OK;
+}
+
+int afp_fingerprint_from_logs(afp_ctx* c, const void* logs, int logs_on_host, int32_t nfiles,
+                              const int32_t* item_frames, const double* item_stats, int64_t* total_hashes) {
+  if (!c) return AFP_ERR_INVALID;
+  if (!c->analyzer_set) AFP_FAIL(c, AFP_ERR_STATE, "afp_set_analyzer has not been called");
+  if (nfiles < 0 || (nfiles > 0 && (!item_frames || !item_stats)))
+    AFP_FAIL(c, AFP_ERR_INVALID, "null item frames / stats");
+  const int S = c->ap.shifts;
+  int64_t frames = 0;
+  for (int f = 0; f < nfiles; ++f)
+    for (int s = 0; s < S; ++s) {
+      const int32_t n = item_frames[(size_t)f * S + s];
+      if (n < 0) AFP_FAIL(c, AFP_ERR_INVALID, "item frame counts must be >= 0");
+      if (n > item_frames[(size_t)f * S]) AFP_FAIL(c, AFP_ERR_INVALID, "a shift item is longer than shift 0");
+      frames += n;
+    }
+  if (frames > 0 && !logs) AFP_FAIL(c, AFP_ERR_INVALID, "null logs");
+  AFP_CUDA(c, cudaSetDevice(c->device));
+  c->batch_valid = false;
+  c->ev_valid = false;
+  c->total_hashes = -1;
+  c->nfiles = nfiles;
+  c->nitems = nfiles * S;
+  c->h_items.assign((size_t)c->nitems, ItemDesc{});
+  c->h_file_col_base.resize((size_t)nfiles + 1);
+  std::vector<ItemStats> st((size_t)c->nitems);
+  int64_t base = 0, cols = 0;
+  for (int i = 0; i < c->nitems; ++i) {
+    ItemDesc& it = c->h_items[(size_t)i];
+    it.nframes = item_frames[i];
+    it.frame_base = base;
+    base += it.nframes;
+    if (i % S == 0) {
+      c->h_file_col_base[(size_t)i / S] = cols;
+      cols += it.nframes;
+    }
+    st[(size_t)i] = ItemStats{item_stats[3 * i], item_stats[3 * i + 1], item_stats[3 * i + 2] != 0.0 ? 1 : 0, 0};
+  }
+  c->h_file_col_base[(size_t)nfiles] = cols;
+  c->total_frames = frames;
+  c->total_tiles = 0;
+  c->total_cols = cols;
+  int rc = reserve_batch(c);
+  if (rc) return rc;
+  // K2 bulk-copies its columns out of d_logs, as it does after K1
+  const size_t esz = c->ap.spectrogram_fp32 ? sizeof(float) : sizeof(double);
+  if (frames > 0)
+    AFP_CUDA(c, cudaMemcpyAsync(c->d_logs.p, logs, esz * AFP_NBINS * (size_t)frames,
+                                logs_on_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, c->stream));
+  if (c->nitems > 0)
+    AFP_CUDA(c, cudaMemcpyAsync(c->d_item_stats.p, st.data(), sizeof(ItemStats) * st.size(), cudaMemcpyHostToDevice,
+                                c->stream));
+  if ((rc = afp_launch_peaks(c, 0, c->nitems))) return rc;
+  if ((rc = afp_launch_landmarks(c, 0, c->nitems))) return rc;
+  if ((rc = afp_launch_hashes(c))) return rc;
+  if ((rc = afp_write_hashes(c))) return rc;
+  c->batch_valid = true;
+  c->total_hashes = 0;
+  if (nfiles > 0)
+    AFP_CUDA(c, cudaMemcpyAsync(&c->total_hashes, c->d_file_off.as<int64_t>() + nfiles, sizeof(int64_t),
+                                cudaMemcpyDeviceToHost, c->stream));
+  AFP_CUDA(c, cudaStreamSynchronize(c->stream));   // `st` and host logs must outlive their copies
+  if (total_hashes) *total_hashes = c->total_hashes;
   return AFP_OK;
 }
 

@@ -159,8 +159,9 @@ int afp_fetch_peaks(afp_ctx* ctx, int32_t shift, int32_t* rows, int rows_on_host
 /* Analyzer.peaks2landmarks (audfprint_analyze.py:310-343) on an explicit peak
  * list (e.g. read from a precomputed .afpk file): `peak_rows` int32 [n][2] =
  * (col, bin), column-major with bins ascending.  Result (fetch): int32 [L][4] =
- * (col, bin1, bin2, dt) in the reference's generation order.  Invalidates the
- * last fingerprint batch. */
+ * (col, bin1, bin2, dt) in the reference's generation order.  Columns may be
+ * anywhere in [0, 2^28]; like afp_fingerprint_batch, the pairing does not depend
+ * on how far from column 0 the peaks lie.  Invalidates the last fingerprint batch. */
 int afp_landmarks_from_peaks(afp_ctx* ctx, const int32_t* peak_rows, int64_t npeaks, int on_host,
                              int64_t* nlandmarks);
 int afp_fetch_landmarks(afp_ctx* ctx, int32_t* rows, int rows_on_host);
@@ -184,6 +185,15 @@ int afp_stft_mag(afp_ctx* ctx, const void* pcm, int pcm_dtype, int pcm_on_host, 
  * (audfprint_analyze.py:280-295). */
 int afp_sgram(afp_ctx* ctx, const void* pcm, int pcm_dtype, int pcm_on_host, int64_t n,
               double* sgram, int sgram_on_host);
+/* Exposed for the K2/K3 checks: run the product's K2 -> K3 -> merge chain on a caller-supplied
+ * log-magnitude spectrogram instead of K1's output.
+ *   logs         [sum of item frames][256], double (float in the FP32 spectrogram mode), items
+ *                file-major (item f*shifts + s), the same layout as the workspace's d_logs
+ *   item_frames  HOST int32 [nfiles*shifts]; an item of shift s > 0 may not be longer than shift 0
+ *   item_stats   HOST double [nitems][3] = (logfloor, mean, allzero != 0)
+ * Afterwards afp_fetch_hashes / afp_fetch_peaks return results as after afp_fingerprint_batch. */
+int afp_fingerprint_from_logs(afp_ctx* ctx, const void* logs, int logs_on_host, int32_t nfiles,
+                              const int32_t* item_frames, const double* item_stats, int64_t* total_hashes);
 
 /* ---- HashTable --------------------------------------------------------------
  * Device-resident copy of HashTable.table / counts / hashesperid

@@ -246,7 +246,12 @@ def fingerprint(d: np.ndarray, density: float = 20.0, fanout: int = 3, shifts: i
             lists.append(find_peaks(d[off:], density, f_sd, maxpks))
     if shifts < 2 and len(lists[0]) == 0:
         return np.zeros((0, 2), np.int32)
-    rows = np.concatenate([landmarks_to_hashes(peaks_to_landmarks(pl, fanout)) for pl in lists])
+    return unique_rows(np.concatenate([landmarks_to_hashes(peaks_to_landmarks(pl, fanout)) for pl in lists]))
+
+
+def unique_rows(rows: np.ndarray) -> np.ndarray:
+    """int32 (N,2) [time, hash] rows of all shifts -> sorted by (time, hash), duplicates removed.
+    audfprint_analyze.py:415-421."""
     key = (rows[:, 0].astype(np.uint64) << np.uint64(32)) + rows[:, 1].astype(np.uint64)
     key = np.unique(key)
     return np.stack([key >> np.uint64(32), key & np.uint64(0xFFFFFFFF)], axis=1).astype(np.int32)
