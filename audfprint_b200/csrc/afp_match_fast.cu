@@ -45,9 +45,10 @@ constexpr int SCAP = 4096;                  // rank-sort capacity: selected memb
 constexpr int XCAP = 2048;                  // single-record ids pass 3 may admit
 constexpr int PROBE_MAX = 256;              // insertion gives up (set full) after this many probes
 constexpr int WBINS = 4096;                 // weight histogram bins (float image of the weight, top 16 bits)
-// why a query was handed to the general kernel (afp_fetch_match_status)
+// why a query was handed to the general kernel (afp_fetch_match_status, include/afp.h); 6 is the
+// long-query path's code, never the fast kernel's
 enum { FS_DONE = 0, FS_SET_FULL = 1, FS_HITS_FULL = 2, FS_EXTRAS_FULL = 3, FS_NDIST_UNKNOWN = 4, FS_DEPTH = 5,
-       FS_INCONSISTENT = 6, FS_TIES = 7 };
+       FS_TIES = 7, FS_INCONSISTENT = 8 };
 
 // dynamic shared memory (bytes).  R0 is the "seen" bitmap in pass 1, the "member" bitmap in
 // pass 2, then the member counters + selection / rank arrays; R2 holds the sorted query chunk

@@ -110,8 +110,12 @@ class Matcher(object):
     @staticmethod
     def last_status(ht, nqueries):
         """int32 (nqueries, 8) of the last device call (afp_fetch_match_status): column 0 is 0 for the
-        fast kernel, 1-5 = reason for the general kernel, 6 = the long-query path (rows * depth >= 2^24,
-        whether or not the fast kernel ran), -1 = the fast kernel did not run."""
+        fast kernel; the reason the fast kernel handed the query to the general kernel: 1 member set
+        full, 2 member-hit list full, 3 more than 2048 single-record ids admitted, 4 shard mode with
+        > 2^20 ids and fewer members than search_depth, 5 candidate depth > 1024, 7 more than 2048
+        members at or above the K-th member's weight bin, 8 internal consistency check; 6 = the
+        long-query path (rows * depth >= 2^24, whether or not the fast kernel ran); -1 = the fast
+        kernel did not run."""
         ctx = _lib.context(ht.device)
         st = np.zeros((max(nqueries, 1), 8), np.int32)
         ctx.check(ctx.lib.afp_fetch_match_status(ctx.h, st.ctypes.data))

@@ -287,8 +287,9 @@ int afp_match_general_count(afp_ctx* ctx, int64_t* n);
  *   [0] 0 = the fast kernel finished it, > 0 = why it was handed to the general kernel
  *       (1 multi-record id set full, 2 member-hit list full, 3 too many single-record ids outrank
  *       the K-th member, 4 shard mode with > 2^20 ids and fewer members than search_depth,
- *       5 candidate depth > 1024), 6 = the long-query path finished it (columns 1-7 are 0 then),
- *       -1 = the fast kernel did not run;
+ *       5 candidate depth > 1024, 7 more than 2048 members at or above the weight bin of the
+ *       K-th member, 8 internal consistency check), 6 = the long-query path finished it
+ *       (columns 1-7 are 0 then), -1 = the fast kernel did not run;
  *   [1] multi-record ids, [2] their hits, [3] single-record ids admitted by pass 3,
  *   [4] candidate depth, [5] ids above threshcount, [6] largest bucket multiplicity, [7] distinct
  *       ids (shard mode only). */

@@ -1,9 +1,11 @@
 """The fast matching kernel (csrc/afp_match_fast.cu) against the oracle and against the general
-kernel, on tables big enough that most probed track ids are hit exactly once - the regime it is
-built for - and on inputs crafted to drive each of its branches: pruning of single-record ids,
-pass 3 (single-record ids that DO outrank members), no pruning (hashesperid == 0 referenced),
-hashed bitmap (> 2^20 ids), chunked long queries, capacity overflow -> handover to the general
-kernel, table-shard (publish) mode."""
+kernel, on random tables big enough that most probed track ids are hit exactly once - the regime it
+is built for - with pruning of single-record ids, pass 3 (single-record ids that DO outrank
+members), no pruning (hashesperid == 0 referenced), hashed bitmap (> 2^20 ids), chunked long
+queries, a member-set overflow handed to the general kernel, and table-shard (publish) mode.
+Rows are compared with the oracle as sets, so a wrong id deep in the candidate list that yields no
+row goes unseen here: tests/test_gpu_k4_ranking_edges.py compares the ranked lists themselves, in
+order, and reaches each handover reason on both sides of its limit."""
 import numpy as np
 import pytest
 

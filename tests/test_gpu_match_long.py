@@ -2,8 +2,8 @@
 broadcast days - matched over the whole grid with memory sized by their actual hits.
 
 The oracle's get_hits loops over query rows in Python; for queries of 10^5 rows and more the
-same semantics are stated here in NumPy (_np_rows), checked first against the oracle on small
-queries.  The general kernel is the other side of the A/B comparisons (force_general_kernel)."""
+same semantics are stated in NumPy (tests/k4_reference.py), checked first against the oracle on
+small queries.  The general kernel is the other side of the A/B comparisons (force_general_kernel)."""
 import os
 
 import numpy as np
@@ -12,60 +12,13 @@ import pytest
 from audfprint_b200 import HashTable, Matcher
 from oracle import afp_oracle as orc
 from tests import cases
+from tests.k4_reference import by_count as _by_count, np_hits as _np_hits, np_rows as _np_rows
 from tests.conftest import GOLDEN
 
 pytestmark = pytest.mark.gpu
 
 LONG_HITS = 1 << 24
 LONG_STATUS = 6
-
-
-# ---- NumPy statement of get_hits -> rank_candidates -> offset_histogram_rows -------------------
-def _np_hits(table, counts, hashbits, depth, mtb, q):
-    """(ids, dtimes) of every hit in (query row, slot) order, as orc.get_hits."""
-    q = np.asarray(q, np.int64).reshape(-1, 2)
-    b = q[:, 1] & ((1 << hashbits) - 1)
-    n = np.minimum(depth, counts[b]).astype(np.int64)
-    rep = np.repeat(np.arange(len(q)), n)
-    slot = np.arange(int(n.sum())) - np.repeat(np.cumsum(n) - n, n)
-    v = table[b[rep], slot].astype(np.int64)
-    return (v >> mtb) - 1, (v & ((1 << mtb) - 1)) - q[rep, 0]
-
-
-def _np_rows(table, counts, hashbits, depth, mtb, hpi, q, window, thresh, sdepth, maxalign=100):
-    """Rows [id, count, dtime, raw, rank, 0, 0] in rank order (not sorted by count)."""
-    ids, dts = _np_hits(table, counts, hashbits, depth, mtb, q)
-    if len(ids) == 0:
-        return np.zeros((0, 7), np.int32)
-    uid, raw = np.unique(ids, return_counts=True)
-    order = np.argsort(raw / hpi[uid].astype(float), kind="stable")[::-1]
-    order = order[:min(int(np.count_nonzero(raw > thresh)), sdepth)]
-    by_id = np.argsort(ids, kind="stable")
-    sid, sdt = ids[by_id], dts[by_id]
-    rows = []
-    for rank, k in enumerate(order):
-        id_, r = int(uid[k]), int(raw[k])
-        lo, hi = np.searchsorted(sid, [id_, id_ + 1])
-        d = sdt[lo:hi]
-        tmin = int(d.min())
-        bc = np.bincount(d - tmin)
-        lm = np.where(orc.local_max_mask(bc), bc, 0)
-        found = 0
-        while True:
-            mode = int(np.argmax(lm))
-            if lm[mode] <= thresh:
-                break
-            a, b = max(0, mode - window), mode + window + 1
-            rows.append([id_, int(bc[a:b].sum()), mode + tmin, r, rank, 0, 0])
-            lm[a:b] = 0
-            found += 1
-            if found > maxalign:
-                break
-    return np.array(rows, np.int32).reshape(-1, 7)
-
-
-def _by_count(rows):
-    return rows[np.argsort(-rows[:, 1], kind="stable")]
 
 
 def _table(hashbits, depth, mtb, tracks):
