@@ -7,9 +7,13 @@
 //   out[n]  = sum_j taps[n*down + half - j*up] * mono[j]                   (polyphase FIR, zero phase)
 // with the `up`-scaled Kaiser-windowed low-pass `taps` (2*half + 1 coefficients) computed by the
 // host in float64 exactly as scipy.signal.resample_poly designs it; len(out) = ceil(n*up/down).
-// ffmpeg's resampler is not reproducible bit for bit by any other implementation, so - as §8f-2
-// says - this row is pinned by tolerance against scipy.signal.resample_poly (tests/test_gpu_pcm.py),
-// and every parity statement on fingerprints is made on 11025 Hz PCM.
+// The channel sum is exact in float32 (ch <= 512), so mono[j] is rounded once.  The FIR sums in
+// float64, whose error (about m 2^-53 sum|t x| for m terms) is far below half a float32 ulp, so
+// out[n] is the correctly rounded float32 of the exact sum except in a tie zone where that sum lies
+// within the error bound of a rounding boundary.  tests/test_gpu_pcm_exact.py holds every output to
+// that bar against the extended-precision statement of tests/exact_resample.py, which
+// scipy.signal.resample_poly cross-checks on the CPU.  ffmpeg's resampler, which the reference uses,
+// is not reproduced (§8f-2); parity statements against the reference are made on 11025 Hz PCM.
 #include "afp_internal.cuh"
 
 namespace {

@@ -115,7 +115,14 @@ int afp_get_stage_ms(afp_ctx* ctx, float* ms /* [AFP_NSTAGES] */);
  * (2*half+1 doubles, already scaled by `up`; the host designs them as
  * scipy.signal.resample_poly does).  up = down = 1: down-mix only (taps may be NULL).
  * *nout = ceil(nframes*up/down) samples are written to `out` (HOST or DEVICE float32).
- * Tolerance-pinned, not bit-pinned: no two resamplers agree bit for bit (SURVEY.md 8f-2). */
+ * Each output is the correctly rounded float32 of
+ *   out[n] = sum_j taps[n*down + half - j*up] * RN32(sum_c pcm[j][c] / (32768 channels)),
+ * except in a tie zone where the exact sum lies within the float64 accumulation's error bound of a
+ * float32 rounding boundary (there: within 1 ulp).  Held to an extended-precision statement of that
+ * sum (tests/exact_resample.py), with scipy.signal.resample_poly as its CPU cross-check.  ffmpeg's
+ * resampler, which the reference uses, is not reproduced (SURVEY.md 8f-2).
+ * AFP_ERR_INVALID for nframes < 0, channels < 1, up or down < 1, a resampling call without an
+ * odd-length `taps`, or NULL pcm/out with nframes > 0; nframes = 0 gives *nout = 0. */
 int afp_pcm_frontend(afp_ctx* ctx, const int16_t* pcm, int pcm_on_host, int64_t nframes, int32_t channels,
                      int32_t up, int32_t down, const double* taps, int32_t ntaps, float* out, int out_on_host,
                      int64_t* nout);

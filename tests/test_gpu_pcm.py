@@ -1,6 +1,8 @@
-"""The device PCM front-end (csrc/afp_pcm.cu, SURVEY.md §8f-2): down-mix + polyphase resampling,
-pinned by TOLERANCE against scipy.signal.resample_poly (the reference delegates this step to
-ffmpeg, audio_read.py:196-203, whose resampler no other implementation reproduces bit for bit)."""
+"""The device PCM front-end (csrc/afp_pcm.cu, SURVEY.md §8f-2): down-mix + polyphase resampling
+against scipy.signal.resample_poly, and through the WAV reader to fingerprints.  The reference
+delegates this step to ffmpeg (audio_read.py:196-203), whose resampler no other implementation
+reproduces bit for bit; the front-end's own output is held to its correctly rounded statement at
+every sample by tests/test_gpu_pcm_exact.py."""
 import wave
 
 import numpy as np
@@ -10,6 +12,8 @@ from scipy.signal import resample_poly
 from audfprint_b200 import Analyzer
 from audfprint_b200 import analyzer as an_mod
 from audfprint_b200.synth import synth_track
+from oracle import afp_oracle as orc
+from tests.exact_resample import TARGET, check_rounded, downmix, reference, up_down
 
 pytestmark = pytest.mark.gpu
 
@@ -40,26 +44,36 @@ def test_frontend_matches_resample_poly(fs, nch):
     assert len(an_mod.pcm_frontend(raw[:0], nch, fs, 11025)) == 0
 
 
-def test_wav_reader_and_file_level_api(tmp_path):
-    """A stereo 44.1 kHz WAV of a known track: read (device down-mix + resample), fingerprint,
-    and compare with fingerprinting the host statement of the same front-end."""
-    fs = 44100
+def _file_level_api(tmp_path, fs, nch):
+    """A WAV of a known track at fs with nch channels: read (device down-mix + resample) and
+    fingerprint.  The samples are the correctly rounded front-end statement of tests/exact_resample.py
+    (its tie zone is empty on this file), so the hashes equal the oracle's on those samples bit for bit."""
     mono11 = synth_track(4242, 8.0)
-    up = resample_poly(mono11.astype(np.float64), 4, 1)
-    stereo = np.stack([up * 0.9, up * 0.7], axis=1).clip(-32768, 32767).astype(np.int16)
+    up_fs, down_fs = up_down(TARGET, fs)
+    x = resample_poly(mono11.astype(np.float64), up_fs, down_fs)
+    pcm = np.stack([x * g for g in (0.8, 0.7)[:nch]], axis=1).clip(-32768, 32767).astype(np.int16)
     fn = str(tmp_path / "s.wav")
     with wave.open(fn, "wb") as w:
-        w.setnchannels(2); w.setsampwidth(2); w.setframerate(fs)
-        w.writeframes(stereo.tobytes())
-    d, sr = an_mod._wav_reader(fn, sr=11025, channels=1)
-    want = _host_statement(stereo.reshape(-1), 2, fs, 11025)
-    assert sr == 11025 and d.dtype == np.float32 and len(d) == len(want)
-    assert np.max(np.abs(d - want)) < 2e-6
+        w.setnchannels(nch); w.setsampwidth(2); w.setframerate(fs)
+        w.writeframes(pcm.tobytes())
+    d, sr = an_mod._wav_reader(fn, sr=TARGET, channels=1)
+    up, down = up_down(fs, TARGET)
+    ref, S, m = reference(downmix(pcm, nch), up, down)
+    assert sr == TARGET and d.dtype == np.float32 and len(d) == len(ref)
+    assert check_rounded(d, ref, S, m, "%d Hz x %d WAV" % (fs, nch)) == 0
+    want = ref.astype(np.float32)
+    assert np.array_equal(d, want)
     d2, sr2 = an_mod._wav_reader(fn)                      # no target rate: native rate, still mono
-    assert sr2 == fs and len(d2) == len(stereo)
+    assert sr2 == fs and np.array_equal(d2, downmix(pcm, nch))
     an = Analyzer()
     h = an.wavfile2hashes(fn)
-    h_want = an.fingerprint_batch([want])[0]
-    # identical samples up to 2e-6 -> practically the same landmarks (not a bit-parity claim)
-    a, b = set(map(tuple, h.tolist())), set(map(tuple, h_want.tolist()))
-    assert len(a & b) / max(1, len(a | b)) > 0.97 and abs(an.soundfiledur - 8.0) < 0.01
+    assert np.array_equal(h, orc.fingerprint(want)) and abs(an.soundfiledur - 8.0) < 0.01
+
+
+def test_wav_reader_and_file_level_api(tmp_path):
+    _file_level_api(tmp_path, 44100, 2)
+
+
+@pytest.mark.parametrize("nch", [1, 2])
+def test_wav_reader_and_file_level_api_48k(tmp_path, nch):
+    _file_level_api(tmp_path, 48000, nch)
