@@ -21,7 +21,9 @@
 //      implementation of CPython's MT19937 / _randbelow, afp_mt_randint_replay below) and sends
 //      back the resulting (bucket, slot, value) patches.
 // With the same RNG state the device table is therefore bit-identical to what the reference's
-// store() builds (tests/test_gpu_store.py, against the reference-pinned host store()).
+// store() builds (tests/test_gpu_store.py, against the reference-pinned host store();
+// tests/test_gpu_table_edges.py, against the sequential statement of tests/table_reference.py at
+// the LIGHT / SCAP / SB edges, the scan carry, the masks and the last-writer scratch).
 #include <algorithm>
 #include "afp_internal.cuh"
 

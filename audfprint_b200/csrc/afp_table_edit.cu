@@ -16,6 +16,10 @@
 // exclusive scan over the buckets gives every bucket its output segment; the entries are written
 // as (time, hash) in (hash, slot) order with their request index as key; a stable radix sort by
 // that key groups them per requested id without changing that order.
+//
+// Tests: tests/test_gpu_table_edit.py (the reference's table-ops fixture, the host methods, the bench
+// geometry); tests/test_gpu_table_edges.py (the sequential statement of tests/table_reference.py at
+// depths around the 32-slot chunks, bitmap word edges, 2^k / 2^k + 1 distinct ids, 2^21 buckets).
 #include <algorithm>
 #include <unordered_map>
 #include <cub/cub.cuh>

@@ -248,8 +248,9 @@ class HashTable(object):
             raise AfpStateError("the device copy is a shard (restrict_device_ids): cannot store into it")
         if getattr(self, "_store_pending", False):
             raise AfpStateError("store_batch_begin: the previous batch was not finished")
+        plan = self._plan_ids(names)              # an integer id outside the names raises here, nothing changed
         ctx = self._sync_device()                 # the device holds this table's current state
-        ids = self._names_to_ids(names)           # (host bookkeeping; the device copy stays the current one)
+        ids = self._take_ids(plan)                # (host bookkeeping; the device copy stays the current one)
         nov = C.c_int64(0)
         if hashes is None:
             roff = np.empty(nfiles + 1, np.int64)
@@ -282,55 +283,70 @@ class HashTable(object):
             return []
         ctx, ids, roff, cnt = token
         n = len(cnt)
-        if n:
-            # overflow entries: random.randint(0, count) is replayed for each, in sequence, on a C
-            # copy of CPython's generator; the drawn slots go back and the device applies them (the
-            # last entry of a slot wins, as in the reference's sequential loop)
-            st = random.getstate()
-            state = np.array(st[1], dtype=np.uint32)
-            slot = np.empty(n, np.int32)
-            ctx.check(ctx.lib.afp_mt_randint_replay(state.ctypes.data, cnt.ctypes.data, n, slot.ctypes.data))
-            random.setstate((st[0], tuple(state.tolist()), st[2]))
-            ctx.check(ctx.lib.afp_table_apply_slots(ctx.h, slot.ctypes.data, n))
-        per_track = np.diff(roff)
-        np.add.at(self.__dict__["_hashesperid"], ids, per_track.astype(np.uint32))
-        hpi = np.ascontiguousarray(self.hashesperid, dtype=np.uint32)
-        ctx.check(ctx.lib.afp_table_set_hashesperid(ctx.h, hpi.ctypes.data if len(hpi) else None, len(hpi)))
-        self._store_pending = False
+        try:
+            if n:
+                # overflow entries: random.randint(0, count) is replayed for each, in sequence, on a C
+                # copy of CPython's generator; the drawn slots go back and the device applies them (the
+                # last entry of a slot wins, as in the reference's sequential loop)
+                st = random.getstate()
+                state = np.array(st[1], dtype=np.uint32)
+                slot = np.empty(n, np.int32)
+                ctx.check(ctx.lib.afp_mt_randint_replay(state.ctypes.data, cnt.ctypes.data, n, slot.ctypes.data))
+                random.setstate((st[0], tuple(state.tolist()), st[2]))
+                ctx.check(ctx.lib.afp_table_apply_slots(ctx.h, slot.ctypes.data, n))
+            per_track = np.diff(roff)
+            np.add.at(self.__dict__["_hashesperid"], ids, per_track.astype(np.uint32))
+            hpi = np.ascontiguousarray(self.hashesperid, dtype=np.uint32)
+            ctx.check(ctx.lib.afp_table_set_hashesperid(ctx.h, hpi.ctypes.data if len(hpi) else None, len(hpi)))
+        finally:
+            self._store_pending = False       # a failed finish must not lock the table against every later edit
         self._touch()
         ctx.table_key = self._dev_key = self._stamp()      # the device copy IS this version
         return [int(x) for x in per_track]
 
-    def _names_to_ids(self, names):
+    def _plan_ids(self, names):
         """name_to_id(name, add_if_missing=True) (hash_table.py:325-345) for a list of names, without
-        the per-name list search: a known name keeps its id, a new one takes the first freed slot,
-        else the end of the list."""
+        the per-name list search and without changing anything yet (_take_ids applies the result): a
+        known name keeps its id, a new one takes the first freed slot, else the end of the list.  An
+        integer id must name a track that exists at its place in the sequence, as hashesperid[id]
+        does in the reference's store(); otherwise IndexError."""
         known = {}
         for i, n in enumerate(self.names):
             if n is not None and n not in known:
                 known[n] = i
         free = [i for i, n in enumerate(self.names) if n is None]
         free.reverse()
+        nids = len(self.names)
         ids = np.empty(len(names), np.int64)
-        hpi = self.__dict__["_hashesperid"]
-        grown = []
+        reused, grown = [], []
         for k, name in enumerate(names):
             if not isinstance(name, (str, bytes)):
-                ids[k] = name
+                i = int(name)
+                if not 0 <= i < nids + len(grown):
+                    raise IndexError("track id %d outside [0, %d)" % (i, nids + len(grown)))
+                ids[k] = i
                 continue
             i = known.get(name)
             if i is None:
                 if free:
                     i = free.pop()
-                    self.names[i] = name
-                    hpi[i] = 0
+                    reused.append((i, name))
                 else:
-                    i = len(self.names)
-                    self.names.append(name)
-                    grown.append(0)
+                    i = nids + len(grown)
+                    grown.append(name)
                 known[name] = i
             ids[k] = i
+        return ids, reused, grown
+
+    def _take_ids(self, plan):
+        """Enter the new names of a _plan_ids result; returns the ids."""
+        ids, reused, grown = plan
+        hpi = self.__dict__["_hashesperid"]
+        for i, name in reused:
+            self.names[i] = name
+            hpi[i] = 0
         if grown:
+            self.names.extend(grown)
             self.hashesperid = np.concatenate([hpi, np.zeros(len(grown), np.uint32)]).astype(np.uint32)
         return ids
 
