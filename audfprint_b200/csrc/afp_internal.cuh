@@ -135,6 +135,9 @@ struct afp_ctx {
   int64_t rt_total = -1;              // rows of the last afp_table_retrieve_ids; -1 = none
   int rt_src = 0;                     // where they are: 0 d_ed_val, 1 d_ed_val2, 2 d_ed_rows
   std::vector<int64_t> h_rt_off;      // [n+1] row offsets per requested id
+  // device-side HashTable.merge (afp_table_merge.cu): incoming rows + counts, per-bucket flags and
+  // pool sizes, their scan, overflowing buckets + pool sizes, one chunk's pool indices and new rows
+  DevBuf d_mg_in, d_mg_flag, d_mg_off, d_mg_bkt, d_mg_idx, d_mg_row;
   DevBuf d_mfast, d_mqlist;    // fast path: member-hit lists; [count + pad][query list] handed to the general kernel
   int64_t match_general = 0;   // queries of the last batch the general kernel processed
   int match_general_h = 0;

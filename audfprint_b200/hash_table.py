@@ -9,8 +9,8 @@ time) runs on the GPU against a lazily refreshed device copy.  `store` exists
 twice: per track on the host, and batched on the device (`store_batch`,
 SURVEY.md §8f-1: the device copy then leads and the host arrays refresh from it
 when read).  `remove` and `retrieve` also exist batched on the device (`remove_batch`,
-`retrieve_batch`), which the per-name forms use while the device copy leads; `merge` is
-host bookkeeping.  All of them reproduce the
+`retrieve_batch`), which the per-name forms use while the device copy leads.  `merge` runs on
+the host; `merge_batch` merges a list of tables on the device.  All of them reproduce the
 reference's results exactly, including its draws from the global `random` /
 `np.random` generators on bucket overflow.
 """
@@ -479,6 +479,77 @@ class HashTable(object):
         ctx.check(ctx.lib.afp_fetch_retrieved(ctx.h, rows.ctypes.data if len(rows) else None, 1,
                                               off.ctypes.data_as(C.POINTER(C.c_int64))))
         return [rows[off[k]:off[k + 1]] for k in range(len(ids))]
+
+    def merge_batch(self, tables):
+        """HashTable.merge (hash_table.py:291-323) of a list of tables, on the device table.
+
+        Leaves table, counts, names, hashesperid, `dirty` and the np.random state as
+        `for t in tables: self.merge(t)` does (`random` is not used).  Each incoming table's host
+        arrays are read first (a table whose device copy leads pulls it), then the merges run on
+        this table's device copy: buckets whose pool fits are appended in place, the overflowing
+        ones are drawn by a C replay of np.random.permutation on the host, chunk by chunk while
+        the device applies the previous chunk.  Afterwards the DEVICE copy is the current one (as
+        after store_batch).
+        The whole list is checked before anything changes: AssertionError for another maxtimebits,
+        IndexError for a non-zero incoming count outside this table, ValueError for `self` in the
+        list (or a negative count), AfpStateError for a shard device copy or a pending
+        store_batch_begin, and OverflowError when a merged id does not fit in 32 - maxtimebits bits
+        (the rule of store; the host merge instead wraps the shifted entries and writes a corrupt
+        table).  Returns the number of buckets that overflowed."""
+        tables = list(tables)
+        self._check_device_edit("merge_batch")
+        mtb, nb = int(self.maxtimebits), 1 << int(self.hashbits)
+        nnames = len(self.names)
+        plan = []
+        for t in tables:
+            if t is self:
+                raise ValueError("a table cannot be merged into itself")
+            if getattr(t, "_store_pending", False):
+                raise AfpStateError("merge_batch: an incoming table has an unfinished store_batch_begin")
+            if self.maxtimebits != t.maxtimebits:
+                raise AssertionError("tables disagree on maxtimebits (%d vs %d)" % (self.maxtimebits, t.maxtimebits))
+            table = np.ascontiguousarray(t.table, dtype=np.uint32)           # (pulls its device copy if it leads)
+            counts = np.ascontiguousarray(t.counts, dtype=np.int32)
+            if table.shape != (1 << int(t.hashbits), int(t.depth)) or counts.shape != (1 << int(t.hashbits),):
+                raise ValueError("table/counts shapes of an incoming table do not match its hashbits/depth")
+            if (counts < 0).any():
+                raise ValueError("an incoming table has a negative count")
+            outside = np.nonzero(counts[nb:])[0]
+            if len(outside):
+                raise IndexError("bucket %d of an incoming table lies outside this table's %d buckets"
+                                 % (nb + int(outside[0]), nb))
+            if nnames << mtb >= 1 << 32:
+                raise OverflowError("id offset %d does not fit in %d id bits" % (nnames, 32 - mtb))
+            plan.append((t, table, counts, nnames))
+            nnames += len(t.names)
+            if len(t.names) and (nnames + 1) << mtb > 1 << 32:
+                raise OverflowError("id %d does not fit in %d id bits" % (nnames - 1, 32 - mtb))
+        if not plan:
+            return 0
+        ctx = self._sync_device()
+        st = np.random.get_state()
+        state = np.empty(625, np.uint32)
+        state[:624], state[624] = st[1], st[2]
+        novf, total = C.c_int64(0), 0
+        try:
+            for t, table, counts, offset in plan:
+                ctx.check(ctx.lib.afp_table_merge(ctx.h, table.ctypes.data, counts.ctypes.data, int(t.hashbits),
+                                                  int(t.depth), offset, state.ctypes.data, C.byref(novf), None))
+                total += int(novf.value)
+            hpi = np.concatenate([self.hashesperid] + [np.asarray(t.hashesperid) for t, _, _, _ in plan]).astype(np.uint32)
+            ctx.check(ctx.lib.afp_table_set_hashesperid(ctx.h, hpi.ctypes.data if len(hpi) else None, len(hpi)))
+        except BaseException:
+            ctx.table_key = None              # the device copy is neither the old table nor the merged one
+            raise
+        np.random.set_state((st[0], state[:624].copy(), int(state[624]), st[3], st[4]))
+        for t, _, _, _ in plan:
+            self.names += t.names
+        self.__dict__["_hashesperid"] = hpi
+        self._touch()
+        self._dev_newer = True
+        ctx.table_key = self._dev_key = self._stamp()      # the device copy IS this version
+        ctx.table_owner = weakref.ref(self)
+        return total
 
     def _check_device_edit(self, what):
         # a shard stamp left behind after another table took the device is no shard: _sync_device

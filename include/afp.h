@@ -258,6 +258,33 @@ int afp_table_remove_ids(afp_ctx* ctx, const int64_t* ids, int64_t n, int64_t* r
  * HOST int64 [n+1] offsets of every id's block. */
 int afp_table_retrieve_ids(afp_ctx* ctx, const int64_t* ids, int64_t n, int64_t* total_rows);
 int afp_fetch_retrieved(afp_ctx* ctx, int32_t* rows, int rows_on_host, int64_t* row_offsets /* HOST [n+1] */);
+/* HashTable.merge (hash_table.py:291-323) of one incoming table into the device table.
+ *   table, counts  HOST uint32 [2^hashbits][depth] and int32 [2^hashbits] of the incoming table
+ *                  (any hashbits and depth; its maxtimebits must be the device table's)
+ *   id_offset      len(self.names) before this merge: every incoming entry moves up by
+ *                  id_offset << maxtimebits (uint32), which must stay below 2^32
+ *   np_state625    NumPy's legacy MT19937 state, np.random.get_state()[1] (624 words) then [2] (the
+ *                  position); updated in place as the reference's np.random.permutation calls leave it
+ *   noverflow      HOST, may be NULL: number of buckets that overflowed (and drew)
+ *   stage_ms       HOST double [6] or NULL: incoming upload, classify + compaction, host replay,
+ *                  pool-index uploads, apply kernels (CUDA events), wait after the last replay.
+ *                  With stage_ms the upload and the classify step are synchronised to be timed.
+ * For every incoming bucket with a non-zero count, in ascending order: pool = our first
+ * min(count, depth) entries then its first min(count, its depth) shifted entries; a pool of at most
+ * `depth` entries is written from slot 0 (later slots keep their values) and becomes the count; a
+ * larger one gets table[b] = np.random.permutation(pool)[:depth] and counts[b] += its count (raw).
+ * AFP_ERR_INDEX when a non-zero count of the incoming table lies outside the device table,
+ * AFP_ERR_INVALID for a negative incoming count; both are found before anything changes.  The
+ * device hashesperid is not touched and the pruning bound is 0 (no pruning) until
+ * afp_table_set_hashesperid uploads the merged one. */
+int afp_table_merge(afp_ctx* ctx, const uint32_t* table, const int32_t* counts, int32_t hashbits, int32_t depth,
+                    int64_t id_offset, uint32_t* np_state625, int64_t* noverflow, double* stage_ms);
+/* np.random.permutation of n pools (hash_table.py:291-323, the draws of HashTable.merge), replayed
+ * on index arrays: out (HOST int32 [n][keep]) receives the first `keep` entries of the permutation of
+ * 0..pool_sizes[i]-1 that RandomState.permutation would return for a pool of that size, the pools in
+ * order from the state state625 (as in afp_table_merge), which is advanced in place.  Host
+ * arithmetic only.  AFP_ERR_INVALID, state unchanged, for keep < 1 or a pool size below keep. */
+int afp_np_permutation_replay(uint32_t* state625, const int32_t* pool_sizes, int64_t n, int32_t keep, int32_t* out);
 /* The fast matching kernel's pruning bound of the device table: its smallest non-zero hashesperid,
  * or 0 (no pruning) when no id has hashes or a live entry names an id whose hashesperid is 0.
  * Recomputed by every call that changes hashesperid (upload, set_hashesperid, remove_ids). */
