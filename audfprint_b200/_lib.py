@@ -89,6 +89,9 @@ _SIGS = {
     "afp_fetch_match_candidates": (C.c_int, [_P, _P, _P, C.c_int]),
     "afp_match_options_batch": (C.c_int, [_P, _P, C.c_int, C.c_int32, _I64P, C.POINTER(MatcherParams), C.c_int32,
                                           C.c_int32, C.c_double, _I64P, _I64P]),
+    "afp_match_options_shard_rank": (C.c_int, [_P, _P, C.c_int, C.c_int32, _I64P, C.POINTER(MatcherParams),
+                                               C.c_int32, C.c_int32, C.c_double, _I64P, _P, _I64P]),
+    "afp_match_options_shard_finish": (C.c_int, [_P, _P, _I64P]),
 }
 
 _lib = None

@@ -157,6 +157,20 @@ struct afp_ctx {
   // exact_count / find_time_range finish (afp_match_options.cu): per-slot segments and lookup,
   // routed hits, approximate-row flags, mode supports, packed keys, qtimes, CUB temp, finished rows
   DevBuf d_op_slot, d_op_hit, d_op_mode, d_op_sup, d_op_key, d_op_tq, d_op_cub, d_op_rows;
+  // the same finish on one shard of an id-range sharded table, in two calls around the caller's
+  // all-reduce of the per-query largest qtime: what the ranking call leaves for the finish call,
+  // and the smallest local rank per query whose quantile read failed (0x7f7f7f7f: none)
+  struct {
+    bool pending = false;        // afp_match_options_shard_rank ran; its finish has not
+    bool finished = false;       // the last result is a shard finish: afp_shard_pack packs it
+    afp_matcher_params p{};
+    int32_t nq = 0, exact = 0, trange = 0;
+    int64_t nrows = 0, ranked = 0;
+    double quant = 0.0;
+    int64_t breaks[32] = {};
+    const int32_t* dq = nullptr;
+  } sopt;
+  DevBuf d_op_qfail;
 };
 
 #define AFP_CUDA(ctx, call)                                                        \

@@ -702,6 +702,7 @@ int afp_match_batch(afp_ctx* c, const int32_t* q_rows, int q_on_host, int32_t nq
   c->match_total_rows = -1;
   c->match_nq = nqueries;
   c->match_long.clear();
+  c->sopt.pending = c->sopt.finished = false;
   // A query of rows * depth >= AFP_LONG_HITS takes the long-query path (afp_match_long.cu) unless
   // force_general is set; the rule depends on the query and the table only.  The fast and general
   // kernels' scratch is sized over the other queries.

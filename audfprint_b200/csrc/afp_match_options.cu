@@ -24,6 +24,11 @@
 // window + 1 exact-count supports (modes are at least two bins apart) and in at most 2 approximate
 // ones - plus O(nqueries * search_depth); nothing is sized by rows x depth.  Every result is read
 // from sorted data, so nothing depends on the order of the probe's atomics.
+//
+// A shard of an id-range sharded table runs the same finish in two calls around the caller's
+// all-reduce (MAX) of each query's largest qtime (afp_match_options_shard_rank / _finish): every
+// published candidate is finished (the merge keeps global ranks < D), the key width comes from the
+// reduced maximum, and a failed quantile read is recorded per query for the merge (afp_shard.cu).
 #include <math.h>
 #include <algorithm>
 #include <cub/cub.cuh>
@@ -55,12 +60,16 @@ __device__ __forceinline__ int64_t bound(const T* v, int64_t lo, int64_t hi, lon
   return lo;
 }
 
-__device__ __forceinline__ int depth_of(const int32_t* cnt, int qi, int sd) {
-  return max(0, min(min(cnt[2 * qi + 1], sd), cnt[2 * qi]));
+// candidates finished per query: a whole table reaches rank min(n_above, search_depth) (:139-146);
+// a shard of an id-range sharded table finishes every candidate it publishes, because one of its
+// ids can be inside the global top-D while at or past the shard's own n_above (the merge drops
+// the rows of global rank >= D)
+__device__ __forceinline__ int depth_of(const int32_t* cnt, int qi, int sd, int shard) {
+  return max(0, min(shard ? sd : min(cnt[2 * qi + 1], sd), cnt[2 * qi]));
 }
 
 // 1. per (query, rank) slot: segment length, lookup key (id, or ~0 when not routed) and rank
-__global__ void opt_slots_kernel(const double* cand, const int32_t* cnt, int nq, int sd, int thresh,
+__global__ void opt_slots_kernel(const double* cand, const int32_t* cnt, int nq, int sd, int thresh, int shard,
                                  int64_t* seglen, uint32_t* lkey, int32_t* lval, int32_t* loff, int* qmax) {
   const int64_t n = (int64_t)nq * sd;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += (int64_t)gridDim.x * blockDim.x) {
@@ -71,7 +80,7 @@ __global__ void opt_slots_kernel(const double* cand, const int32_t* cnt, int nq,
     bool routed = false;
     int raw = 0;
     uint32_t id = 0xffffffffu;
-    if (j < depth_of(cnt, qi, sd)) {
+    if (j < depth_of(cnt, qi, sd, shard)) {
       raw = (int)cand[3 * i + 1];
       routed = raw >= max(thresh, 1);          // find_modes keeps bins >= threshcount (:78-90)
       if (routed) id = (uint32_t)cand[3 * i];
@@ -142,11 +151,11 @@ __global__ void opt_modes_kernel(const int32_t* dt, const int32_t* hseg, const i
 
 // 4b. find_time_range alone: flag the approximate rows of rank < depth
 __global__ void opt_rowflags_kernel(const int32_t* rows, int64_t nr, const int64_t* roff, int nq, const int32_t* cnt,
-                                    int sd, int32_t* flag) {
+                                    int sd, int shard, int32_t* flag) {
   for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r <= nr; r += (int64_t)gridDim.x * blockDim.x) {
     if (r == nr) { flag[nr] = 0; continue; }
     const int qi = (int)bound(roff, 0, nq + 1, r, true) - 1;
-    flag[r] = rows[7 * r + 4] < depth_of(cnt, qi, sd) ? 1 : 0;
+    flag[r] = rows[7 * r + 4] < depth_of(cnt, qi, sd, shard) ? 1 : 0;
   }
 }
 
@@ -205,10 +214,13 @@ __device__ __forceinline__ bool py_index(double x, int64_t n, int64_t& i) {
   return true;
 }
 
-// 5c. one warp per mode: distinct keys of its sorted support, the two quantile reads, the row flag
+// 5c. one warp per mode: distinct keys of its sorted support, the two quantile reads, the row flag.
+// A failed quantile read is an error of the call (err), or on a shard (qfail != nullptr) the
+// candidate's local rank, kept per query (the smallest) for the merge to judge
 __global__ void __launch_bounds__(OT) opt_stats_kernel(const int64_t* soff, int nm, const unsigned long long* pk,
-                                                       const int32_t* tq, int thresh, double quant, int32_t* mcnt,
-                                                       int32_t* mtlo, int32_t* mthi, int32_t* keep, int* err) {
+                                                       const int32_t* tq, int thresh, double quant, const int32_t* mslot,
+                                                       int sd, int32_t* mcnt, int32_t* mtlo, int32_t* mthi,
+                                                       int32_t* keep, int* err, int32_t* qfail) {
   const int lane = threadIdx.x & 31;
   const int64_t nwarps = (int64_t)gridDim.x * (OT / 32);
   for (int64_t m = (int64_t)blockIdx.x * (OT / 32) + (threadIdx.x >> 5); m <= nm; m += nwarps) {
@@ -229,6 +241,9 @@ __global__ void __launch_bounds__(OT) opt_stats_kernel(const int64_t* soff, int 
         if (py_index((double)n * quant, n, ilo) && py_index(trunc((double)n * (1.0 - quant)) - 1.0, n, ihi)) {
           mtlo[m] = tq[a + ilo];
           mthi[m] = tq[a + ihi];
+        } else if (qfail) {
+          mtlo[m] = mthi[m] = 0;
+          atomicMin(&qfail[mslot[m] / sd], mslot[m] % sd);
         } else {
           atomicExch(err, 1);
         }
@@ -294,10 +309,14 @@ int read_back(afp_ctx* c, const T* d, T* h, size_t n = 1) {
   return AFP_OK;
 }
 
-// The finish on the ranking afp_match_batch left in the context (publish mode).
+// The finish on the ranking afp_match_batch left in the context (publish mode).  On a shard
+// (qmax_shard != nullptr): every published candidate is finished, the key width comes from the
+// caller's per-query largest qtime over ALL shards, and quantile failures go to qfail.
 int finish_options(afp_ctx* c, const int32_t* dq, int nq, int64_t nrows, int64_t napprox, const afp_matcher_params* p,
-                   int exact, int trange, double quant, const Breaks& br, int64_t* total_out) {
+                   int exact, int trange, double quant, const Breaks& br, const int* qmax_shard, int32_t* qfail,
+                   int64_t* total_out) {
   cudaStream_t st = c->stream;
+  const int shard = qmax_shard ? 1 : 0;
   const int sd = p->search_depth, thresh = p->threshcount, window = p->window;
   const int64_t nslot = (int64_t)nq * sd;
   if (nslot >= ((int64_t)1 << 31)) AFP_FAIL(c, AFP_ERR_UNSUPPORTED, "nqueries * search_depth >= 2^31");
@@ -323,7 +342,7 @@ int finish_options(afp_ctx* c, const int32_t* dq, int nq, int64_t nrows, int64_t
   AFP_CUDA(c, cudaMemsetAsync(cur, 0, sizeof(unsigned) * (size_t)std::max<int64_t>(nslot, 1), st));
   AFP_CUDA(c, cudaMemsetAsync(err, 0, sizeof(int) * 4, st));
   AFP_CUDA(c, cudaMemsetAsync(qcnt, 0, sizeof(unsigned long long) * (size_t)(nq + 1), st));
-  opt_slots_kernel<<<grid_for(nslot + 1, OT), OT, 0, st>>>(cand, cnt, nq, sd, thresh, seglen, lkey, lval, loff, qmax);
+  opt_slots_kernel<<<grid_for(nslot + 1, OT), OT, 0, st>>>(cand, cnt, nq, sd, thresh, shard, seglen, lkey, lval, loff, qmax);
   AFP_CUDA(c, cudaGetLastError());
   c->launches++;
   if ((rc = cub_call(c, [&](void* t, size_t& b) {
@@ -376,7 +395,7 @@ int finish_options(afp_ctx* c, const int32_t* dq, int nq, int64_t nrows, int64_t
     AFP_CUDA(c, c->d_op_mode.reserve(2 * carve_bytes<int32_t>(nsrc + 1)));
     flag = c->d_op_mode.as<int32_t>();
     pos = flag + ((carve_bytes<int32_t>(nsrc + 1)) / sizeof(int32_t));
-    opt_rowflags_kernel<<<grid_for(nsrc + 1, OT), OT, 0, st>>>(approx, nsrc, roff, nq, cnt, sd, flag);
+    opt_rowflags_kernel<<<grid_for(nsrc + 1, OT), OT, 0, st>>>(approx, nsrc, roff, nq, cnt, sd, shard, flag);
   } else {
     opt_modes_kernel<<<grid_for(nsrc + 1, OT), OT, 0, st>>>(dt2, hseg, segoff, nsrc, thresh, flag);
   }
@@ -429,7 +448,8 @@ int finish_options(afp_ctx* c, const int32_t* dq, int nq, int64_t nrows, int64_t
   int32_t* tq = trange ? c->d_op_tq.as<int32_t>() : nullptr;
   int32_t* tq2 = trange ? tq + carve_bytes<int32_t>(ns) / sizeof(int32_t) : nullptr;
   if (ns > 0) {
-    opt_gather_kernel<<<grid_for(ns, OT), OT, 0, st>>>(soff, nm, mlo, mslot, sd, pay2, qmax, br, pk, tq);
+    opt_gather_kernel<<<grid_for(ns, OT), OT, 0, st>>>(soff, nm, mlo, mslot, sd, pay2, shard ? qmax_shard : qmax,
+                                                        br, pk, tq);
     AFP_CUDA(c, cudaGetLastError());
     c->launches++;
     if (exact && (rc = cub_call(c, [&](void* t, size_t& b) {
@@ -442,8 +462,8 @@ int finish_options(afp_ctx* c, const int32_t* dq, int nq, int64_t nrows, int64_t
       return rc;
   }
   // ---- 6. counts, quantiles, rows
-  opt_stats_kernel<<<grid_for(nm + 1, OT / 32), OT, 0, st>>>(soff, nm, pk2, tq2, thresh, quant, mcnt, mtlo, mthi, keep,
-                                                             err + 1);
+  opt_stats_kernel<<<grid_for(nm + 1, OT / 32), OT, 0, st>>>(soff, nm, pk2, tq2, thresh, quant, mslot, sd, mcnt, mtlo,
+                                                             mthi, keep, err + 1, qfail);
   AFP_CUDA(c, cudaGetLastError());
   c->launches++;
   if ((rc = cub_call(c, [&](void* t, size_t& b) {
@@ -474,12 +494,22 @@ int finish_options(afp_ctx* c, const int32_t* dq, int nq, int64_t nrows, int64_t
   return AFP_OK;
 }
 
-}  // namespace
+// a shard's largest query time over the query rows whose bucket is non-empty on it - the rows the
+// probe's atomicMax reads (step 2), so that the maximum over the shards is the whole table's
+__global__ void opt_shard_qmax_kernel(const int32_t* q, int64_t nrows, const int64_t* qoff, int nq,
+                                      const int32_t* counts, int hashbits, int depth, int* qmax) {
+  const uint32_t hmask = (1u << hashbits) - 1u;
+  for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < nrows; r += (int64_t)gridDim.x * blockDim.x) {
+    if (min(depth, counts[(uint32_t)q[2 * r + 1] & hmask]) <= 0) continue;
+    const int qi = (int)bound(qoff, 0, nq + 1, r, true) - 1;
+    atomicMax(&qmax[qi], q[2 * r]);
+  }
+}
 
-extern "C" int afp_match_options_batch(afp_ctx* c, const int32_t* q_rows, int q_on_host, int32_t nqueries,
-                                       const int64_t* q_offsets, const afp_matcher_params* p, int32_t exact_count,
-                                       int32_t find_time_range, double time_quantile, const int64_t* timebits_breaks,
-                                       int64_t* total_rows) {
+// argument checks and the ranking (publish mode) shared by the whole-table and the shard form
+int rank_options(afp_ctx* c, const int32_t* q_rows, int q_on_host, int32_t nqueries, const int64_t* q_offsets,
+                 const afp_matcher_params* p, int32_t exact_count, int32_t find_time_range, double time_quantile,
+                 const int64_t* timebits_breaks, Breaks& br, int64_t* ranked, const int32_t** dq) {
   if (!c || !p || !timebits_breaks) return AFP_ERR_INVALID;
   if ((exact_count != 0 && exact_count != 1) || (find_time_range != 0 && find_time_range != 1) ||
       !(exact_count || find_time_range))
@@ -487,7 +517,6 @@ extern "C" int afp_match_options_batch(afp_ctx* c, const int32_t* q_rows, int q_
   if (!isfinite(time_quantile)) AFP_FAIL(c, AFP_ERR_INVALID, "time_quantile must be finite");
   if (p->window < 0 || p->window > 4096 || p->search_depth < 0 || p->max_alignments_per_id < 0)
     AFP_FAIL(c, AFP_ERR_INVALID, "bad matcher parameters");
-  Breaks br;
   for (int k = 0; k < 32; ++k) {
     br.v[k] = timebits_breaks[k];
     if (br.v[k] < 1 || (k > 0 && br.v[k] < br.v[k - 1]))
@@ -501,21 +530,103 @@ extern "C" int afp_match_options_batch(afp_ctx* c, const int32_t* q_rows, int q_
     rp.max_alignments_per_id = 0;
     rp.row_capacity = std::max(p->row_capacity > 0 ? p->row_capacity : 256, p->search_depth);
   }
-  int64_t ranked = 0;
-  int rc = afp_match_batch(c, q_rows, q_on_host, nqueries, q_offsets, &rp, &ranked);
+  *ranked = 0;
+  int rc = afp_match_batch(c, q_rows, q_on_host, nqueries, q_offsets, &rp, ranked);
   if (rc) return rc;
   const int64_t nrows = nqueries ? q_offsets[nqueries] : 0;
-  const int32_t* dq = (q_on_host && nrows > 0) ? c->d_q.as<int32_t>() : q_rows;
+  *dq = (q_on_host && nrows > 0) ? c->d_q.as<int32_t>() : q_rows;
+  return AFP_OK;
+}
+
+}  // namespace
+
+extern "C" int afp_match_options_batch(afp_ctx* c, const int32_t* q_rows, int q_on_host, int32_t nqueries,
+                                       const int64_t* q_offsets, const afp_matcher_params* p, int32_t exact_count,
+                                       int32_t find_time_range, double time_quantile, const int64_t* timebits_breaks,
+                                       int64_t* total_rows) {
+  Breaks br;
+  int64_t ranked = 0;
+  const int32_t* dq = nullptr;
+  int rc = rank_options(c, q_rows, q_on_host, nqueries, q_offsets, p, exact_count, find_time_range, time_quantile,
+                        timebits_breaks, br, &ranked, &dq);
+  if (rc) return rc;
+  const int64_t nrows = nqueries ? q_offsets[nqueries] : 0;
   int64_t total = 0;
   c->match_total_rows = -1;                 // the approximate rows are not this call's result
   if (nqueries > 0 && p->search_depth > 0) {
-    if ((rc = finish_options(c, dq, nqueries, nrows, ranked, p, exact_count, find_time_range, time_quantile, br, &total)))
+    if ((rc = finish_options(c, dq, nqueries, nrows, ranked, p, exact_count, find_time_range, time_quantile, br,
+                             nullptr, nullptr, &total)))
       return rc;
   } else if (nqueries > 0) {
     AFP_CUDA(c, cudaMemsetAsync(c->d_mrow_off.p, 0, sizeof(int64_t) * (size_t)(nqueries + 1), c->stream));
     AFP_CUDA(c, cudaStreamSynchronize(c->stream));
   }
   c->match_total_rows = total;
+  if (total_rows) *total_rows = total;
+  return AFP_OK;
+}
+
+extern "C" int afp_match_options_shard_rank(afp_ctx* c, const int32_t* q_rows, int q_on_host, int32_t nqueries,
+                                            const int64_t* q_offsets, const afp_matcher_params* p,
+                                            int32_t exact_count, int32_t find_time_range, double time_quantile,
+                                            const int64_t* timebits_breaks, int32_t* qmax_dev, int64_t* ranked_rows) {
+  if (c) c->sopt.pending = c->sopt.finished = false;
+  if (c && nqueries > 0 && !qmax_dev) return AFP_ERR_INVALID;
+  Breaks br;
+  int64_t ranked = 0;
+  const int32_t* dq = nullptr;
+  int rc = rank_options(c, q_rows, q_on_host, nqueries, q_offsets, p, exact_count, find_time_range, time_quantile,
+                        timebits_breaks, br, &ranked, &dq);
+  if (rc) return rc;
+  const int64_t nrows = nqueries ? q_offsets[nqueries] : 0;
+  if (nqueries > 0) {
+    AFP_CUDA(c, cudaMemsetAsync(qmax_dev, 0, sizeof(int32_t) * (size_t)nqueries, c->stream));
+    if (nrows > 0) {
+      opt_shard_qmax_kernel<<<grid_for(nrows, OT), OT, 0, c->stream>>>(
+          dq, nrows, c->d_qoff.as<int64_t>(), nqueries, c->tab.counts.as<int32_t>(), c->tab.hashbits, c->tab.depth,
+          qmax_dev);
+      AFP_CUDA(c, cudaGetLastError());
+      c->launches++;
+    }
+  }
+  AFP_CUDA(c, cudaStreamSynchronize(c->stream));       // qmax is the caller's to all-reduce now
+  c->match_total_rows = -1;                             // nothing to fetch or pack before the finish
+  c->sopt.pending = true;
+  c->sopt.p = *p;
+  c->sopt.nq = nqueries;
+  c->sopt.exact = exact_count;
+  c->sopt.trange = find_time_range;
+  c->sopt.quant = time_quantile;
+  c->sopt.nrows = nrows;
+  c->sopt.ranked = ranked;
+  c->sopt.dq = dq;
+  for (int k = 0; k < 32; ++k) c->sopt.breaks[k] = br.v[k];
+  if (ranked_rows) *ranked_rows = ranked;
+  return AFP_OK;
+}
+
+extern "C" int afp_match_options_shard_finish(afp_ctx* c, const int32_t* qmax_dev, int64_t* total_rows) {
+  if (!c) return AFP_ERR_INVALID;
+  if (!c->sopt.pending) AFP_FAIL(c, AFP_ERR_STATE, "afp_match_options_shard_rank has not been called");
+  c->sopt.pending = false;
+  const int nq = c->sopt.nq;
+  if (nq > 0 && !qmax_dev) return AFP_ERR_INVALID;
+  AFP_CUDA(c, cudaSetDevice(c->device));
+  Breaks br;
+  for (int k = 0; k < 32; ++k) br.v[k] = c->sopt.breaks[k];
+  AFP_CUDA(c, c->d_op_qfail.reserve(sizeof(int32_t) * (size_t)std::max(nq, 1)));
+  AFP_CUDA(c, cudaMemsetAsync(c->d_op_qfail.p, 0x7f, sizeof(int32_t) * (size_t)std::max(nq, 1), c->stream));
+  int64_t total = 0;
+  if (nq > 0 && c->sopt.p.search_depth > 0) {
+    int rc = finish_options(c, c->sopt.dq, nq, c->sopt.nrows, c->sopt.ranked, &c->sopt.p, c->sopt.exact,
+                            c->sopt.trange, c->sopt.quant, br, qmax_dev, c->d_op_qfail.as<int32_t>(), &total);
+    if (rc) return rc;
+  } else if (nq > 0) {
+    AFP_CUDA(c, cudaMemsetAsync(c->d_mrow_off.p, 0, sizeof(int64_t) * (size_t)(nq + 1), c->stream));
+    AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+  }
+  c->match_total_rows = total;
+  c->sopt.finished = true;
   if (total_rows) *total_rows = total;
   return AFP_OK;
 }

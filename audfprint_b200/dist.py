@@ -13,6 +13,9 @@ pickling results back.  The same shape is used here:
   ITS ids, and ONE all-gather of fixed-size per-query records merges them:
   `merge_sharded_results` below is exact because an id inside the global top-D
   (D = min(sum n_above, search_depth)) is inside its own shard's local top-D.
+  With exact_count / find_time_range one all-reduce (MAX) of each query's largest
+  query time comes first, so that every shard packs its (qtime, hash) keys with the
+  whole table's key width; see match_sharded_batch.
 
 Nothing here computes on the CPU; it only moves and merges small result records.
 """
@@ -174,7 +177,16 @@ def match_sharded(matcher, ht, queries, row_cap: int = 16, group=None):
     device table must already be restricted to its id range
     (HashTable.restrict_device_ids(*id_range(nids, rank, world))).  Returns the rows a
     single table gives, on every rank.  Per-query host objects (API convenience; the batch form
-    below is the throughput path)."""
+    below is the throughput path).  With exact_count or find_time_range set the queries go through
+    match_sharded_batch, which finishes them on the device."""
+    if matcher.exact_count or matcher.find_time_range:
+        arrs = [np.asarray(q, dtype=np.int32).reshape(-1, 2) for q in queries]
+        qoff = np.zeros(len(arrs) + 1, np.int64)
+        if arrs:
+            qoff[1:] = np.cumsum([len(a) for a in arrs])
+        packed = np.ascontiguousarray(np.concatenate(arrs)) if arrs else np.zeros((0, 2), np.int32)
+        rows, roff = match_sharded_batch(matcher, ht, (packed, qoff), row_cap, group)
+        return [r[(-r[:, 1]).argsort(), ] for r in (rows[roff[i]:roff[i + 1]] for i in range(len(arrs)))]
     mine = matcher.match_batch_shard(ht, queries)
     shards = allgather_shard_records(mine, matcher.search_depth, row_cap, group)
     out = []
@@ -185,16 +197,28 @@ def match_sharded(matcher, ht, queries, row_cap: int = 16, group=None):
 
 
 # ---- vectorised host statement of pack / merge (tests; checks the device kernels) --------
-def pack_shard_batch(cand, counts, rows, row_off, row_cap: int) -> np.ndarray:
+STATUS_OVERFLOW = 1        # status word (hdr[3]) after an options finish: bit 0 = more rows than row_cap,
+                           # bits 1-30 = 1 + the smallest local rank whose quantile read failed
+
+
+def pack_shard_batch(cand, counts, rows, row_off, row_cap: int, fail_rank=None) -> np.ndarray:
     """The wire records built without a Python loop from what afp_fetch_match_candidates /
     afp_fetch_match_rows return: cand (nq, sd, 3) f64, counts (nq, 2) i32 [entries, n_above],
-    rows (R, 7) i32, row_off (nq+1)."""
+    rows (R, 7) i32, row_off (nq+1).
+
+    fail_rank (nq,) int, -1 = none: the records of an options finish on a shard (what
+    afp_shard_pack writes after afp_match_options_shard_finish).  Then nothing raises: the status
+    word carries the smallest local rank whose quantile read failed and the overflow bit, nrows is
+    the number of rows the shard produced and the record holds the first row_cap of them."""
     nq, sd = cand.shape[0], cand.shape[1]
     nrows = np.diff(row_off)
-    if nq and nrows.max(initial=0) > row_cap:
+    if fail_rank is None and nq and nrows.max(initial=0) > row_cap:
         raise ValueError("a shard produced %d rows for one query, row_cap is %d" % (int(nrows.max()), row_cap))
     out = np.zeros(nq, record_dtype(sd, row_cap))
     out["hdr"][:, 0], out["hdr"][:, 1], out["hdr"][:, 2] = counts[:, 1], counts[:, 0], nrows
+    if fail_rank is not None:
+        fail_rank = np.asarray(fail_rank, np.int64)
+        out["hdr"][:, 3] = np.where(nrows > row_cap, STATUS_OVERFLOW, 0) | np.where(fail_rank >= 0, (fail_rank + 1) << 1, 0)
     valid = np.arange(sd)[None, :] < counts[:, :1]
     out["w"] = np.where(valid, cand[:, :, 2], 0.0)
     out["id"] = np.where(valid, cand[:, :, 0], 0).astype(np.uint32)
@@ -202,8 +226,51 @@ def pack_shard_batch(cand, counts, rows, row_off, row_cap: int) -> np.ndarray:
     if len(rows):
         q = np.repeat(np.arange(nq), nrows)
         k = np.arange(len(rows)) - np.repeat(row_off[:-1], nrows)
-        out["rows"][q, k] = rows
+        held = k < row_cap
+        out["rows"][q[held], k[held]] = rows[held]
     return out
+
+
+def _global_ranks(W, I, ncand, s_idx, q_idx, lr):
+    """Global rank of local rank lr of shard s_idx for query q_idx: the number of published
+    candidates of all shards that order before it by (weight desc, id desc) - one bisection per
+    shard in that shard's already ordered list (in its own shard that number is lr)."""
+    S, sd = W.shape[0], W.shape[2]
+    w_x = W[s_idx, q_idx, lr][:, None]
+    i_x = I[s_idx, q_idx, lr][:, None]
+    shard = np.arange(S)[None, :]
+    lo = np.zeros((len(lr), S), np.int64)
+    hi = ncand[:, q_idx].T.copy()                                                             # (n, S)
+    for _ in range(int(sd).bit_length()):
+        active = lo < hi
+        mid = (lo + hi) >> 1
+        at = np.minimum(mid, sd - 1)
+        w = W[shard, q_idx[:, None], at]
+        before = (w > w_x) | ((w == w_x) & (I[shard, q_idx[:, None], at] > i_x))
+        lo = np.where(active & before, mid + 1, lo)
+        hi = np.where(active & ~before, mid, hi)
+    return lo.sum(axis=1)
+
+
+def check_shard_status(gathered: np.ndarray, search_depth: int = None):
+    """The merge's reading of the status words of all shards' records (afp_shard_merge): IndexError
+    if a failed quantile read lies at a global rank < D (the single table reaches that candidate
+    too), else ValueError naming the largest row count of an overflowed record."""
+    st = gathered["hdr"][:, :, 3].astype(np.int64)
+    if not st.any():
+        return
+    sd = gathered.dtype["w"].shape[0]
+    depth = np.minimum(gathered["hdr"][:, :, 0].sum(axis=0), sd if search_depth is None else search_depth)
+    s_idx, q_idx = np.nonzero((st >> 1) > 0)
+    if len(s_idx):
+        g = _global_ranks(gathered["w"], gathered["id"].astype(np.int64), gathered["hdr"][:, :, 1].astype(np.int64),
+                          s_idx, q_idx, (st[s_idx, q_idx] >> 1) - 1)
+        if np.any(g < depth[q_idx]):
+            raise IndexError("time_quantile index outside a support (IndexError)")
+    over = (st & STATUS_OVERFLOW) != 0
+    if over.any():
+        raise ValueError("row capacity: a shard produced %d rows for one query, row_cap is %d"
+                         % (int(gathered["hdr"][:, :, 2][over].max()), gathered.dtype["rows"].shape[0]))
 
 
 def merge_shard_batch(gathered: np.ndarray, search_depth: int = None, row_cap: int = None):
@@ -214,6 +281,7 @@ def merge_shard_batch(gathered: np.ndarray, search_depth: int = None, row_cap: i
     No sort of the merged candidate lists: only ids that produced rows need a global rank, and
     the rank of id x is the number of published candidates that order before it by (weight desc,
     id desc) - found by one bisection per (row, shard) in that shard's already ordered list."""
+    check_shard_status(gathered, search_depth)
     S, nq = gathered.shape
     sd = gathered.dtype["w"].shape[0]
     rcap = gathered.dtype["rows"].shape[0]
@@ -225,20 +293,7 @@ def merge_shard_batch(gathered: np.ndarray, search_depth: int = None, row_cap: i
     if len(q_idx) == 0:
         return np.zeros((0, 7), np.int32), np.zeros(nq + 1, np.int64)
     r = gathered["rows"][s_idx, q_idx, k_idx].astype(np.int64)                                 # (R0, 7)
-    w_x = W[s_idx, q_idx, r[:, 4]][:, None]          # column 4 = rank in the shard's own list
-    i_x = r[:, :1]
-    shard = np.arange(S)[None, :]
-    lo = np.zeros((len(r), S), np.int64)
-    hi = ncand[:, q_idx].T.copy()                                                             # (R0, S)
-    for _ in range(int(sd).bit_length()):
-        active = lo < hi
-        mid = (lo + hi) >> 1
-        at = np.minimum(mid, sd - 1)
-        w = W[shard, q_idx[:, None], at]
-        before = (w > w_x) | ((w == w_x) & (I[shard, q_idx[:, None], at] > i_x))
-        lo = np.where(active & before, mid + 1, lo)
-        hi = np.where(active & ~before, mid, hi)
-    pos = lo.sum(axis=1)
+    pos = _global_ranks(W, I, ncand, s_idx, q_idx, r[:, 4])      # column 4 = rank in the shard's own list
     keep = pos < depth[q_idx]
     r, q_idx, pos, k_idx = r[keep], q_idx[keep], pos[keep], k_idx[keep]
     r[:, 4] = pos
@@ -257,7 +312,16 @@ def match_sharded_batch(matcher, ht, packed_queries, row_cap: int = 16, group=No
     the record buffers (torch.distributed: NCCL device-to-device; under gloo the bytes take the
     host route), merge (afp_shard_merge).  Returns (rows, offsets): the rows a single table gives,
     in candidate-rank order per query (what Matcher.match_batch(sort=False) returns); with
-    fetch=False the result stays on the device (None, None)."""
+    fetch=False the result stays on the device (None, None).
+
+    With matcher.exact_count / find_time_range (time_quantile) the shard is finished before the
+    pack, in two calls around one all-reduce (MAX) of one int32 per query - the query's largest
+    qtime, which sets the width of the (qtime, hash) keys the exact count compares
+    (audfprint_match.py:157-167) and must be the whole table's: afp_match_options_shard_rank,
+    the all-reduce (NCCL in place; gloo through host memory), afp_match_options_shard_finish.
+    Nothing data-dependent raises between the collectives; the merge raises the same error on every
+    rank: IndexError when a quantile index leaves its support at a candidate the single table
+    finishes, ValueError when a shard produced more than row_cap rows for a query."""
     import ctypes as C
     import torch
     from . import _lib
@@ -270,11 +334,28 @@ def match_sharded_batch(matcher, ht, packed_queries, row_cap: int = 16, group=No
     p = matcher._params()
     p.publish_candidates = 1
     ctx = ht._sync_device()
-    matcher._run(ctx, p, qrows, nq, qoff)
+    options = bool(matcher.exact_count or matcher.find_time_range)
     rb = int(ctx.lib.afp_shard_record_bytes(sd, int(row_cap)))
     if rb < 0:
         raise ValueError("row_cap must be even and >= 2")
     dev = torch.device("cuda", ctx.device)
+    rank, ws = world()
+    if not options:
+        matcher._run(ctx, p, qrows, nq, qoff)
+    else:
+        qmax = torch.empty(max(nq, 1), dtype=torch.int32, device=dev)      # written by the ranking call
+        matcher._run(ctx, p, qrows, nq, qoff, (matcher.exact_count, matcher.find_time_range, matcher.time_quantile),
+                     shard_qmax=qmax.data_ptr())
+        if ws > 1:
+            import torch.distributed as dist
+            if dist.get_backend(group) == "nccl":
+                dist.all_reduce(qmax, op=dist.ReduceOp.MAX, group=group)
+            else:                                # gloo: through host memory
+                h = qmax.cpu()
+                dist.all_reduce(h, op=dist.ReduceOp.MAX, group=group)
+                qmax.copy_(h)
+            torch.cuda.current_stream(dev).synchronize()
+        ctx.check(ctx.lib.afp_match_options_shard_finish(ctx.h, C.c_void_p(qmax.data_ptr()), None))
     mine = torch.empty((max(nq, 1), rb), dtype=torch.uint8, device=dev)
     try:
         ctx.check(ctx.lib.afp_shard_pack(ctx.h, int(row_cap), mine.data_ptr()))
@@ -282,7 +363,6 @@ def match_sharded_batch(matcher, ht, packed_queries, row_cap: int = 16, group=No
         if "row capacity" in str(e):
             raise ValueError("a shard produced more than row_cap=%d rows for one query" % row_cap)
         raise
-    rank, ws = world()
     if ws == 1:
         gathered = mine
     else:

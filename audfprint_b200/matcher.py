@@ -71,10 +71,12 @@ class Matcher(object):
                                   1 if getattr(self, "force_general_kernel", False) else 0)
 
     @staticmethod
-    def _run(ctx, p, packed, nq, qoff, options=None):
+    def _run(ctx, p, packed, nq, qoff, options=None, shard_qmax=None):
         """afp_match_batch - or afp_match_options_batch with options = (exact_count,
         find_time_range, time_quantile) - growing the per-query row capacity of the approximate
-        rows when a query overflows it."""
+        rows when a query overflows it.  With shard_qmax (the address of a device int32
+        [nq]) the options call is afp_match_options_shard_rank instead: the ranking of one shard,
+        whose finish waits for the all-reduce of shard_qmax."""
         total = C.c_int64(0)
         cap = 256
         ptr, on_host = _lib.ptr_of(packed) if len(packed) else (None, 1)     # NumPy (host) or torch CUDA tensor
@@ -88,9 +90,13 @@ class Matcher(object):
                     ctx.check(ctx.lib.afp_match_batch(ctx.h, ptr, on_host, nq, qp, C.byref(p), C.byref(total)))
                 else:
                     exact, trange, quant = options
-                    ctx.check(ctx.lib.afp_match_options_batch(
-                        ctx.h, ptr, on_host, nq, qp, C.byref(p), int(bool(exact)), int(bool(trange)), float(quant),
-                        breaks.ctypes.data_as(C.POINTER(C.c_int64)), C.byref(total)))
+                    args = (ctx.h, ptr, on_host, nq, qp, C.byref(p), int(bool(exact)), int(bool(trange)), float(quant),
+                            breaks.ctypes.data_as(C.POINTER(C.c_int64)))
+                    if shard_qmax is None:
+                        ctx.check(ctx.lib.afp_match_options_batch(*args, C.byref(total)))
+                    else:
+                        ctx.check(ctx.lib.afp_match_options_shard_rank(*args, C.c_void_p(shard_qmax),
+                                                                       C.byref(total)))
                 return int(total.value)
             except _lib.RowCapacityError:
                 # the reference emits at most max_alignments_per_id + 1 rows per candidate (:309-311)

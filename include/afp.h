@@ -359,8 +359,39 @@ int afp_match_options_batch(afp_ctx* ctx, const int32_t* q_rows, int q_on_host, 
  * on ALL queries, packs one fixed-size record per query into a caller-owned DEVICE buffer, the
  * caller all-gathers the buffers (NCCL), and afp_shard_merge rebuilds on the device the rows a
  * single table would give (same rows, same ranks); fetch them with afp_fetch_match_rows.
- * Record (little endian): int32 {n_above, ncand, nrows, 0}; f64 weight[sd]; uint32 id[sd];
- * uint32 raw[sd]; int32 rows[row_cap][7].  row_cap must be even. */
+ * Record (little endian): int32 {n_above, ncand, nrows, status}; f64 weight[sd]; uint32 id[sd];
+ * uint32 raw[sd]; int32 rows[row_cap][7].  row_cap must be even.
+ *
+ * exact_count / find_time_range on a sharded table (audfprint_match.py:149-244): the reference
+ * finishes each candidate from that candidate's hits alone, and a track id lives in one shard, so
+ * a shard can finish its own ids - given three things that are not local:
+ *   - depth: the whole table finishes ranks < D = min(sum n_above, search_depth); a shard's id can
+ *     be inside the global top-D at or past its shard's n_above, so a shard finishes every
+ *     candidate it publishes (rank < min(entries, search_depth)) and the merge drops ranks >= D;
+ *   - key width: the packed (qtime, hash) keys take ceil(log(qmax)/log(2)) bits of the query's
+ *     largest qtime over ALL its hits (:157-167), the maximum over the shards of the shard maxima;
+ *   - errors: a quantile index outside its support (IndexError, :184-188) counts only at a global
+ *     rank < D, and a rank must not fail between the collectives; the shard records it instead.
+ * Hence two calls around one all-reduce (MAX) of one int32 per query:
+ *   afp_match_options_shard_rank    the ranking of afp_match_options_batch (same arguments), then
+ *                                   writes each query's largest qtime over the rows whose bucket is
+ *                                   non-empty on this shard into the CALLER's device int32
+ *                                   qmax_dev[nqueries] (the caller all-reduces it in place; no other
+ *                                   call on the context in between, and device query rows must
+ *                                   stay valid until the finish);
+ *   afp_match_options_shard_finish  the finish with that depth rule and the reduced qmax_dev;
+ *                                   fails only for reasons that are not data-dependent.
+ * afp_shard_pack then packs the finished rows (nrows = the rows the shard produced, which may
+ * exceed row_cap) and the status word: bit 0 = more rows than row_cap, bits 1-30 = 1 + the
+ * smallest local rank whose quantile read failed.  afp_shard_merge returns AFP_ERR_INDEX when such
+ * a candidate's global rank is < D, else AFP_ERR_INVALID ("row capacity: ...") when any record
+ * overflowed - the same outcome on every rank, as every rank merges the same bytes.  After a
+ * plain afp_match_batch the status word is 0 and an overflow fails afp_shard_pack itself. */
+int afp_match_options_shard_rank(afp_ctx* ctx, const int32_t* q_rows, int q_on_host, int32_t nqueries,
+                                 const int64_t* q_offsets, const afp_matcher_params* p, int32_t exact_count,
+                                 int32_t find_time_range, double time_quantile,
+                                 const int64_t* timebits_breaks, int32_t* qmax_dev, int64_t* ranked_rows);
+int afp_match_options_shard_finish(afp_ctx* ctx, const int32_t* qmax_dev, int64_t* total_rows);
 int64_t afp_shard_record_bytes(int32_t search_depth, int32_t row_cap);
 int afp_shard_pack(afp_ctx* ctx, int32_t row_cap, void* records_dev /* [nqueries][record bytes] */);
 int afp_shard_merge(afp_ctx* ctx, const void* gathered_dev /* [nshards][nqueries][record bytes] */,
