@@ -75,6 +75,8 @@ _SIGS = {
     "afp_table_retrieve_ids": (C.c_int, [_P, _I64P, C.c_int64, _I64P]),
     "afp_fetch_retrieved": (C.c_int, [_P, _P, C.c_int, _I64P]),
     "afp_table_merge": (C.c_int, [_P, _P, _P, C.c_int32, C.c_int32, C.c_int64, _P, _I64P, _P]),
+    "afp_table_merge_device": (C.c_int, [_P, _P, _P, C.c_int32, C.c_int32, C.c_int64, _P, _I64P, _P]),
+    "afp_table_export": (C.c_int, [_P, _P, _P]),
     "afp_np_permutation_replay": (C.c_int, [_P, _P, C.c_int64, C.c_int32, _P]),
     "afp_table_pruning_bound": (C.c_int, [_P, C.POINTER(C.c_uint32)]),
     "afp_get_hits": (C.c_int, [_P, _P, C.c_int64, C.c_int, _I64P]),

@@ -11,7 +11,10 @@
 // Only overflowing buckets draw from NumPy's global MT19937, one bucket after the other, and how
 // many words a bucket draws depends on its pool SIZE alone (Fisher-Yates with masked rejection,
 // afp_np_permutation_replay below).  So:
-//   1. the incoming table goes up as raw rows (the buckets this table has) with its counts;
+//   1. the incoming table goes up as raw rows (the buckets this table has) with its counts -
+//      afp_table_merge; afp_table_merge_device reads rows and counts where they already lie in
+//      device memory (a table exported by afp_table_export, e.g. received from another GPU) and
+//      copies only the counts to the host for the checks;
 //   2. one warp per bucket classifies it: a fitting pool is appended in place (only slots at or
 //      beyond our prefix are written), an overflowing bucket is flagged with its pool size; a scan
 //      compacts the flagged buckets in ascending order and their pool sizes go to the host;
@@ -245,29 +248,10 @@ int apply_overflow(afp_ctx* c, const MergeArgs& a, const std::vector<int32_t>& p
   return fail(AFP_OK);
 }
 
-}  // namespace
-
-extern "C" {
-
-int afp_np_permutation_replay(uint32_t* state625, const int32_t* pool_sizes, int64_t n, int32_t keep,
-                              int32_t* out) {
-  if (!state625 || n < 0 || keep < 1 || (n > 0 && (!pool_sizes || !out))) return AFP_ERR_INVALID;
-  if (state625[624] > 624u) return AFP_ERR_INVALID;
-  for (int64_t i = 0; i < n; ++i)
-    if (pool_sizes[i] < keep) return AFP_ERR_INVALID;          // nothing drawn yet: the state is unchanged
-  Mt g;
-  std::copy(state625, state625 + 624, g.mt);
-  g.pos = state625[624];
-  std::vector<uint32_t> x;
-  for (int64_t i = 0; i < n; ++i) permute_one(g, (uint32_t)pool_sizes[i], (uint32_t)keep, x, out + (size_t)i * keep);
-  std::copy(g.mt, g.mt + 624, state625);
-  state625[624] = g.pos;
-  return AFP_OK;
-}
-
-int afp_table_merge(afp_ctx* c, const uint32_t* table, const int32_t* counts, int32_t hashbits, int32_t depth,
-                    int64_t id_offset, uint32_t* np_state625, int64_t* noverflow, double* stage_ms) {
-  if (!c || !table || !counts || !np_state625) return AFP_ERR_INVALID;
+// the checks both merge entries make before anything changes; `counts` is a HOST copy of the
+// incoming counts [2^hashbits]
+int merge_check(afp_ctx* c, const int32_t* counts, int32_t hashbits, int32_t depth, int64_t id_offset,
+                const uint32_t* np_state625) {
   if (!c->tab.loaded) AFP_FAIL(c, AFP_ERR_STATE, "no table on the device");
   if (hashbits < 1 || hashbits > 28 || depth < 1) AFP_FAIL(c, AFP_ERR_INVALID, "bad geometry of the incoming table");
   if (np_state625[624] > 624u) AFP_FAIL(c, AFP_ERR_INVALID, "MT19937 position above 624");
@@ -280,26 +264,18 @@ int afp_table_merge(afp_ctx* c, const uint32_t* table, const int32_t* counts, in
     if (b >= nb && counts[b] != 0)
       AFP_FAIL(c, AFP_ERR_INDEX, "a live bucket of the incoming table lies outside this table (hash_table.py:302)");
   }
-  if (noverflow) *noverflow = 0;
-  if (stage_ms) std::fill(stage_ms, stage_ms + 6, 0.0);
-  const int64_t nm = std::min(nb, in_nb);       // buckets beyond are empty in the incoming table
-  AFP_CUDA(c, cudaSetDevice(c->device));
+  return AFP_OK;
+}
+
+// classify, compaction, replay and apply on incoming rows that are already on the device: d_in
+// [nm][depth] rows of the incoming table (only the buckets we have), d_cnt [nm] its counts
+int merge_body(afp_ctx* c, const uint32_t* d_in, const int32_t* d_cnt, int32_t depth, int64_t nm, int64_t id_offset,
+               uint32_t* np_state625, int64_t* noverflow, double* stage_ms) {
   auto t0 = std::chrono::steady_clock::now();
-  const size_t tbytes = (size_t)nm * (size_t)depth * sizeof(uint32_t);
-  AFP_CUDA(c, c->d_mg_in.reserve(tbytes + sizeof(int32_t) * (size_t)nm));
-  uint32_t* d_in = c->d_mg_in.as<uint32_t>();
-  int32_t* d_cnt = reinterpret_cast<int32_t*>(c->d_mg_in.as<char>() + tbytes);
-  AFP_CUDA(c, cudaMemcpyAsync(d_in, table, tbytes, cudaMemcpyHostToDevice, c->stream));
-  AFP_CUDA(c, cudaMemcpyAsync(d_cnt, counts, sizeof(int32_t) * (size_t)nm, cudaMemcpyHostToDevice, c->stream));
-  if (stage_ms) {
-    AFP_CUDA(c, cudaStreamSynchronize(c->stream));
-    stage_ms[0] = ms_since(t0);
-    t0 = std::chrono::steady_clock::now();
-  }
   MergeArgs a;
   a.table = c->tab.table.as<uint32_t>(); a.counts = c->tab.counts.as<int32_t>(); a.depth = c->tab.depth;
   a.in_table = d_in; a.in_counts = d_cnt; a.in_depth = depth; a.in_nb = nm;
-  a.shift = (uint32_t)(id_offset << mtb);
+  a.shift = (uint32_t)(id_offset << c->tab.maxtimebits);
   AFP_CUDA(c, c->d_mg_flag.reserve(sizeof(int32_t) * 2 * (size_t)nm));
   AFP_CUDA(c, c->d_mg_off.reserve(sizeof(int64_t) * (size_t)(nm + 1)));
   int32_t* flag = c->d_mg_flag.as<int32_t>();
@@ -339,6 +315,85 @@ int afp_table_merge(afp_ctx* c, const uint32_t* table, const int32_t* counts, in
   // the table now names ids the device's hashesperid does not have yet: no pruning until the
   // caller's afp_table_set_hashesperid recomputes the bound over the merged table
   c->tab.hmin = 0;
+  return AFP_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int afp_np_permutation_replay(uint32_t* state625, const int32_t* pool_sizes, int64_t n, int32_t keep,
+                              int32_t* out) {
+  if (!state625 || n < 0 || keep < 1 || (n > 0 && (!pool_sizes || !out))) return AFP_ERR_INVALID;
+  if (state625[624] > 624u) return AFP_ERR_INVALID;
+  for (int64_t i = 0; i < n; ++i)
+    if (pool_sizes[i] < keep) return AFP_ERR_INVALID;          // nothing drawn yet: the state is unchanged
+  Mt g;
+  std::copy(state625, state625 + 624, g.mt);
+  g.pos = state625[624];
+  std::vector<uint32_t> x;
+  for (int64_t i = 0; i < n; ++i) permute_one(g, (uint32_t)pool_sizes[i], (uint32_t)keep, x, out + (size_t)i * keep);
+  std::copy(g.mt, g.mt + 624, state625);
+  state625[624] = g.pos;
+  return AFP_OK;
+}
+
+int afp_table_merge(afp_ctx* c, const uint32_t* table, const int32_t* counts, int32_t hashbits, int32_t depth,
+                    int64_t id_offset, uint32_t* np_state625, int64_t* noverflow, double* stage_ms) {
+  if (!c || !table || !counts || !np_state625) return AFP_ERR_INVALID;
+  int rc = merge_check(c, counts, hashbits, depth, id_offset, np_state625);
+  if (rc) return rc;
+  const int64_t nm = std::min((int64_t)1 << c->tab.hashbits, (int64_t)1 << hashbits);
+  if (noverflow) *noverflow = 0;
+  if (stage_ms) std::fill(stage_ms, stage_ms + 6, 0.0);
+  AFP_CUDA(c, cudaSetDevice(c->device));
+  const auto t0 = std::chrono::steady_clock::now();
+  const size_t tbytes = (size_t)nm * (size_t)depth * sizeof(uint32_t);
+  AFP_CUDA(c, c->d_mg_in.reserve(tbytes + sizeof(int32_t) * (size_t)nm));
+  uint32_t* d_in = c->d_mg_in.as<uint32_t>();
+  int32_t* d_cnt = reinterpret_cast<int32_t*>(c->d_mg_in.as<char>() + tbytes);
+  AFP_CUDA(c, cudaMemcpyAsync(d_in, table, tbytes, cudaMemcpyHostToDevice, c->stream));
+  AFP_CUDA(c, cudaMemcpyAsync(d_cnt, counts, sizeof(int32_t) * (size_t)nm, cudaMemcpyHostToDevice, c->stream));
+  if (stage_ms) {
+    AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+    stage_ms[0] = ms_since(t0);
+  }
+  return merge_body(c, d_in, d_cnt, depth, nm, id_offset, np_state625, noverflow, stage_ms);
+}
+
+int afp_table_merge_device(afp_ctx* c, const uint32_t* table_dev, const int32_t* counts_dev, int32_t hashbits,
+                           int32_t depth, int64_t id_offset, uint32_t* np_state625, int64_t* noverflow,
+                           double* stage_ms) {
+  if (!c || !table_dev || !counts_dev || !np_state625) return AFP_ERR_INVALID;
+  if (hashbits < 1 || hashbits > 28 || depth < 1) AFP_FAIL(c, AFP_ERR_INVALID, "bad geometry of the incoming table");
+  AFP_CUDA(c, cudaSetDevice(c->device));
+  // the checks read the counts on the host (4 MB at 2^20 buckets); the rows stay where they are
+  const auto t0 = std::chrono::steady_clock::now();
+  std::vector<int32_t> h_counts((size_t)1 << hashbits);
+  AFP_CUDA(c, cudaMemcpyAsync(h_counts.data(), counts_dev, sizeof(int32_t) * h_counts.size(), cudaMemcpyDeviceToHost,
+                              c->stream));
+  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+  const double download_ms = ms_since(t0);
+  int rc = merge_check(c, h_counts.data(), hashbits, depth, id_offset, np_state625);
+  if (rc) return rc;
+  if (noverflow) *noverflow = 0;
+  if (stage_ms) {
+    std::fill(stage_ms, stage_ms + 6, 0.0);
+    stage_ms[0] = download_ms;
+  }
+  const int64_t nm = std::min((int64_t)1 << c->tab.hashbits, (int64_t)1 << hashbits);
+  return merge_body(c, table_dev, counts_dev, depth, nm, id_offset, np_state625, noverflow, stage_ms);
+}
+
+int afp_table_export(afp_ctx* c, uint32_t* table_dev, int32_t* counts_dev) {
+  if (!c || !table_dev || !counts_dev) return AFP_ERR_INVALID;
+  if (!c->tab.loaded) AFP_FAIL(c, AFP_ERR_STATE, "no table on the device");
+  AFP_CUDA(c, cudaSetDevice(c->device));
+  const size_t nb = (size_t)1 << c->tab.hashbits;
+  AFP_CUDA(c, cudaMemcpyAsync(table_dev, c->tab.table.p, nb * (size_t)c->tab.depth * sizeof(uint32_t),
+                              cudaMemcpyDeviceToDevice, c->stream));
+  AFP_CUDA(c, cudaMemcpyAsync(counts_dev, c->tab.counts.p, nb * sizeof(int32_t), cudaMemcpyDeviceToDevice, c->stream));
+  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
   return AFP_OK;
 }
 

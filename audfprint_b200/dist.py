@@ -6,6 +6,11 @@ pickling results back.  The same shape is used here:
 
 * fingerprinting: file i -> rank i % world; NO data-path collective (results are
   per-file and gathered as host objects only if the caller asks for them);
+* building ONE table from a multi-GPU ingest (`ingest_sharded`, the reference's
+  `new` / `add --ncores N`): every rank stores its own files into a fresh table on
+  its GPU, the root receives the tables in rank order (NCCL device to device) and
+  merges each into its table on the device, as `multiproc_add` merges its workers'
+  tables;
 * matching, table replicated (419 MB << 80 GB): query j -> rank j % world; no
   collective;
 * matching, table sharded by track-id range (SURVEY.md §8e, BASELINE configs[4]):
@@ -17,7 +22,7 @@ pickling results back.  The same shape is used here:
   query time comes first, so that every shard packs its (qtime, hash) keys with the
   whole table's key width; see match_sharded_batch.
 
-Nothing here computes on the CPU; it only moves and merges small result records.
+Nothing here computes on the CPU; it only moves tables and small result records.
 """
 from __future__ import annotations
 
@@ -385,3 +390,146 @@ def match_sharded_batch(matcher, ht, packed_queries, row_cap: int = 16, group=No
     ctx.check(ctx.lib.afp_fetch_match_rows(ctx.h, rows.ctypes.data if len(rows) else None, 1,
                                            roff.ctypes.data_as(C.POINTER(C.c_int64))))
     return rows, roff
+
+
+# ---- one table from a multi-GPU ingest (the reference's multiproc_add) --------------------
+def _group_rank(group):
+    import torch.distributed as dist
+    if not (dist.is_available() and dist.is_initialized()):
+        return 0, 1
+    return dist.get_rank(group), dist.get_world_size(group)
+
+
+def _global_rank(group, r):
+    import torch.distributed as dist
+    return r if group is None else dist.get_global_rank(group, r)
+
+
+def ingest_sharded(analyzer, ht, names, signals, root=0, replicate=False, report=None, group=None):
+    """`audfprint.py new / add --ncores N` (multiproc_add, audfprint.py:199-235) over the ranks of
+    a process group, one GPU each.  `names` / `signals` are this rank's own files, dealt as the
+    reference deals them (shard_indices: file i -> rank i % world).
+
+    1. The rank ingests its files into a fresh table of ht's geometry on its GPU
+       (Analyzer.ingest_batch), drawing from this process's `random` state; the reference's worker r
+       draws from its own, so seed each rank's `random` (e.g. random.seed(1000 + rank)).
+    2. One all-gather of a status word, the rank's name and hash counts and the root's base name
+       count and geometry.  If any rank's ingest raised, every rank raises before any table moves:
+       the failing rank its own exception, the others a RuntimeError naming the first failing rank.
+       Geometries that disagree raise ValueError, and a merged id that would not fit in
+       32 - maxtimebits bits raises OverflowError, on every rank alike.
+    3. The rank's table is exported on its device (HashTable.export_device).  The root receives the
+       tables in rank order - NCCL send / recv device to device, or through host memory under gloo -
+       and merges them into `ht` with ONE merge_batch, in rank order, its own table included (the
+       merge of an empty table is not the table itself: counts above depth become depth).  The root's
+       own table never goes through the host.
+    4. Names and hashesperid travel as host objects.  The merged names are rank-major:
+       ht.names + names of rank 0 + names of rank 1 + ...
+    5. `report`, on the root, receives the reference's line "hash_table r has N files H hashes" for
+       each rank r, in rank order, as a one-line list.
+    6. With replicate=True the root exports the merged table and broadcasts it; every rank installs it
+       as its device copy (afp_table_upload from device memory) with the same names and hashesperid.
+       Otherwise the other ranks' `ht` are unchanged.  np.random advances on the root only.
+    Returns the number of hashes stored for each of this rank's files."""
+    import torch
+    from . import _lib
+    from .hash_table import DeviceTable, HashTable
+    rank, ws = _group_rank(group)
+    root = int(root)
+    if not 0 <= root < ws:
+        raise ValueError("root %d outside the group's %d ranks" % (root, ws))
+    if len(names) != len(signals):
+        raise ValueError("%d names for %d signals" % (len(names), len(signals)))
+    ctx = _lib.context(ht.device)
+    dev = torch.device("cuda", ctx.device)
+    nccl = False
+    if ws > 1:
+        import torch.distributed as dist
+        nccl = dist.get_backend(group) == "nccl"
+    hb, depth, mtb = int(ht.hashbits), int(ht.depth), int(ht.maxtimebits)
+
+    # 1. this rank's files into a fresh table
+    local = HashTable(hashbits=hb, depth=depth, maxtime=1 << mtb, device=ht.device)
+    err, mine, counts = None, None, []
+    try:
+        counts = analyzer.ingest_batch(local, list(names), list(signals))
+        mine = local.export_device()
+    except Exception as e:          # raised on every rank after the all-gather
+        err = e
+    if ctx.table_owner is not None and ctx.table_owner() is local:
+        ctx.table_owner = None      # its rows live on in `mine`: no pull to the host when `ht` takes the device
+    del local
+    nhashes = int(mine.counts.sum(dtype=torch.int64)) if mine is not None else 0
+
+    # 2. status, name and hash counts, the root's base and geometry, from every rank
+    info = np.array([0 if err is None else 1, len(mine.names) if mine is not None else 0, nhashes,
+                     len(ht.names), hb, depth, mtb], np.int64)
+    if ws > 1:
+        t = torch.from_numpy(info).to(dev if nccl else "cpu")
+        g = torch.empty(ws * len(info), dtype=torch.int64, device=t.device)
+        dist.all_gather_into_tensor(g, t, group=group)
+        infos = g.cpu().numpy().reshape(ws, len(info))
+    else:
+        infos = info[None]
+    failed = np.nonzero(infos[:, 0])[0]
+    if len(failed):
+        if err is not None:
+            raise err
+        raise RuntimeError("ingest_sharded: rank %d failed to ingest its files" % int(failed[0]))
+    if (infos[:, 4:] != infos[root, 4:]).any():
+        raise ValueError("ingest_sharded: the ranks' tables disagree on hashbits / depth / maxtimebits")
+    nn = int(infos[root, 3])
+    for r in range(ws):
+        if nn << mtb >= 1 << 32:
+            raise OverflowError("id offset %d does not fit in %d id bits" % (nn, 32 - mtb))
+        nn += int(infos[r, 1])
+        if infos[r, 1] and (nn + 1) << mtb > 1 << 32:
+            raise OverflowError("id %d does not fit in %d id bits" % (nn - 1, 32 - mtb))
+
+    # 3. + 4. the tables to the root in rank order, names and hashesperid as host objects
+    nb = 1 << hb
+    book = [(mine.names, mine.hashesperid)]
+    if ws > 1:
+        book = [None] * ws if rank == root else None
+        dist.gather_object((mine.names, mine.hashesperid), book, dst=_global_rank(group, root), group=group)
+    if rank == root:
+        tables = []
+        for r in range(ws):
+            if r == rank:
+                tables.append(mine)
+                continue
+            tab = torch.empty((nb, depth), dtype=torch.int32, device=dev if nccl else "cpu")
+            cnt = torch.empty(nb, dtype=torch.int32, device=tab.device)
+            dist.recv(tab, src=_global_rank(group, r), group=group)
+            dist.recv(cnt, src=_global_rank(group, r), group=group)
+            if not nccl:
+                tab, cnt = tab.to(dev), cnt.to(dev)
+            tables.append(DeviceTable(tab, cnt, book[r][0], book[r][1], hb, depth, mtb))
+        if report is not None:
+            for r in range(ws):
+                report(["hash_table %d has %d files %d hashes" % (r, int(infos[r, 1]), int(infos[r, 2]))])
+        ht.merge_batch(tables)
+        del tables
+    else:
+        dst = _global_rank(group, root)
+        dist.send(mine.table if nccl else mine.table.cpu(), dst=dst, group=group)
+        dist.send(mine.counts if nccl else mine.counts.cpu(), dst=dst, group=group)
+    del mine
+
+    # 6. the merged table to every rank
+    if replicate and ws > 1:
+        src = _global_rank(group, root)
+        if rank == root:
+            snap = ht.export_device()
+            obj = [(snap.names, snap.hashesperid)]
+            tab, cnt = (snap.table, snap.counts) if nccl else (snap.table.cpu(), snap.counts.cpu())
+        else:
+            obj = [None]
+            tab = torch.empty((nb, depth), dtype=torch.int32, device=dev if nccl else "cpu")
+            cnt = torch.empty(nb, dtype=torch.int32, device=tab.device)
+        dist.broadcast_object_list(obj, src=src, group=group)
+        dist.broadcast(tab, src=src, group=group)
+        dist.broadcast(cnt, src=src, group=group)
+        if rank != root:
+            ht._install_device(DeviceTable(tab.to(dev), cnt.to(dev), obj[0][0], obj[0][1], hb, depth, mtb))
+    return counts

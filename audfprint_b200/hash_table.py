@@ -10,7 +10,8 @@ twice: per track on the host, and batched on the device (`store_batch`,
 SURVEY.md §8f-1: the device copy then leads and the host arrays refresh from it
 when read).  `remove` and `retrieve` also exist batched on the device (`remove_batch`,
 `retrieve_batch`), which the per-name forms use while the device copy leads.  `merge` runs on
-the host; `merge_batch` merges a list of tables on the device.  All of them reproduce the
+the host; `merge_batch` merges a list of tables on the device, host tables or device snapshots
+(`export_device`, `DeviceTable`) of tables that may come from other GPUs.  All of them reproduce the
 reference's results exactly, including its draws from the global `random` /
 `np.random` generators on bucket overflow.
 """
@@ -95,6 +96,20 @@ def _as_reference_object(ht, cls):
     obj.__dict__.update({k: getattr(ht, k) for k in _REF_ATTRS})
     obj.__dict__["dirty"] = False
     return obj
+
+
+class DeviceTable(object):
+    """A snapshot of a table in device memory (HashTable.export_device), which merge_batch takes
+    next to HashTables and which dist.ingest_sharded moves between GPUs:
+      table   int32 CUDA tensor [2^hashbits, depth], the bits of the uint32 entries (NCCL has no uint32)
+      counts  int32 CUDA tensor [2^hashbits]
+      names, hashesperid, hashbits, depth, maxtimebits   as in the table it was taken from."""
+
+    def __init__(self, table, counts, names, hashesperid, hashbits, depth, maxtimebits):
+        self.table, self.counts = table, counts
+        self.names = list(names)
+        self.hashesperid = np.array(hashesperid, np.uint32)
+        self.hashbits, self.depth, self.maxtimebits = int(hashbits), int(depth), int(maxtimebits)
 
 
 class HashTable(object):
@@ -484,8 +499,11 @@ class HashTable(object):
         """HashTable.merge (hash_table.py:291-323) of a list of tables, on the device table.
 
         Leaves table, counts, names, hashesperid, `dirty` and the np.random state as
-        `for t in tables: self.merge(t)` does (`random` is not used).  Each incoming table's host
-        arrays are read first (a table whose device copy leads pulls it), then the merges run on
+        `for t in tables: self.merge(t)` does (`random` is not used).  An entry of the list is a
+        HashTable or a DeviceTable snapshot (export_device) on this table's device.  Each incoming
+        HashTable's host arrays are read first (a table whose device copy leads pulls it); a
+        snapshot's rows are read where they lie (afp_table_merge_device), after the current torch
+        stream of its device is synchronised.  The merges run on
         this table's device copy: buckets whose pool fits are appended in place, the overflowing
         ones are drawn by a C replay of np.random.permutation on the host, chunk by chunk while
         the device applies the previous chunk.  Afterwards the DEVICE copy is the current one (as
@@ -502,6 +520,17 @@ class HashTable(object):
         nnames = len(self.names)
         plan = []
         for t in tables:
+            if isinstance(t, DeviceTable):
+                if self.maxtimebits != t.maxtimebits:
+                    raise AssertionError("tables disagree on maxtimebits (%d vs %d)" % (self.maxtimebits, t.maxtimebits))
+                self._check_snapshot(t, nb)
+                if nnames << mtb >= 1 << 32:
+                    raise OverflowError("id offset %d does not fit in %d id bits" % (nnames, 32 - mtb))
+                plan.append((t, None, None, nnames))
+                nnames += len(t.names)
+                if len(t.names) and (nnames + 1) << mtb > 1 << 32:
+                    raise OverflowError("id %d does not fit in %d id bits" % (nnames - 1, 32 - mtb))
+                continue
             if t is self:
                 raise ValueError("a table cannot be merged into itself")
             if getattr(t, "_store_pending", False):
@@ -527,14 +556,22 @@ class HashTable(object):
         if not plan:
             return 0
         ctx = self._sync_device()
+        if any(table is None for _, table, _, _ in plan):
+            import torch
+            torch.cuda.current_stream(torch.device("cuda", ctx.device)).synchronize()
         st = np.random.get_state()
         state = np.empty(625, np.uint32)
         state[:624], state[624] = st[1], st[2]
         novf, total = C.c_int64(0), 0
         try:
             for t, table, counts, offset in plan:
-                ctx.check(ctx.lib.afp_table_merge(ctx.h, table.ctypes.data, counts.ctypes.data, int(t.hashbits),
-                                                  int(t.depth), offset, state.ctypes.data, C.byref(novf), None))
+                if table is None:
+                    ctx.check(ctx.lib.afp_table_merge_device(ctx.h, t.table.data_ptr(), t.counts.data_ptr(),
+                                                             t.hashbits, t.depth, offset, state.ctypes.data,
+                                                             C.byref(novf), None))
+                else:
+                    ctx.check(ctx.lib.afp_table_merge(ctx.h, table.ctypes.data, counts.ctypes.data, int(t.hashbits),
+                                                      int(t.depth), offset, state.ctypes.data, C.byref(novf), None))
                 total += int(novf.value)
             hpi = np.concatenate([self.hashesperid] + [np.asarray(t.hashesperid) for t, _, _, _ in plan]).astype(np.uint32)
             ctx.check(ctx.lib.afp_table_set_hashesperid(ctx.h, hpi.ctypes.data if len(hpi) else None, len(hpi)))
@@ -550,6 +587,66 @@ class HashTable(object):
         ctx.table_key = self._dev_key = self._stamp()      # the device copy IS this version
         ctx.table_owner = weakref.ref(self)
         return total
+
+    def _check_snapshot(self, t, nb):
+        """merge_batch's checks of a DeviceTable, made on the device (no copy of its arrays)."""
+        import torch
+        dev = torch.device("cuda", _lib.context(self.device).device)
+        nb_in = 1 << t.hashbits
+        for x, shape in ((t.table, (nb_in, t.depth)), (t.counts, (nb_in,))):
+            if (not x.is_cuda or x.device != dev or x.dtype != torch.int32 or tuple(x.shape) != shape
+                    or not x.is_contiguous()):
+                raise ValueError("a device table's arrays must be contiguous int32 tensors of its geometry "
+                                 "on this table's device (%s)" % dev)
+        if bool((t.counts < 0).any()):
+            raise ValueError("an incoming table has a negative count")
+        outside = torch.nonzero(t.counts[nb:])
+        if len(outside):
+            raise IndexError("bucket %d of an incoming table lies outside this table's %d buckets"
+                             % (nb + int(outside[0, 0]), nb))
+
+    def export_device(self):
+        """A DeviceTable snapshot of this table: its current device copy (uploaded first if the host
+        arrays are newer) copied device to device into new CUDA tensors, with copies of names and
+        hashesperid.  The copy is complete when this returns."""
+        import torch
+        self._check_device_edit("export_device")
+        ctx = self._sync_device()
+        dev = torch.device("cuda", ctx.device)
+        nb = 1 << int(self.hashbits)
+        table = torch.empty((nb, int(self.depth)), dtype=torch.int32, device=dev)
+        counts = torch.empty(nb, dtype=torch.int32, device=dev)
+        ctx.check(ctx.lib.afp_table_export(ctx.h, table.data_ptr(), counts.data_ptr()))
+        return DeviceTable(table, counts, self.names, self.hashesperid, self.hashbits, self.depth, self.maxtimebits)
+
+    def _install_device(self, snap):
+        """Make this table a copy of the DeviceTable `snap`: its arrays become the device copy
+        (afp_table_upload from device memory), names and hashesperid are copied.  Afterwards the
+        DEVICE copy is the current one; the host arrays are pulled from it when read."""
+        import torch
+        self._check_device_edit("install a device table")
+        ctx = _lib.context(self.device)
+        owner = ctx.table_owner() if getattr(ctx, "table_owner", None) else None
+        if owner is not None and owner is not self and getattr(owner, "_dev_newer", False):
+            owner._pull_device()
+        ctx.table_owner = None
+        ctx.table_key = None
+        self._shard = None
+        dev = torch.device("cuda", ctx.device)
+        hpi = np.ascontiguousarray(snap.hashesperid, dtype=np.uint32)
+        hpi_dev = torch.from_numpy(hpi.view(np.int32)).to(dev) if len(hpi) else None
+        torch.cuda.current_stream(dev).synchronize()
+        ctx.check(ctx.lib.afp_table_upload(ctx.h, snap.table.data_ptr(), snap.counts.data_ptr(), snap.hashbits,
+                                           snap.depth, snap.maxtimebits,
+                                           hpi_dev.data_ptr() if hpi_dev is not None else None, len(hpi), 0))
+        self.hashbits, self.depth, self.maxtimebits = snap.hashbits, snap.depth, snap.maxtimebits
+        self.__dict__["_table"] = self.__dict__["_counts"] = None     # pulled from the device when read
+        self.names = list(snap.names)
+        self.__dict__["_hashesperid"] = hpi.copy()
+        self._touch()
+        self._dev_newer = True
+        ctx.table_key = self._dev_key = self._stamp()      # the device copy IS this version
+        ctx.table_owner = weakref.ref(self)
 
     def _check_device_edit(self, what):
         # a shard stamp left behind after another table took the device is no shard: _sync_device

@@ -279,6 +279,18 @@ int afp_fetch_retrieved(afp_ctx* ctx, int32_t* rows, int rows_on_host, int64_t* 
  * afp_table_set_hashesperid uploads the merged one. */
 int afp_table_merge(afp_ctx* ctx, const uint32_t* table, const int32_t* counts, int32_t hashbits, int32_t depth,
                     int64_t id_offset, uint32_t* np_state625, int64_t* noverflow, double* stage_ms);
+/* afp_table_merge with the incoming table in DEVICE memory (same arguments, same result, same
+ * errors): table_dev uint32 [2^hashbits][depth] and counts_dev int32 [2^hashbits], e.g. a table
+ * exported by afp_table_export on this or another GPU.  The rows are read in place; only the counts
+ * are copied to the host, for the checks, which fail (AFP_ERR_INVALID / AFP_ERR_INDEX) before anything
+ * changes.  stage_ms[0] is that copy.  The buffers are no longer read when the call returns. */
+int afp_table_merge_device(afp_ctx* ctx, const uint32_t* table_dev, const int32_t* counts_dev, int32_t hashbits,
+                           int32_t depth, int64_t id_offset, uint32_t* np_state625, int64_t* noverflow,
+                           double* stage_ms);
+/* Device-to-device copy of the device table into caller-owned DEVICE buffers: table_dev uint32
+ * [2^hashbits][depth], counts_dev int32 [2^hashbits] (the geometry of the last upload / create).
+ * Synchronises before it returns, so the buffers may go straight to a transfer on another stream. */
+int afp_table_export(afp_ctx* ctx, uint32_t* table_dev, int32_t* counts_dev);
 /* np.random.permutation of n pools (hash_table.py:291-323, the draws of HashTable.merge), replayed
  * on index arrays: out (HOST int32 [n][keep]) receives the first `keep` entries of the permutation of
  * 0..pool_sizes[i]-1 that RandomState.permutation would return for a pool of that size, the pools in
