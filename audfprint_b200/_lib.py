@@ -50,6 +50,8 @@ _SIGS = {
     "afp_get_stage_ms": (C.c_int, [_P, C.POINTER(C.c_float)]),
     "afp_pcm_frontend": (C.c_int, [_P, _P, C.c_int, C.c_int64, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int32, _P,
                                    C.c_int, _I64P]),
+    "afp_pcm_frontend_batch": (C.c_int, [_P, _P, C.c_int, C.c_int64, C.c_int32, _I64P, _I64P, _P, _P, _P, C.c_int32,
+                                         _P, _I64P, _P, _P, C.c_int64, _I64P, _I64P]),
     "afp_set_analyzer": (C.c_int, [_P, C.POINTER(AnalyzerParams), _P, _P, C.c_double]),
     "afp_fingerprint_batch": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int32, _I64P, _I64P, _I64P]),
     "afp_fetch_hashes": (C.c_int, [_P, _P, C.c_int, _I64P]),

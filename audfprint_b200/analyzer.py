@@ -94,6 +94,17 @@ def pcm_frontend(raw, channels, src_rate, dst_rate=None, device=None, to_host=Tr
     return out
 
 
+def _wav_read_raw(filename):
+    """The host half of _wav_reader: parse a PCM WAV -> (int16 interleaved samples, channels, rate).
+    Raises what _wav_reader raises for a file it cannot read."""
+    with wave.open(filename, 'rb') as w:
+        nch, width, fs, n = w.getnchannels(), w.getsampwidth(), w.getframerate(), w.getnframes()
+        if width != 2:
+            raise IOError("only 16-bit PCM WAV is supported, got %d-byte samples" % width)
+        raw = np.frombuffer(w.readframes(n), dtype='<i2')
+    return raw, nch, fs
+
+
 def _wav_reader(filename, sr=None, channels=None, device=None):
     """PCM-WAV reader standing in for audio_read.audio_read (audio_read.py:56-68; ffmpeg decoding
     is out of scope, SURVEY §2 #9).  Returns (float32 samples in [-1,1), sr) like the reference
@@ -101,16 +112,117 @@ def _wav_reader(filename, sr=None, channels=None, device=None):
     reference hands to ffmpeg - down-mix to mono, resampling to `sr` - runs on the device
     (afp_pcm_frontend, SURVEY.md 8f-2).  No two resamplers agree bit for bit, so parity statements
     in this repo are made on 11025 Hz PCM."""
-    with wave.open(filename, 'rb') as w:
-        nch, width, fs, n = w.getnchannels(), w.getsampwidth(), w.getframerate(), w.getnframes()
-        if width != 2:
-            raise IOError("only 16-bit PCM WAV is supported, got %d-byte samples" % width)
-        raw = np.frombuffer(w.readframes(n), dtype='<i2')
+    raw, nch, fs = _wav_read_raw(filename)
     if nch == 1 and (sr is None or fs == sr):
         # nothing to do but the reader's own scaling (exact in float32)
         return raw.astype(np.float32) * np.float32(1.0 / 32768.0), fs
     data = pcm_frontend(raw, nch, fs, sr, device=device)
     return data, (fs if sr is None else sr)
+
+
+_TAPS = {}
+
+
+def taps_table(pairs):
+    """The designs of the distinct resampling pairs among `pairs` ((up, down) per file; (1, 1) needs
+    none), in order of first appearance -> (pair_rates int32 (P,2), tap_offsets int64 (P+1,),
+    taps float64): what afp_pcm_frontend_batch takes.  Each design is resample_taps(up, down),
+    computed once per process."""
+    uniq = []
+    for ud in pairs:
+        ud = (int(ud[0]), int(ud[1]))
+        if ud != (1, 1) and ud not in uniq:
+            uniq.append(ud)
+    designs = []
+    for ud in uniq:
+        if ud not in _TAPS:
+            _TAPS[ud] = resample_taps(*ud)
+        designs.append(_TAPS[ud])
+    off = np.zeros(len(uniq) + 1, np.int64)
+    off[1:] = np.cumsum([len(t) for t in designs])
+    taps = np.ascontiguousarray(np.concatenate(designs)) if designs else np.zeros(1, np.float64)
+    return np.array(uniq, np.int32).reshape(-1, 2), off, taps
+
+
+def pcm_frontend_batch(raws, channels, src_rates, dst_rate, device=None):
+    """Many files' interleaved int16 PCM -> mono float32 at dst_rate in ONE device buffer
+    (afp_pcm_frontend_batch: one upload of the packed PCM, one launch, one synchronise).
+    Every file's samples are bit-identical to pcm_frontend on that file alone.
+    Returns (out torch CUDA float32, offsets int64 [n+1], lengths int64 [n]): file i is
+    out[offsets[i]:offsets[i] + lengths[i]], starting on a 16-byte boundary - the layout
+    Analyzer.fingerprint_packed(out, offsets, sample_lengths=lengths) takes as it is."""
+    import torch
+    from math import gcd
+    n = len(raws)
+    raws = [np.ascontiguousarray(r, dtype=np.int16).reshape(-1) for r in raws]
+    ch = np.array([int(c) for c in channels], np.int32)
+    nfr = np.array([len(r) // max(1, int(c)) for r, c in zip(raws, ch)], np.int64)
+    up, down = np.ones(n, np.int32), np.ones(n, np.int32)
+    for i, fs in enumerate(src_rates):
+        if dst_rate is not None and int(dst_rate) != int(fs):
+            g = gcd(int(dst_rate), int(fs))
+            up[i], down[i] = int(dst_rate) // g, int(fs) // g
+    rates, toff, taps = taps_table(zip(up, down))
+    inoff = np.zeros(n + 1, np.int64)
+    inoff[1:] = np.cumsum([len(r) for r in raws])
+    packed = np.concatenate(raws) if n else np.zeros(0, np.int16)
+    ctx = _lib.context(device)
+    off = np.zeros(n + 1, np.int64)
+    lens = np.zeros(n, np.int64)
+    P = C.POINTER(C.c_int64)
+    args = [ctx.h, packed.ctypes.data if len(packed) else None, 1, len(packed), n, inoff.ctypes.data_as(P),
+            nfr.ctypes.data_as(P), ch.ctypes.data, up.ctypes.data, down.ctypes.data, len(rates), rates.ctypes.data,
+            toff.ctypes.data_as(P), taps.ctypes.data]
+    ctx.check(ctx.lib.afp_pcm_frontend_batch(*args, None, 0, off.ctypes.data_as(P), lens.ctypes.data_as(P)))
+    # 16 bytes of zeros past the last file, as Analyzer._pack leaves
+    out = torch.zeros(int(off[-1]) + 4, dtype=torch.float32, device=torch.device("cuda", ctx.device))
+    torch.cuda.current_stream(out.device).synchronize()         # the zeros land before the library's stream writes
+    ctx.check(ctx.lib.afp_pcm_frontend_batch(*args, out.data_ptr(), out.numel(), None, None))
+    return out, off, lens
+
+
+class _ChunkPlanner(object):
+    """Greedy chunking in list order: a chunk grows while its frames stay within max_frames and its
+    bytes within max_bytes; a file over either cap goes alone."""
+
+    def __init__(self, max_frames, max_bytes):
+        self.max_frames, self.max_bytes = max_frames, max_bytes
+        self.n = self.frames = self.nbytes = 0
+
+    def add(self, frames, nbytes):
+        """Account one more file; True when it has to start a new chunk (the open one is full)."""
+        new = self.n > 0 and (self.frames + frames > self.max_frames or self.nbytes + nbytes > self.max_bytes)
+        if new:
+            self.n = self.frames = self.nbytes = 0
+        self.n += 1
+        self.frames += frames
+        self.nbytes += nbytes
+        return new
+
+
+def plan_chunks(frames, nbytes, max_frames, max_bytes):
+    """[start, end) of the chunks _ChunkPlanner makes of a list (what wavfiles2hashes does while it
+    reads): where a chunk ends depends only on the files before it."""
+    planner, out, start = _ChunkPlanner(max_frames, max_bytes), [], 0
+    for i, (f, b) in enumerate(zip(frames, nbytes)):
+        if planner.add(f, b):
+            out.append((start, i))
+            start = i
+    if len(frames) > start:
+        out.append((start, len(frames)))
+    return out
+
+
+class DeviceHashes(object):
+    """One file's hashes left on the device by Analyzer._hashes_of_files(rows_on_device=True):
+    `rows` is a torch CUDA int32 (n, 2) view, `last_time` the time of its last row (np.int32)."""
+    __slots__ = ("rows", "last_time")
+
+    def __init__(self, rows, last_time):
+        self.rows, self.last_time = rows, last_time
+
+    def __len__(self):
+        return int(self.rows.shape[0])
 
 
 def _as_pcm(d):
@@ -351,13 +463,17 @@ class Analyzer(object):
         try:
             d, sr = self.reader(filename, sr=self.target_sr, channels=1)
         except Exception as e:
-            message = "wavfile2peaks: Error reading " + filename
-            if self.fail_on_error:
-                print(e)
-                raise IOError(message)
-            print(message, "skipping")
+            self._read_failed(filename, e)
             d, sr = [], self.target_sr
         return d, sr
+
+    def _read_failed(self, filename, e):
+        """What the reference does with a file it cannot read: raise IOError, or report and skip it."""
+        message = "wavfile2peaks: Error reading " + filename
+        if self.fail_on_error:
+            print(e)
+            raise IOError(message)
+        print(message, "skipping")
 
     def _account(self, dur):
         self.soundfiledur = dur
@@ -412,6 +528,116 @@ class Analyzer(object):
         if self.shifts < 2 and len(hashes) == 0:
             return []        # the reference returns [] when there are no peaks (:401-402)
         return hashes
+
+    # bytes of raw PCM (int16 WAV samples, or a custom reader's float32) that wavfiles2hashes stages
+    # per device call
+    max_pcm_bytes_per_call = 1 << 30
+
+    def wavfiles2hashes(self, filenames):
+        """List form of wavfile2hashes: per file exactly what wavfile2hashes returns ([] included),
+        with soundfiledur / soundfiletotaldur / soundfilecount left as the per-file loop leaves them
+        and the files' durations in `last_batch_durations`.
+
+        WAVs read by the default reader are parsed on the host (_wav_read_raw); the raw PCM of a
+        chunk of files is staged once, down-mixed and resampled by ONE afp_pcm_frontend_batch call
+        into a device buffer, and fingerprinted there in place (fingerprint_packed).  A custom
+        `reader` is called per file and its output packed as it is.  .afpt / .afpk files take
+        the per-file code.  Chunks follow max_frames_per_call and max_pcm_bytes_per_call (a file
+        over a cap goes alone); the results do not depend on where they fall.
+
+        Files are read in list order.  With fail_on_error, the first unreadable file raises the
+        IOError _read raises, and nothing is returned: unlike the per-file loop, which has already
+        returned the earlier files' hashes by then, the counters are left as they were."""
+        return self._hashes_of_files(filenames, rows_on_device=False)
+
+    def _hashes_of_files(self, filenames, rows_on_device=False):
+        """wavfiles2hashes; with rows_on_device the fingerprinted files' hashes stay on the device
+        (afp_fetch_hashes into a torch tensor) as DeviceHashes."""
+        saved = (self.soundfiledur, self.soundfiletotaldur, self.soundfilecount)
+        n = len(filenames)
+        results, durs = [None] * n, [0.0] * n
+        nsh = max(1, int(self.shifts))
+        planner = _ChunkPlanner(self.max_frames_per_call, self.max_pcm_bytes_per_call)
+        chunk = []
+        try:
+            for i, fn in enumerate(filenames):
+                ext = os.path.splitext(fn)[1]
+                if ext in (PRECOMPEXT, PRECOMPPKEXT):
+                    results[i] = self.wavfile2hashes(fn)
+                    durs[i] = self.soundfiledur
+                    self.soundfiledur, self.soundfiletotaldur, self.soundfilecount = saved
+                    continue
+                if self.reader is _wav_reader:
+                    try:
+                        raw, nch, fs = _wav_read_raw(fn)
+                        if fs < 1:
+                            # the per-file reader fails here in the device front-end (down < 1)
+                            raise ValueError("%s: sample rate %d" % (fn, fs))
+                    except Exception as e:
+                        self._read_failed(fn, e)
+                        raw, nch, fs = np.zeros(0, np.int16), 1, self.target_sr
+                    nout = -(-(len(raw) // nch) * self.target_sr // fs)      # ceil(nframes * up / down)
+                    item = (i, (raw, nch, fs), nout, raw.nbytes)
+                else:
+                    d, sr = self._read(fn)
+                    durs[i] = len(d) / sr
+                    a = _as_pcm(d)[0] if len(d) else None
+                    item = (i, a, len(d), a.nbytes if a is not None else 0)
+                if item[2] == 0:                                  # nothing to fingerprint: []
+                    results[i] = []
+                    continue
+                if planner.add(nsh * (1 + item[2] // self.n_hop), item[3]):
+                    self._hash_chunk(chunk, results, durs, rows_on_device)
+                    chunk = []
+                chunk.append(item)
+            self._hash_chunk(chunk, results, durs, rows_on_device)
+        except BaseException:
+            self.soundfiledur, self.soundfiletotaldur, self.soundfilecount = saved
+            raise
+        for dur in durs:
+            self._account(dur)
+        self.last_batch_durations = durs
+        return results
+
+    def _hash_chunk(self, chunk, results, durs, rows_on_device):
+        """Fingerprint one chunk of files [(index, data, nsamples, nbytes)] in one device call and put
+        each file's hashes at its index of `results`."""
+        if not chunk:
+            return
+        idx = [it[0] for it in chunk]
+        if self.reader is _wav_reader:
+            raws = [it[1] for it in chunk]
+            out, off, lens = pcm_frontend_batch([r[0] for r in raws], [r[1] for r in raws], [r[2] for r in raws],
+                                                self.target_sr, device=self.device)
+            for i, ln in zip(idx, lens):
+                durs[i] = int(ln) / self.target_sr
+            self.fingerprint_packed(out, off, self.shifts, fetch=False, sample_lengths=lens)
+        else:
+            packed, starts, lens = self._pack([it[1] for it in chunk])
+            self.fingerprint_packed(packed, starts, self.shifts, fetch=False, sample_lengths=lens)
+        ctx = _lib.context(self.device)
+        roff = np.empty(len(chunk) + 1, np.int64)
+        ctx.check(ctx.lib.afp_fetch_hashes(ctx.h, None, 1, roff.ctypes.data_as(C.POINTER(C.c_int64))))
+        total = int(roff[-1])
+        if rows_on_device:
+            import torch
+            rows = torch.empty((max(total, 1), 2), dtype=torch.int32, device=torch.device("cuda", ctx.device))
+            # the library writes `rows` on its own stream: torch's earlier work on this memory is done first
+            torch.cuda.current_stream(rows.device).synchronize()
+            ctx.check(ctx.lib.afp_fetch_hashes(ctx.h, C.c_void_p(rows.data_ptr()), 0, None))
+            ends = np.maximum(roff[1:] - 1, 0)
+            last = rows[torch.from_numpy(ends).to(rows.device), 0].cpu().numpy() if total else np.zeros(len(idx), np.int32)
+        else:
+            rows = np.empty((total, 2), np.int32)
+            ctx.check(ctx.lib.afp_fetch_hashes(ctx.h, rows.ctypes.data, 1, None))
+        for k, i in enumerate(idx):
+            lo, hi = int(roff[k]), int(roff[k + 1])
+            if self.shifts < 2 and hi == lo:
+                results[i] = []            # the reference returns [] when there are no peaks (:401-402)
+            elif rows_on_device:
+                results[i] = DeviceHashes(rows[lo:hi], last[k])
+            else:
+                results[i] = rows[lo:hi]
 
     def ingest(self, hashtable, filename):
         """Read a file and add it to the table (audfprint_analyze.py:430-457)."""

@@ -14,6 +14,13 @@
 // that bar against the extended-precision statement of tests/exact_resample.py, which
 // scipy.signal.resample_poly cross-checks on the CPU.  ffmpeg's resampler, which the reference uses,
 // is not reproduced (§8f-2); parity statements against the reference are made on 11025 Hz PCM.
+//
+// afp_pcm_frontend_batch runs the same per-output function over a list of files in one launch: each
+// block belongs to one file (a per-file block prefix), each file's output starts on a 16-byte boundary
+// of one device buffer, laid out as afp_fingerprint_batch takes it, and every distinct (up, down)
+// design is uploaded once.  tests/test_gpu_pcm_batch.py holds it bit-equal to afp_pcm_frontend per file.
+#include <cstring>
+
 #include "afp_internal.cuh"
 
 namespace {
@@ -25,15 +32,11 @@ __device__ __forceinline__ float mono_at(const int16_t* pcm, int64_t j, int ch) 
   return ch == 1 ? s : s / (float)ch;
 }
 
-__global__ void __launch_bounds__(256) afp_pcm_frontend_kernel(const int16_t* pcm, int64_t nframes, int ch, int up,
-                                                               int down, const double* taps, int half, float* out,
-                                                               int64_t nout) {
-  const int64_t n = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (n >= nout) return;
-  if (up == 1 && down == 1) {
-    out[n] = mono_at(pcm, n, ch);
-    return;
-  }
+// Output n of one file: the down-mix alone (up = down = 1) or the polyphase FIR over it.  The single-file
+// and the batched kernel both call this, so a file gives the same bits through either entry point.
+__device__ __forceinline__ float frontend_sample(const int16_t* pcm, int64_t nframes, int ch, int up, int down,
+                                                 const double* taps, int half, int64_t n) {
+  if (up == 1 && down == 1) return mono_at(pcm, n, ch);
   const int64_t centre = n * down + half;                 // tap index of input frame j is centre - j*up
   int64_t j_lo = (centre - 2 * (int64_t)half + up - 1) / up;            // ceil((centre - 2 half) / up)
   if (centre - 2 * (int64_t)half < 0) j_lo = 0;
@@ -41,7 +44,48 @@ __global__ void __launch_bounds__(256) afp_pcm_frontend_kernel(const int16_t* pc
   if (j_hi > nframes - 1) j_hi = nframes - 1;
   double acc = 0.0;
   for (int64_t j = j_lo; j <= j_hi; ++j) acc += taps[centre - j * up] * (double)mono_at(pcm, j, ch);
-  out[n] = (float)acc;
+  return (float)acc;
+}
+
+__global__ void __launch_bounds__(256) afp_pcm_frontend_kernel(const int16_t* pcm, int64_t nframes, int ch, int up,
+                                                               int down, const double* taps, int half, float* out,
+                                                               int64_t nout) {
+  const int64_t n = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= nout) return;
+  out[n] = frontend_sample(pcm, nframes, ch, up, down, taps, half, n);
+}
+
+// One file of a batched front-end call, built on the host.
+struct PcmFileDesc {
+  int64_t in_off;       // first int16 of the file in the packed PCM
+  int64_t nframes;
+  int64_t out_off;      // first output sample (a multiple of 4: 16-byte aligned)
+  int64_t nout;         // ceil(nframes * up / down)
+  int64_t tap_off;      // first tap of the file's (up, down) design in the packed taps
+  int64_t block_base;   // first block of the file: the prefix sum of ceil(nout / 256)
+  int32_t ch, up, down, half;
+};
+
+// Block b belongs to the last file whose block_base <= b (a file without outputs has the same base as
+// the next one), found by one thread per block with a binary search over the block prefix.
+__global__ void __launch_bounds__(256) afp_pcm_frontend_batch_kernel(const int16_t* pcm, const PcmFileDesc* files,
+                                                                     int nfiles, const double* taps, float* out) {
+  __shared__ int s_file;
+  const int64_t b = blockIdx.x;
+  if (threadIdx.x == 0) {
+    int lo = 0, hi = nfiles - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (files[mid].block_base <= b) lo = mid; else hi = mid - 1;
+    }
+    s_file = lo;
+  }
+  __syncthreads();
+  const PcmFileDesc& f = files[s_file];
+  const int64_t n = (b - f.block_base) * blockDim.x + threadIdx.x;
+  const int64_t nout = f.nout;
+  if (n >= nout) return;
+  out[f.out_off + n] = frontend_sample(pcm + f.in_off, f.nframes, f.ch, f.up, f.down, taps + f.tap_off, f.half, n);
 }
 
 }  // namespace
@@ -82,5 +126,90 @@ extern "C" int afp_pcm_frontend(afp_ctx* c, const int16_t* pcm, int pcm_on_host,
     AFP_CUDA(c, cudaMemcpyAsync(out, dout, sizeof(float) * (size_t)n_out, cudaMemcpyDeviceToHost, c->stream));
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));
   c->batch_valid = false;     // the PCM staging buffer of the last batch may have been reused
+  return AFP_OK;
+}
+
+extern "C" int afp_pcm_frontend_batch(afp_ctx* c, const int16_t* pcm, int pcm_on_host, int64_t pcm_len, int32_t nfiles,
+                                      const int64_t* pcm_offsets, const int64_t* nframes, const int32_t* channels,
+                                      const int32_t* up, const int32_t* down, int32_t npairs, const int32_t* pair_rates,
+                                      const int64_t* tap_offsets, const double* taps, float* out, int64_t out_capacity,
+                                      int64_t* out_offsets, int64_t* out_lengths) {
+  if (!c) return AFP_ERR_INVALID;
+  if (nfiles < 0 || npairs < 0 || pcm_len < 0) AFP_FAIL(c, AFP_ERR_INVALID, "negative count");
+  if (nfiles > 0 && (!pcm_offsets || !nframes || !channels || !up || !down))
+    AFP_FAIL(c, AFP_ERR_INVALID, "null per-file array");
+  if (npairs > 0 && (!pair_rates || !tap_offsets || !taps)) AFP_FAIL(c, AFP_ERR_INVALID, "null taps table");
+  // the taps table: one odd-length design per distinct (up, down), packed one after the other
+  if (npairs > 0 && tap_offsets[0] != 0) AFP_FAIL(c, AFP_ERR_INVALID, "tap_offsets[0] must be 0");
+  for (int p = 0; p < npairs; ++p) {
+    const int64_t nt = tap_offsets[p + 1] - tap_offsets[p];
+    if (pair_rates[2 * p] < 1 || pair_rates[2 * p + 1] < 1) AFP_FAIL(c, AFP_ERR_INVALID, "taps table: up and down must be >= 1");
+    if (nt < 1 || !(nt & 1) || nt > INT32_MAX) AFP_FAIL(c, AFP_ERR_INVALID, "taps: odd length required");
+  }
+  std::vector<PcmFileDesc> d((size_t)nfiles);
+  int64_t o = 0, blocks = 0;
+  for (int f = 0; f < nfiles; ++f) {
+    PcmFileDesc& x = d[f];
+    x.nframes = nframes[f];
+    x.ch = channels[f];
+    x.up = up[f];
+    x.down = down[f];
+    x.in_off = pcm_offsets[f];
+    if (x.nframes < 0) AFP_FAIL(c, AFP_ERR_INVALID, "file " + std::to_string(f) + ": negative length");
+    if (x.ch < 1) AFP_FAIL(c, AFP_ERR_INVALID, "file " + std::to_string(f) + ": channels must be >= 1");
+    if (x.up < 1 || x.down < 1) AFP_FAIL(c, AFP_ERR_INVALID, "file " + std::to_string(f) + ": up and down must be >= 1");
+    if (x.nframes > 0 && (x.in_off < 0 || x.in_off > pcm_len || x.nframes > (pcm_len - x.in_off) / x.ch))
+      AFP_FAIL(c, AFP_ERR_INVALID, "file " + std::to_string(f) + ": input range outside the PCM buffer");
+    if (x.nframes > (INT64_MAX - x.down) / x.up) AFP_FAIL(c, AFP_ERR_INVALID, "file " + std::to_string(f) + ": too long");
+    x.tap_off = 0;
+    x.half = 0;
+    if (!(x.up == 1 && x.down == 1)) {
+      int p = 0;
+      while (p < npairs && !(pair_rates[2 * p] == x.up && pair_rates[2 * p + 1] == x.down)) ++p;
+      if (p == npairs) AFP_FAIL(c, AFP_ERR_INVALID, "file " + std::to_string(f) + ": no taps for its (up, down)");
+      x.tap_off = tap_offsets[p];
+      x.half = (int32_t)((tap_offsets[p + 1] - tap_offsets[p] - 1) / 2);
+    }
+    x.nout = (x.nframes * x.up + x.down - 1) / x.down;                   // ceil, as resample_poly
+    x.out_off = o;
+    x.block_base = blocks;
+    o += (x.nout + 3) & ~(int64_t)3;
+    blocks += (x.nout + 255) / 256;
+  }
+  if (blocks > INT32_MAX) AFP_FAIL(c, AFP_ERR_INVALID, "batch too large for one launch");
+  if (out) {
+    if (o > out_capacity) AFP_FAIL(c, AFP_ERR_INVALID, "output buffer smaller than the batch's " + std::to_string(o) + " samples");
+    if (blocks > 0 && !pcm) AFP_FAIL(c, AFP_ERR_INVALID, "null pcm");
+  }
+  if (out_offsets) {
+    for (int f = 0; f < nfiles; ++f) out_offsets[f] = d[f].out_off;
+    out_offsets[nfiles] = o;
+  }
+  if (out_lengths)
+    for (int f = 0; f < nfiles; ++f) out_lengths[f] = d[f].nout;
+  if (!out || blocks == 0) return AFP_OK;                                 // sizing call, or nothing to compute
+  AFP_CUDA(c, cudaSetDevice(c->device));
+  const int16_t* dpcm = pcm;
+  if (pcm_on_host) {
+    AFP_CUDA(c, c->d_pcm_stage.reserve(sizeof(int16_t) * (size_t)pcm_len + 16));
+    AFP_CUDA(c, cudaMemcpyAsync(c->d_pcm_stage.p, pcm, sizeof(int16_t) * (size_t)pcm_len, cudaMemcpyHostToDevice,
+                                c->stream));
+    dpcm = c->d_pcm_stage.as<int16_t>();
+    c->batch_valid = false;   // the PCM staging buffer of the last fingerprint batch is overwritten
+  }
+  // descriptors and every distinct design's taps in one upload
+  const size_t desc_bytes = ((sizeof(PcmFileDesc) * (size_t)nfiles + 15) & ~(size_t)15);
+  const size_t tap_bytes = npairs > 0 ? sizeof(double) * (size_t)tap_offsets[npairs] : 0;
+  std::vector<char> h(desc_bytes + tap_bytes);
+  memcpy(h.data(), d.data(), sizeof(PcmFileDesc) * (size_t)nfiles);
+  if (tap_bytes) memcpy(h.data() + desc_bytes, taps, tap_bytes);
+  AFP_CUDA(c, c->d_tmp.reserve(h.size() + 64));
+  AFP_CUDA(c, cudaMemcpyAsync(c->d_tmp.p, h.data(), h.size(), cudaMemcpyHostToDevice, c->stream));
+  const PcmFileDesc* dd = c->d_tmp.as<PcmFileDesc>();
+  const double* dtaps = reinterpret_cast<const double*>(c->d_tmp.as<char>() + desc_bytes);
+  afp_pcm_frontend_batch_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(dpcm, dd, nfiles, dtaps, out);
+  AFP_CUDA(c, cudaGetLastError());
+  c->launches++;
+  AFP_CUDA(c, cudaStreamSynchronize(c->stream));       // one synchronise for the whole list (`h` is pageable)
   return AFP_OK;
 }

@@ -12,7 +12,7 @@ pickling results back.  The same shape is used here:
   merges each into its table on the device, as `multiproc_add` merges its workers'
   tables;
 * matching, table replicated (419 MB << 80 GB): query j -> rank j % world; no
-  collective;
+  data-path collective (`match_files_sharded`, the reference's `match --ncores N`);
 * matching, table sharded by track-id range (SURVEY.md §8e, BASELINE configs[4]):
   every rank sees every query, computes the candidate list and result rows of
   ITS ids, and ONE all-gather of fixed-size per-query records merges them:
@@ -533,3 +533,73 @@ def ingest_sharded(analyzer, ht, names, signals, root=0, replicate=False, report
         if rank != root:
             ht._install_device(DeviceTable(tab.to(dev), cnt.to(dev), obj[0][0], obj[0][1], hb, depth, mtb))
     return counts
+
+
+# ---- matching a list of files against a replicated table (the reference's match --ncores N) ----
+def gather_in_list_order(mine, n, root=0, group=None):
+    """Rank r's results of items r, r + world, r + 2 world, ... (shard_indices) -> the whole list of
+    n results in list order on the root, None on the other ranks: one gather_object."""
+    rank, ws = _group_rank(group)
+    if ws == 1:
+        return list(mine)
+    import torch.distributed as dist
+    book = [None] * ws if rank == root else None
+    dist.gather_object(list(mine), book, dst=_global_rank(group, root), group=group)
+    return interleave_shards(book, n) if rank == root else None
+
+
+def match_files_sharded(matcher, analyzer, ht, filenames, root=0, group=None):
+    """`audfprint.py match --ncores N` (audfprint.py:257-267) over the ranks of a process group, one
+    GPU each, with the same table on every rank (e.g. ingest_sharded(replicate=True), or one database
+    loaded by every rank).  Every rank passes the whole list.
+
+    1. One all-gather of every rank's table geometry (hashbits, depth, maxtimebits) and name count;
+       a mismatch raises ValueError on every rank before any file is read.
+    2. File j goes to rank j % world (shard_indices).  Each rank runs Matcher.files_match_to_msgs on
+       its files, numbering file j as j, and its analyzer counts its own files.
+    3. One all-gather of a status word.  If a rank failed, every rank raises: the same IOError when
+       the failure was an unreadable file (analyzer.fail_on_error), otherwise the failing rank its
+       own exception and the others a RuntimeError naming it.  No rank is left in a collective.
+    4. The root returns the message lists in list order, as joblib returns them; the other ranks
+       return None."""
+    import torch
+    rank, ws = _group_rank(group)
+    root = int(root)
+    if not 0 <= root < ws:
+        raise ValueError("root %d outside the group's %d ranks" % (root, ws))
+    n = len(filenames)
+    info = np.array([int(ht.hashbits), int(ht.depth), int(ht.maxtimebits), len(ht.names)], np.int64)
+    infos = info[None]
+    if ws > 1:
+        import torch.distributed as dist
+        from . import _lib
+        dev = torch.device("cuda", _lib.context(ht.device).device) if dist.get_backend(group) == "nccl" else "cpu"
+        t = torch.from_numpy(info).to(dev)
+        g = torch.empty(ws * len(info), dtype=torch.int64, device=dev)
+        dist.all_gather_into_tensor(g, t, group=group)
+        infos = g.cpu().numpy().reshape(ws, len(info))
+    if (infos != infos[0]).any():
+        raise ValueError("match_files_sharded: the ranks' tables disagree on hashbits / depth / maxtimebits / "
+                         "number of names: %s" % infos.tolist())
+    idx = shard_indices(n, rank, ws)
+    err, mine = None, []
+    try:
+        mine = matcher._files_msgs(analyzer, ht, [filenames[i] for i in idx], [int(i) for i in idx])
+    except Exception as e:          # raised on every rank after the status exchange
+        err = e
+    status = (0, "") if err is None else ((1 if isinstance(err, IOError) else 2), str(err))
+    if ws > 1:
+        import torch.distributed as dist
+        everyone = [None] * ws
+        dist.all_gather_object(everyone, status, group=group)
+    else:
+        everyone = [status]
+    failed = [r for r, st in enumerate(everyone) if st[0]]
+    if failed:
+        if err is not None:
+            raise err
+        kind, msg = everyone[failed[0]]
+        if kind == 1:
+            raise IOError(msg)
+        raise RuntimeError("match_files_sharded: rank %d failed: %s" % (failed[0], msg))
+    return gather_in_list_order(mine, n, root, group)

@@ -26,6 +26,7 @@ import time
 import numpy as np
 
 from . import _lib
+from .analyzer import DeviceHashes
 
 
 def timebits_breaks():
@@ -136,7 +137,8 @@ class Matcher(object):
                  sorted by count descending like match_hashes."""
         if isinstance(queries, tuple):
             packed, qoff = queries
-            packed = np.ascontiguousarray(packed, dtype=np.int32).reshape(-1, 2)
+            if not getattr(packed, "is_cuda", False):       # a torch CUDA tensor (int32 [R][2]) is used in place
+                packed = np.ascontiguousarray(packed, dtype=np.int32).reshape(-1, 2)
             qoff = np.ascontiguousarray(qoff, dtype=np.int64)
         else:
             arrs = [np.asarray(q, dtype=np.int32).reshape(-1, 2) for q in queries]
@@ -467,18 +469,97 @@ class Matcher(object):
         nhashes = len(query)
         seconds = analyzer.n_hop * query[-1][0] / analyzer.target_sr if nhashes else 0.0
         if self.verbose:
-            tag = "#%d" % number if number is not None else ""
-            print(time.ctime(), "Analyzed", tag, filename, "of", ('%.3f' % seconds), "s "
-                  "to", nhashes, "hashes")
+            self._print_analyzed(filename, number, seconds, nhashes)
         rows = self.match_hashes(ht, query)
         if self.sort_by_time:
             rows = rows[(-rows[:, 2]).argsort(), :]
         return rows[:self.max_returns, :], seconds, nhashes
 
+    @staticmethod
+    def _print_analyzed(filename, number, seconds, nhashes):
+        tag = "#%d" % number if number is not None else ""
+        print(time.ctime(), "Analyzed", tag, filename, "of", ('%.3f' % seconds), "s "
+              "to", nhashes, "hashes")
+
+    # files per wavfiles2hashes + match_batch round of match_files
+    max_files_per_call = 2048
+
+    def match_files(self, analyzer, ht, filenames, start=0):
+        """List form of match_file, file i numbered start + i: the same (rows[:max_returns], seconds,
+        nhashes) per file, and the verbose "Analyzed" lines in list order.  Every round of
+        max_files_per_call files is one Analyzer.wavfiles2hashes and one match_batch; when the
+        analyzer and the table share a device the hashes go from the fingerprint workspace to the
+        matcher without leaving it (afp_fetch_hashes into device memory).
+
+        With analyzer.fail_on_error, an unreadable file raises the IOError match_file raises and
+        leaves the analyzer's counters as they were; nothing is returned (the per-file loop would
+        have matched the earlier files by then)."""
+        return self._match_files(analyzer, ht, filenames, range(start, start + len(filenames)))
+
+    def _match_files(self, analyzer, ht, filenames, numbers):
+        self._params()                     # illustrate raises before any file is read
+        saved = (analyzer.soundfiledur, analyzer.soundfiletotaldur, analyzer.soundfilecount)
+        durs = []
+        on_device = hasattr(ht, "_sync_device") and _lib.context(ht.device) is _lib.context(analyzer.device)
+        out = []
+        try:
+            for c0 in range(0, len(filenames), max(1, int(self.max_files_per_call))):
+                names = filenames[c0:c0 + max(1, int(self.max_files_per_call))]
+                queries = analyzer._hashes_of_files(names, rows_on_device=on_device)
+                durs += analyzer.last_batch_durations
+                secs = []
+                for fn, num, q in zip(names, numbers[c0:c0 + len(names)], queries):
+                    nh = len(q)
+                    last = q.last_time if isinstance(q, DeviceHashes) else (q[-1][0] if nh else None)
+                    secs.append(analyzer.n_hop * last / analyzer.target_sr if nh else 0.0)
+                    if self.verbose:
+                        self._print_analyzed(fn, num, secs[-1], nh)
+                for q, sec, rows in zip(queries, secs, self.match_batch(ht, self._pack_queries(queries, on_device))):
+                    if self.sort_by_time:
+                        rows = rows[(-rows[:, 2]).argsort(), :]
+                    out.append((rows[:self.max_returns, :], sec, len(q)))
+        except BaseException:
+            analyzer.soundfiledur, analyzer.soundfiletotaldur, analyzer.soundfilecount = saved
+            raise
+        analyzer.last_batch_durations = durs
+        return out
+
+    @staticmethod
+    def _pack_queries(queries, on_device):
+        """Queries -> what match_batch takes: a host list, or one packed (device rows, offsets) tuple."""
+        if not on_device:
+            return [q for q in queries]
+        import torch
+        dev = next((q.rows.device for q in queries if isinstance(q, DeviceHashes)), None)
+        parts = [q.rows if isinstance(q, DeviceHashes)
+                 else torch.from_numpy(np.asarray(q, np.int32).reshape(-1, 2)) for q in queries]
+        if dev is None:
+            return [np.asarray(q, np.int32).reshape(-1, 2) for q in queries]
+        qoff = np.zeros(len(parts) + 1, np.int64)
+        qoff[1:] = np.cumsum([len(p) for p in parts])
+        packed = torch.cat([p.to(dev) for p in parts]) if qoff[-1] else torch.zeros((0, 2), dtype=torch.int32, device=dev)
+        packed = packed.contiguous()
+        # the library reads `packed` in place on its own (non-blocking) stream: the copies and the
+        # concatenation on torch's stream must be done first
+        torch.cuda.current_stream(dev).synchronize()
+        return packed, qoff
+
     def file_match_to_msgs(self, analyzer, ht, qry, number=None):
         """Match one file and format the reference's report lines
         (audfprint_match.py:381-420)."""
         rows, seconds, nhashes = self.match_file(analyzer, ht, qry, number)
+        return self._msgs(analyzer, ht, qry, rows, seconds, nhashes)
+
+    def files_match_to_msgs(self, analyzer, ht, filenames, start=0):
+        """List form of file_match_to_msgs (match_files, file i numbered start + i): one list of
+        report lines per file, in list order."""
+        return self._files_msgs(analyzer, ht, filenames, range(start, start + len(filenames)))
+
+    def _files_msgs(self, analyzer, ht, filenames, numbers):
+        res = self._match_files(analyzer, ht, filenames, numbers)
+        return [self._msgs(analyzer, ht, fn, *r) for fn, r in zip(filenames, res)]
+
+    def _msgs(self, analyzer, ht, qry, rows, seconds, nhashes):
         frame_s = analyzer.n_hop / analyzer.target_sr
         head = qry
         if self.verbose:

@@ -126,6 +126,29 @@ int afp_get_stage_ms(afp_ctx* ctx, float* ms /* [AFP_NSTAGES] */);
 int afp_pcm_frontend(afp_ctx* ctx, const int16_t* pcm, int pcm_on_host, int64_t nframes, int32_t channels,
                      int32_t up, int32_t down, const double* taps, int32_t ntaps, float* out, int out_on_host,
                      int64_t* nout);
+/* afp_pcm_frontend for a list of files in one launch, every output bit-identical to that file
+ * through afp_pcm_frontend alone (both kernels call one per-output function).
+ *   pcm            packed interleaved int16 of all files, HOST or DEVICE, pcm_len int16 values
+ *   pcm_offsets    HOST int64 [nfiles]: file i's frames start at pcm[pcm_offsets[i]]
+ *   nframes, channels, up, down   HOST [nfiles]: file i's frame count, channel count and rate ratio
+ *   pair_rates     HOST int32 [npairs][2]: the distinct (up, down) of the resampled files
+ *   tap_offsets    HOST int64 [npairs+1], taps HOST float64: pair p's odd-length design (resample_taps)
+ *                  is taps[tap_offsets[p] .. tap_offsets[p+1]); each pair is uploaded once per call
+ *   out            DEVICE float32 of out_capacity samples, or NULL for a sizing call
+ *   out_offsets    HOST int64 [nfiles+1] (may be NULL): file i's ceil(nframes*up/down) outputs start
+ *                  at out[out_offsets[i]], a multiple of 4 (16 bytes); out_offsets[nfiles] is the
+ *                  buffer length the call needs.  out_lengths HOST int64 [nfiles] (may be NULL).
+ * The layout is afp_fingerprint_batch's packed float32 input (sample_offsets = out_offsets,
+ * sample_lengths = out_lengths).  Nothing outside each file's [start, start + length) is written.
+ * Every argument is checked before anything is launched: AFP_ERR_INVALID for a negative length,
+ * channels < 1, up or down < 1, a resampled file whose (up, down) has no taps, an even-length
+ * design, an input range outside [0, pcm_len), or an output larger than out_capacity.  One kernel
+ * launch and one stream synchronise for the whole list; none when no file has an output. */
+int afp_pcm_frontend_batch(afp_ctx* ctx, const int16_t* pcm, int pcm_on_host, int64_t pcm_len, int32_t nfiles,
+                           const int64_t* pcm_offsets, const int64_t* nframes, const int32_t* channels,
+                           const int32_t* up, const int32_t* down, int32_t npairs, const int32_t* pair_rates,
+                           const int64_t* tap_offsets, const double* taps, float* out, int64_t out_capacity,
+                           int64_t* out_offsets, int64_t* out_lengths);
 
 /* ---- Analyzer --------------------------------------------------------------
  * Replaces stft.stft (stft.py:62-94) + Analyzer.find_peaks
