@@ -58,6 +58,7 @@ _SIGS = {
     "afp_fetch_peaks": (C.c_int, [_P, C.c_int32, _P, C.c_int, _I64P]),
     "afp_landmarks_from_peaks": (C.c_int, [_P, _P, C.c_int64, C.c_int, _I64P]),
     "afp_fetch_landmarks": (C.c_int, [_P, _P, C.c_int]),
+    "afp_fingerprint_from_peaks": (C.c_int, [_P, _P, C.c_int, C.c_int32, _I64P, _P, _I64P]),
     "afp_spread_peaks": (C.c_int, [_P, _P, C.c_int32, _P, C.c_double, _P, _P]),
     "afp_stft_mag": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int64, _P, C.c_int]),
     "afp_sgram": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int64, _P, C.c_int]),

@@ -13,6 +13,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 import struct
+import time
 import wave
 
 import numpy as np
@@ -211,6 +212,68 @@ def plan_chunks(frames, nbytes, max_frames, max_bytes):
     if len(frames) > start:
         out.append((start, len(frames)))
     return out
+
+
+def _peak_rows(peaks):
+    """A peak list ((col, bin) pairs) -> contiguous int32 (n, 2)."""
+    return np.ascontiguousarray(np.asarray(peaks, dtype=np.int32).reshape(-1, 2))
+
+
+def precompute_name(filename, precompdir, hashes_not_peaks=True, strip_prefix=None):
+    """Output file of `precompute` for `filename` (audfprint.py:76-93): `strip_prefix` removed when
+    the name starts with it, '.', '..' and empty components dropped (so absolute and relative names
+    land inside `precompdir`), the extension replaced by .afpt (hashes) or .afpk (peaks)."""
+    if strip_prefix and filename[:len(strip_prefix)] == strip_prefix:
+        tail = filename[len(strip_prefix):]
+    else:
+        tail = filename
+    relname = '/'.join([comp for comp in tail.split('/') if comp not in ('.', '..', '')])
+    return os.path.join(precompdir, os.path.splitext(relname)[0] + (PRECOMPEXT if hashes_not_peaks else PRECOMPPKEXT))
+
+
+def _ensure_dir(dirname):
+    """Create `dirname` if it is missing (audfprint.py:55-60, failures ignored as there)."""
+    if not os.path.exists(dirname):
+        try:
+            os.makedirs(dirname)
+        except OSError:
+            pass
+
+
+def _precompute_write(filename, opfname, hashes_not_peaks, output, dur):
+    """Write one precompute result as the reference's saver does (magic, then int32 pairs) and return
+    its message (audfprint.py:105-115)."""
+    if len(output) == 0:
+        return "Zero length analysis for " + filename + " -- not saving."
+    _ensure_dir(os.path.split(opfname)[0])
+    with open(opfname, 'wb') as f:
+        f.write(HASH_MAGIC if hashes_not_peaks else PEAK_MAGIC)
+        np.ascontiguousarray(np.asarray(output, dtype='<i4').reshape(-1, 2)).tofile(f)
+    return "wrote " + opfname + " ( %d %s, %.3f sec)" % (len(output), "hashes" if hashes_not_peaks else "peaks", dur)
+
+
+def next_precompute_round(opnames, start, skip_existing, exists, max_files):
+    """The precompute round that starts at file `start` of a list whose output names are `opnames`
+    -> (end, skipped): files [start, end) are analysed together, those in `skipped` are not.
+
+    The round gives what the per-file loop gives as long as every existence check sees the disk the
+    loop would see.  Outputs are written in list order after the round, so with skip_existing a file
+    whose output name an earlier file of the same round has closes the round before it: the earlier
+    file writes (or, with an empty analysis, does not) before the later one is checked.  Without
+    skip_existing a later file of the same name simply overwrites the earlier one's output.
+    `exists(name)` is the check (os.path.isfile)."""
+    seen, skipped = set(), []
+    i = start
+    while i < len(opnames) and i - start < max_files:
+        name = opnames[i]
+        if skip_existing:
+            if name in seen:
+                break
+            if exists(name):
+                skipped.append(i)
+            seen.add(name)
+        i += 1
+    return i, skipped
 
 
 class DeviceHashes(object):
@@ -517,9 +580,10 @@ class Analyzer(object):
             peaks = self.wavfile2peaks(filename, self.shifts)
             if len(peaks) == 0:
                 return []
-            rows = landmarks2hashes(self.peaks2landmarks(peaks))
-            key = np.unique((rows[:, 0].astype(np.uint64) << np.uint64(32)) + rows[:, 1].astype(np.uint64))
-            return np.stack([key >> np.uint64(32), key & np.uint64(0xFFFFFFFF)], axis=1).astype(np.int32)
+            results = [None]
+            self._fingerprint_peaks([_peak_rows(peaks)])
+            self._collect_hashes([0], results, False, False)
+            return results[0]
         d, sr = self._read(filename)
         self._account(len(d) / sr)
         if len(d) == 0:
@@ -541,13 +605,15 @@ class Analyzer(object):
         WAVs read by the default reader are parsed on the host (_wav_read_raw); the raw PCM of a
         chunk of files is staged once, down-mixed and resampled by ONE afp_pcm_frontend_batch call
         into a device buffer, and fingerprinted there in place (fingerprint_packed).  A custom
-        `reader` is called per file and its output packed as it is.  .afpt / .afpk files take
-        the per-file code.  Chunks follow max_frames_per_call and max_pcm_bytes_per_call (a file
+        `reader` is called per file and its output packed as it is.  Runs of .afpk files are loaded
+        on the host and hashed by ONE afp_fingerprint_from_peaks call per chunk; .afpt files are
+        loaded as they are.  Chunks follow max_frames_per_call and max_pcm_bytes_per_call (a file
         over a cap goes alone); the results do not depend on where they fall.
 
         Files are read in list order.  With fail_on_error, the first unreadable file raises the
         IOError _read raises, and nothing is returned: unlike the per-file loop, which has already
-        returned the earlier files' hashes by then, the counters are left as they were."""
+        returned the earlier files' hashes by then, the counters are left as they were.  A malformed
+        precomputed file raises what wavfile2hashes raises for it, the same way."""
         return self._hashes_of_files(filenames, rows_on_device=False)
 
     def _hashes_of_files(self, filenames, rows_on_device=False):
@@ -556,41 +622,21 @@ class Analyzer(object):
         saved = (self.soundfiledur, self.soundfiletotaldur, self.soundfilecount)
         n = len(filenames)
         results, durs = [None] * n, [0.0] * n
-        nsh = max(1, int(self.shifts))
-        planner = _ChunkPlanner(self.max_frames_per_call, self.max_pcm_bytes_per_call)
-        chunk = []
         try:
-            for i, fn in enumerate(filenames):
-                ext = os.path.splitext(fn)[1]
-                if ext in (PRECOMPEXT, PRECOMPPKEXT):
-                    results[i] = self.wavfile2hashes(fn)
-                    durs[i] = self.soundfiledur
-                    self.soundfiledur, self.soundfiletotaldur, self.soundfilecount = saved
-                    continue
-                if self.reader is _wav_reader:
-                    try:
-                        raw, nch, fs = _wav_read_raw(fn)
-                        if fs < 1:
-                            # the per-file reader fails here in the device front-end (down < 1)
-                            raise ValueError("%s: sample rate %d" % (fn, fs))
-                    except Exception as e:
-                        self._read_failed(fn, e)
-                        raw, nch, fs = np.zeros(0, np.int16), 1, self.target_sr
-                    nout = -(-(len(raw) // nch) * self.target_sr // fs)      # ceil(nframes * up / down)
-                    item = (i, (raw, nch, fs), nout, raw.nbytes)
+            for kind, items in self._file_rounds(filenames, False, max(1, int(self.shifts)), False):
+                idx = [it[0] for it in items]
+                if kind == 'host':
+                    for i, value, dur in items:
+                        results[i], durs[i] = ([] if value is None else value), dur
+                elif kind == 'pcm':
+                    self._fingerprint_pcm(items, self.shifts, durs)
+                    # the reference returns [] when a WAV has no peaks (:401-402)
+                    self._collect_hashes(idx, results, rows_on_device, self.shifts < 2)
                 else:
-                    d, sr = self._read(fn)
-                    durs[i] = len(d) / sr
-                    a = _as_pcm(d)[0] if len(d) else None
-                    item = (i, a, len(d), a.nbytes if a is not None else 0)
-                if item[2] == 0:                                  # nothing to fingerprint: []
-                    results[i] = []
-                    continue
-                if planner.add(nsh * (1 + item[2] // self.n_hop), item[3]):
-                    self._hash_chunk(chunk, results, durs, rows_on_device)
-                    chunk = []
-                chunk.append(item)
-            self._hash_chunk(chunk, results, durs, rows_on_device)
+                    self._fingerprint_peaks([it[1] for it in items])
+                    for i, _, dur in items:
+                        durs[i] = dur
+                    self._collect_hashes(idx, results, rows_on_device, False)
         except BaseException:
             self.soundfiledur, self.soundfiletotaldur, self.soundfilecount = saved
             raise
@@ -599,24 +645,121 @@ class Analyzer(object):
         self.last_batch_durations = durs
         return results
 
-    def _hash_chunk(self, chunk, results, durs, rows_on_device):
-        """Fingerprint one chunk of files [(index, data, nsamples, nbytes)] in one device call and put
-        each file's hashes at its index of `results`."""
-        if not chunk:
-            return
-        idx = [it[0] for it in chunk]
+    def _file_rounds(self, filenames, peaks_mode, nsh, in_order):
+        """Read `filenames` in list order and group them into rounds of one kind, each one device call:
+          ('pcm',   [(i, pcm, nsamples, dur)])  audio for one front-end + fingerprint call (dur None
+                                                until the front-end gives the resampled length)
+          ('peaks', [(i, rows int32 (n,2), dur)]) .afpk files for one afp_fingerprint_from_peaks
+          ('host',  [(i, value, dur)])         files whose result is known on the host: .afpt hashes
+                                                (.afpk peaks with peaks_mode), None for audio without samples
+        A round closes when a cap (max_frames_per_call, max_pcm_bytes_per_call) is reached.  With
+        in_order (a caller that stores in list order) it also closes when the kind changes, so rounds
+        come in list order; otherwise a round of each device kind stays open across the other files
+        and host files pass through as rounds of one.  When reading a file raises, the open rounds
+        (files before it) are yielded first, then the exception propagates, so a caller can finish the
+        earlier files as the per-file loop does.  Audio files count nsh frames per hop against
+        max_frames_per_call."""
+        open_ = {}                                 # kind -> (items, planner) of its open round
+        try:
+            for i, fn in enumerate(filenames):
+                k, item, frames, nbytes = self._read_item(i, fn, nsh, peaks_mode)
+                if k == 'host' and not in_order:
+                    yield k, [item]
+                    continue
+                if in_order and open_ and k not in open_:
+                    for kind, (items, _) in list(open_.items()):
+                        yield kind, items
+                    open_.clear()
+                if k not in open_:
+                    open_[k] = ([], _ChunkPlanner(self.max_frames_per_call, self.max_pcm_bytes_per_call))
+                    open_[k][1].add(frames, nbytes)
+                elif open_[k][1].add(frames, nbytes):
+                    yield k, open_[k][0]
+                    open_[k] = ([], open_[k][1])
+                open_[k][0].append(item)
+        except Exception:
+            for kind, (items, _) in list(open_.items()):
+                yield kind, items
+            raise
+        for kind, (items, _) in list(open_.items()):
+            yield kind, items
+
+    def _read_item(self, i, fn, nsh, peaks_mode):
+        """One file of _file_rounds -> (kind, item, frames, bytes).  Raises what the per-file call
+        raises for a file it cannot read (fail_on_error), before anything is counted."""
+        ext = os.path.splitext(fn)[1]
+        if ext == PRECOMPEXT and not peaks_mode:
+            hashes = hashes_load(fn)
+            return 'host', (i, hashes, np.max(hashes, axis=0)[0] * self.n_hop / self.target_sr), 0, 0
+        if ext == PRECOMPPKEXT:
+            peaks = peaks_load(fn)
+            dur = np.max(peaks, axis=0)[0] * self.n_hop / self.target_sr        # raises for an empty file
+            if peaks_mode:
+                return 'host', (i, peaks, dur), 0, 0
+            rows = _peak_rows(peaks)
+            return 'peaks', (i, rows, dur), max(1, int(rows[-1, 0]) + 1), rows.nbytes
         if self.reader is _wav_reader:
-            raws = [it[1] for it in chunk]
+            try:
+                raw, nch, fs = _wav_read_raw(fn)
+                if fs < 1:
+                    # the per-file reader fails here in the device front-end (down < 1)
+                    raise ValueError("%s: sample rate %d" % (fn, fs))
+            except Exception as e:
+                self._read_failed(fn, e)
+                raw, nch, fs = np.zeros(0, np.int16), 1, self.target_sr
+            nout = -(-(len(raw) // nch) * self.target_sr // fs)      # ceil(nframes * up / down)
+            if nout == 0:
+                return 'host', (i, None, 0.0), 0, 0
+            return 'pcm', (i, (raw, nch, fs), nout, None), nsh * (1 + nout // self.n_hop), raw.nbytes
+        d, sr = self._read(fn)
+        if len(d) == 0:
+            return 'host', (i, None, len(d) / sr), 0, 0
+        a = _as_pcm(d)[0]
+        return 'pcm', (i, a, len(d), len(d) / sr), nsh * (1 + len(d) // self.n_hop), a.nbytes
+
+    def _fingerprint_pcm(self, items, shifts, durs):
+        """Fingerprint one 'pcm' round in one device call at `shifts`; the results stay in the
+        workspace.  Each file's duration goes to durs[i]."""
+        idx = [it[0] for it in items]
+        if self.reader is _wav_reader:
+            raws = [it[1] for it in items]
             out, off, lens = pcm_frontend_batch([r[0] for r in raws], [r[1] for r in raws], [r[2] for r in raws],
                                                 self.target_sr, device=self.device)
             for i, ln in zip(idx, lens):
                 durs[i] = int(ln) / self.target_sr
-            self.fingerprint_packed(out, off, self.shifts, fetch=False, sample_lengths=lens)
+            self.fingerprint_packed(out, off, shifts, fetch=False, sample_lengths=lens)
         else:
-            packed, starts, lens = self._pack([it[1] for it in chunk])
-            self.fingerprint_packed(packed, starts, self.shifts, fetch=False, sample_lengths=lens)
+            for it in items:
+                durs[it[0]] = it[3]
+            packed, starts, lens = self._pack([it[1] for it in items])
+            self.fingerprint_packed(packed, starts, shifts, fetch=False, sample_lengths=lens)
+
+    def _fingerprint_peaks(self, arrays):
+        """wavfile2hashes of many .afpk peak lists (int32 (n,2) each, n >= 1) in ONE
+        afp_fingerprint_from_peaks call; the results stay in the workspace.  When a file's peaks are
+        malformed, raises what the per-file call raises for it, with the file's position in
+        `arrays` as the exception's `file_index`."""
+        ctx = self._configure(max(1, int(self.shifts)))
+        n = len(arrays)
+        off = np.zeros(n + 1, np.int64)
+        off[1:] = np.cumsum([len(a) for a in arrays])
+        rows = np.ascontiguousarray(np.concatenate(arrays), dtype=np.int32) if off[-1] else None
+        status = np.zeros(max(n, 1), np.int32)
+        rc = ctx.lib.afp_fingerprint_from_peaks(ctx.h, rows.ctypes.data if rows is not None else None, 1, n,
+                                                off.ctypes.data_as(C.POINTER(C.c_int64)), status.ctypes.data, None)
+        if rc:
+            try:
+                ctx.check(rc)
+            except Exception as e:
+                if status.any():
+                    e.file_index = int(np.flatnonzero(status)[0])
+                raise
+
+    def _collect_hashes(self, idx, results, rows_on_device, empty_as_list):
+        """Put the hashes of the last device call's files at their indices `idx` of `results`; with
+        empty_as_list a file without hashes gets []."""
         ctx = _lib.context(self.device)
-        roff = np.empty(len(chunk) + 1, np.int64)
+        roff = np.empty(len(idx) + 1, np.int64)
         ctx.check(ctx.lib.afp_fetch_hashes(ctx.h, None, 1, roff.ctypes.data_as(C.POINTER(C.c_int64))))
         total = int(roff[-1])
         if rows_on_device:
@@ -632,18 +775,180 @@ class Analyzer(object):
             ctx.check(ctx.lib.afp_fetch_hashes(ctx.h, rows.ctypes.data, 1, None))
         for k, i in enumerate(idx):
             lo, hi = int(roff[k]), int(roff[k + 1])
-            if self.shifts < 2 and hi == lo:
-                results[i] = []            # the reference returns [] when there are no peaks (:401-402)
+            if empty_as_list and hi == lo:
+                results[i] = []
             elif rows_on_device:
                 results[i] = DeviceHashes(rows[lo:hi], last[k])
             else:
                 results[i] = rows[lo:hi]
+
+    def wavfiles2peaks(self, filenames, shifts=None):
+        """List form of wavfile2peaks: per file exactly what wavfile2peaks(filename, shifts) returns,
+        with the counters and `last_batch_durations` as wavfiles2hashes leaves them.
+
+        Audio goes through the batched front-end and ONE fingerprint call per chunk, at 1 shift when
+        `shifts` is None or < 2, else at self.shifts with min(shifts, self.shifts) peak lists per
+        file (the per-file call's rule); one afp_fetch_peaks per shift serves the whole chunk.
+        .afpk files are loaded on the host; .afpt files are read as audio, as the per-file call
+        reads them.  Failures behave as in wavfiles2hashes."""
+        multi = not (shifts is None or shifts < 2)
+        nsh = max(1, int(self.shifts)) if multi else 1
+        saved = (self.soundfiledur, self.soundfiletotaldur, self.soundfilecount)
+        n = len(filenames)
+        results, durs = [None] * n, [0.0] * n
+        try:
+            for kind, items in self._file_rounds(filenames, True, nsh, False):
+                if kind == 'host':
+                    for i, value, dur in items:
+                        if value is None:
+                            value = [[] for _ in range(shifts)] if multi else []
+                        results[i], durs[i] = value, dur
+                    continue
+                self._fingerprint_pcm(items, nsh, durs)
+                ctx = _lib.context(self.device)
+                if multi:
+                    per_shift = [self._fetch_peaks(ctx, s, len(items)) for s in range(min(shifts, nsh))]
+                    for k, it in enumerate(items):
+                        results[it[0]] = [p[k] for p in per_shift]
+                else:
+                    for it, pk in zip(items, self._fetch_peaks(ctx, 0, len(items))):
+                        results[it[0]] = pk
+        except BaseException:
+            self.soundfiledur, self.soundfiletotaldur, self.soundfilecount = saved
+            raise
+        for dur in durs:
+            self._account(dur)
+        self.last_batch_durations = durs
+        return results
 
     def ingest(self, hashtable, filename):
         """Read a file and add it to the table (audfprint_analyze.py:430-457)."""
         hashes = self.wavfile2hashes(filename)
         hashtable.store(filename, hashes)
         return self.soundfiledur, len(hashes)
+
+    def ingest_files(self, hashtable, filenames):
+        """List form of the reference's `new` / `add` loop (audfprint.py:173-187): returns
+        [self.ingest(hashtable, f) for f in filenames], and leaves the table (table, counts, names,
+        hashesperid), the counters and the `random` state exactly as that loop leaves them.
+
+        Audio chunks are fingerprinted on the device and stored from the workspace in place
+        (HashTable.store_batch_begin(names, None)); runs of .afpk files go through ONE
+        afp_fingerprint_from_peaks call per chunk and are stored the same way; .afpt files and files
+        without samples (unreadable under fail_on_error = False, empty, no peaks) are stored from host
+        rows.  A name takes its id in list order whatever its file yields.  The host replay of
+        random.randint for one round's full buckets runs while the device fingerprints the next round.
+
+        With fail_on_error, an unreadable or malformed file raises what the per-file loop raises, after
+        the files before it (those of its own round included) have been stored: a table cannot be
+        rolled back cheaply, so the state is the loop's state at that point, not the state before."""
+        n = len(filenames)
+        out, durs = [None] * n, [0.0] * n
+        pending = [None]          # (store token, indices) of the round begun and not yet finished
+
+        def finish():
+            if pending[0] is not None:
+                token, idx = pending[0]
+                pending[0] = None
+                for i, cnt in zip(idx, hashtable.store_batch_finish(token)):
+                    out[i] = (durs[i], cnt)
+                    self._account(durs[i])
+
+        def begin(idx, hashes):
+            finish()
+            pending[0] = (hashtable.store_batch_begin([filenames[i] for i in idx], hashes), idx)
+
+        try:
+            for kind, items in self._file_rounds(filenames, False, max(1, int(self.shifts)), True):
+                idx = [it[0] for it in items]
+                if kind == 'host':
+                    for i, _, dur in items:
+                        durs[i] = dur
+                    begin(idx, [[] if it[1] is None else it[1] for it in items])
+                    continue
+                if kind == 'pcm':
+                    self._fingerprint_pcm(items, self.shifts, durs)
+                else:
+                    for i, _, dur in items:
+                        durs[i] = dur
+                    try:
+                        self._fingerprint_peaks([it[1] for it in items])
+                    except Exception as e:
+                        k = getattr(e, 'file_index', None)
+                        if k is None:
+                            raise
+                        # the loop stores the files before the malformed one, and has counted it
+                        if k:
+                            self._fingerprint_peaks([it[1] for it in items[:k]])
+                            begin(idx[:k], None)
+                        finish()
+                        self._account(durs[idx[k]])
+                        raise e
+                begin(idx, None)
+            finish()
+        except BaseException:
+            finish()
+            raise
+        return out
+
+    # files analysed together by one precompute_files round
+    max_files_per_precompute = 4096
+
+    def precompute_file(self, filename, precompdir, type='hashes', skip_existing=False, strip_prefix=None):
+        """`precompute` of one file (file_precompute + file_precompute_peaks_or_hashes,
+        audfprint.py:70-127): writes `precompdir`/name.afpt (type 'hashes') or .afpk (any other
+        type: peaks) and returns the one-message list the reference returns."""
+        print(time.ctime(), "precomputing", type, "for", filename, "...")
+        return self._precompute_one(filename, precompdir, type, skip_existing, strip_prefix)
+
+    def _precompute_one(self, filename, precompdir, type, skip_existing, strip_prefix):
+        hashes = type == 'hashes'
+        opfname = precompute_name(filename, precompdir, hashes, strip_prefix)
+        if skip_existing and os.path.isfile(opfname):
+            return ["file " + opfname + " exists (and --skip-existing); skipping"]
+        output = self.wavfile2hashes(filename) if hashes else self.wavfile2peaks(filename)
+        return [_precompute_write(filename, opfname, hashes, output, self.soundfiledur)]
+
+    def precompute_files(self, filenames, precompdir, type='hashes', skip_existing=False, strip_prefix=None):
+        """List form of precompute_file: one message list per file, and the very files the per-file
+        loop writes, byte for byte, including two effects of its order: with skip_existing a file
+        whose output an earlier file of the list wrote is skipped, and a later file with the same
+        output name overwrites an earlier one.
+
+        The list is cut into rounds (next_precompute_round) of at most max_files_per_precompute
+        files; each round prints file_precompute's "precomputing" line for its files in list order,
+        analyses the files it does not skip with ONE wavfiles2hashes / wavfiles2peaks call, and
+        writes them in list order.  When that call raises (fail_on_error), the round runs file by
+        file instead, so that the files before the failing one are written and the per-file
+        exception is raised, as in the loop."""
+        hashes = type == 'hashes'
+        n = len(filenames)
+        opnames = [precompute_name(f, precompdir, hashes, strip_prefix) for f in filenames]
+        msgs = [None] * n
+        start = 0
+        while start < n:
+            end, skipped = next_precompute_round(opnames, start, skip_existing, os.path.isfile,
+                                                 max(1, int(self.max_files_per_precompute)))
+            for i in range(start, end):
+                print(time.ctime(), "precomputing", type, "for", filenames[i], "...")
+            skipped = set(skipped)
+            todo = [i for i in range(start, end) if i not in skipped]
+            try:
+                names = [filenames[i] for i in todo]
+                outs = self.wavfiles2hashes(names) if hashes else self.wavfiles2peaks(names)
+            except Exception:
+                for i in range(start, end):
+                    msgs[i] = self._precompute_one(filenames[i], precompdir, type, skip_existing, strip_prefix)
+                start = end
+                continue
+            durs = self.last_batch_durations
+            for i in range(start, end):
+                if i in skipped:
+                    msgs[i] = ["file " + opnames[i] + " exists (and --skip-existing); skipping"]
+            for k, i in enumerate(todo):
+                msgs[i] = [_precompute_write(filenames[i], opnames[i], hashes, outs[k], durs[k])]
+            start = end
+        return msgs
 
     # ---- parity probes -------------------------------------------------------------
     def stft_magnitude(self, d):

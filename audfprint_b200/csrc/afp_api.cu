@@ -73,7 +73,7 @@ void afp_destroy(afp_ctx* c) {
                     &c->d_logs, &c->d_nyq, &c->d_tile_stats, &c->d_item_stats, &c->d_fwd_val, &c->d_fwd_bin,
                     &c->d_fwd_cnt, &c->d_pk_bin, &c->d_pk_cnt, &c->d_item_scols, &c->d_item_npeaks, &c->d_lm,
                     &c->d_col_cnt, &c->d_file_tot, &c->d_file_off, &c->d_hashes, &c->d_pk_off, &c->d_pk_rows,
-                    &c->d_tmp, &c->tab.table, &c->tab.counts, &c->tab.hashesperid, &c->d_q, &c->d_qoff,
+                    &c->d_pk_in, &c->d_pk_inoff, &c->d_pk_status, &c->d_tmp, &c->tab.table, &c->tab.counts, &c->tab.hashesperid, &c->d_q, &c->d_qoff,
                     &c->d_hit_off, &c->d_hits, &c->d_st_off, &c->d_st_ids, &c->d_st_eval, &c->d_st_seq, &c->d_st_ovf,
                     &c->d_st_cnt, &c->d_st_seg, &c->d_st_heavy, &c->d_st_part, &c->d_st_scan, &c->d_st_obkt,
                     &c->d_st_opos, &c->d_st_oval, &c->d_st_slot, &c->d_st_last, &c->d_mfast, &c->d_mqlist, &c->d_mscratch, &c->d_mrows, &c->d_mrow_cnt,
@@ -448,6 +448,137 @@ int afp_fingerprint_from_logs(afp_ctx* c, const void* logs, int logs_on_host, in
                                 cudaMemcpyDeviceToHost, c->stream));
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));   // `st` and host logs must outlive their copies
   if (total_hashes) *total_hashes = c->total_hashes;
+  return AFP_OK;
+}
+
+int afp_fingerprint_from_peaks(afp_ctx* c, const int32_t* peak_rows, int rows_on_host, int32_t nfiles,
+                               const int64_t* peak_offsets, int32_t* file_status, int64_t* total_hashes) {
+  if (!c) return AFP_ERR_INVALID;
+  if (!c->analyzer_set) AFP_FAIL(c, AFP_ERR_STATE, "afp_set_analyzer has not been called");
+  if (nfiles < 0 || (nfiles > 0 && !peak_offsets)) AFP_FAIL(c, AFP_ERR_INVALID, "null peak offsets");
+  const int64_t* off = peak_offsets;
+  if (nfiles > 0 && off[0] < 0) AFP_FAIL(c, AFP_ERR_INVALID, "peak_offsets[0] must be >= 0");
+  for (int f = 0; f < nfiles; ++f)
+    if (off[f + 1] < off[f]) AFP_FAIL(c, AFP_ERR_INVALID, "peak_offsets must be non-decreasing");
+  const int64_t row0 = nfiles > 0 ? off[0] : 0, nrows = nfiles > 0 ? off[nfiles] - off[0] : 0;
+  if (nrows > 0 && !peak_rows) AFP_FAIL(c, AFP_ERR_INVALID, "null peak rows");
+  AFP_CUDA(c, cudaSetDevice(c->device));
+  c->batch_valid = false;
+  c->ev_valid = false;
+  c->total_hashes = -1;
+  c->nlandmarks = -1;   // d_hashes is rewritten
+  const int S = c->ap.shifts;
+  const size_t P = (size_t)c->ap.maxpksperframe, F = (size_t)c->ap.maxpairsperpeak;
+  AFP_CUDA(c, c->d_pk_inoff.reserve(sizeof(int64_t) * (size_t)(nfiles + 1)));
+  AFP_CUDA(c, c->d_pk_status.reserve(sizeof(int32_t) * (size_t)(nfiles + 1)));
+  // device rows are read in place at the caller's offsets; host rows are staged from row off[0], so
+  // their offsets go to the device relative to it
+  const bool staged = nrows > 0 && rows_on_host;
+  std::vector<int64_t> doff(off, off + (nfiles > 0 ? nfiles + 1 : 0));
+  if (staged)
+    for (int64_t& o : doff) o -= row0;
+  if (nfiles > 0)
+    AFP_CUDA(c, cudaMemcpyAsync(c->d_pk_inoff.p, doff.data(), sizeof(int64_t) * doff.size(), cudaMemcpyHostToDevice,
+                                c->stream));
+  const int32_t* drows = peak_rows;
+  std::vector<int32_t> last((size_t)nfiles, -1);
+  if (staged) {
+    AFP_CUDA(c, c->d_pk_in.reserve(sizeof(int32_t) * 2 * (size_t)nrows));
+    AFP_CUDA(c, cudaMemcpyAsync(c->d_pk_in.p, peak_rows + 2 * row0, sizeof(int32_t) * 2 * (size_t)nrows,
+                                cudaMemcpyHostToDevice, c->stream));
+    drows = c->d_pk_in.as<int32_t>();
+    for (int f = 0; f < nfiles; ++f)
+      if (off[f + 1] > off[f]) last[(size_t)f] = peak_rows[2 * (off[f + 1] - 1)];
+  } else if (nrows > 0) {
+    int rc = afp_launch_peak_last_cols(c, drows, c->d_pk_inoff.as<int64_t>(), nfiles, c->d_pk_status.as<int32_t>());
+    if (rc) return rc;
+    AFP_CUDA(c, cudaMemcpyAsync(last.data(), c->d_pk_status.p, sizeof(int32_t) * (size_t)nfiles,
+                                cudaMemcpyDeviceToHost, c->stream));
+    AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+  }
+  // one item of T_f = last column + 1 columns per file (:321); shift items 1..S-1 are empty.  A last
+  // column outside [0, 2^28] gives T_f = 0, so that every row of the file fails the scatter's bounds.
+  c->nfiles = nfiles;
+  c->nitems = nfiles * S;
+  c->h_items.assign((size_t)c->nitems, ItemDesc{});
+  c->h_file_col_base.resize((size_t)nfiles + 1);
+  std::vector<int32_t> scols((size_t)c->nitems + 1, 0), npeaks((size_t)c->nitems + 1, 0);
+  int64_t cols = 0;
+  for (int f = 0; f < nfiles; ++f) {
+    const int32_t lc = last[(size_t)f];
+    const int32_t T = (lc >= 0 && lc <= (1 << 28)) ? lc + 1 : 0;
+    c->h_file_col_base[(size_t)f] = cols;
+    for (int s = 0; s < S; ++s) {
+      ItemDesc& it = c->h_items[(size_t)f * S + s];
+      it.frame_base = s == 0 ? cols : cols + T;
+      it.nframes = s == 0 ? T : 0;
+    }
+    scols[(size_t)f * S] = T;
+    const int64_t np = off[f + 1] - off[f];
+    npeaks[(size_t)f * S] = np > 0x7fffffff ? 0x7fffffff : (int32_t)np;
+    cols += T;
+  }
+  c->h_file_col_base[(size_t)nfiles] = cols;
+  c->total_frames = cols;
+  c->total_tiles = 0;
+  c->total_cols = cols;
+  // only what the scatter and K3 read: pk slots, landmark slots, column counts, file offsets
+  const size_t fr = (size_t)cols + 1;
+  AFP_CUDA(c, c->d_items.reserve(sizeof(ItemDesc) * (size_t)(c->nitems + 1)));
+  AFP_CUDA(c, c->d_file_col_base.reserve(sizeof(int64_t) * (size_t)(nfiles + 1)));
+  AFP_CUDA(c, c->d_item_scols.reserve(sizeof(int32_t) * scols.size()));
+  AFP_CUDA(c, c->d_item_npeaks.reserve(sizeof(int32_t) * npeaks.size()));
+  AFP_CUDA(c, c->d_pk_bin.reserve(P * fr));
+  AFP_CUDA(c, c->d_pk_cnt.reserve(fr));
+  AFP_CUDA(c, c->d_lm.reserve(sizeof(uint32_t) * P * F * fr));
+  AFP_CUDA(c, c->d_col_cnt.reserve(sizeof(int32_t) * fr));
+  AFP_CUDA(c, c->d_file_tot.reserve(sizeof(int32_t) * (size_t)(nfiles + 1)));
+  AFP_CUDA(c, c->d_file_off.reserve(sizeof(int64_t) * (size_t)(nfiles + 1)));
+  if (c->nitems > 0)
+    AFP_CUDA(c, cudaMemcpyAsync(c->d_items.p, c->h_items.data(), sizeof(ItemDesc) * (size_t)c->nitems,
+                                cudaMemcpyHostToDevice, c->stream));
+  AFP_CUDA(c, cudaMemcpyAsync(c->d_file_col_base.p, c->h_file_col_base.data(), sizeof(int64_t) * (size_t)(nfiles + 1),
+                              cudaMemcpyHostToDevice, c->stream));
+  AFP_CUDA(c, cudaMemcpyAsync(c->d_item_scols.p, scols.data(), sizeof(int32_t) * scols.size(), cudaMemcpyHostToDevice,
+                              c->stream));
+  AFP_CUDA(c, cudaMemcpyAsync(c->d_item_npeaks.p, npeaks.data(), sizeof(int32_t) * npeaks.size(),
+                              cudaMemcpyHostToDevice, c->stream));
+  AFP_CUDA(c, cudaMemsetAsync(c->d_pk_cnt.p, 0, fr, c->stream));
+  AFP_CUDA(c, cudaMemsetAsync(c->d_pk_status.p, 0, sizeof(int32_t) * (size_t)(nfiles + 1), c->stream));
+  if (nfiles == 0) AFP_CUDA(c, cudaMemsetAsync(c->d_file_off.p, 0, sizeof(int64_t), c->stream));
+  // the scatter never writes pk_cnt above maxpks, so K3 runs safely before the status is read: one sync
+  int rc = afp_launch_scatter_peaks(c, drows, c->d_pk_inoff.as<int64_t>(), nrows, nfiles, S,
+                                    c->d_pk_status.as<int32_t>());
+  if (!rc) rc = afp_launch_landmarks(c, 0, c->nitems);
+  if (!rc) rc = afp_launch_hashes(c);
+  if (rc) return rc;
+  std::vector<int32_t> st((size_t)nfiles + 1, 0);
+  int64_t total = 0;
+  if (nfiles > 0) {
+    AFP_CUDA(c, cudaMemcpyAsync(st.data(), c->d_pk_status.p, sizeof(int32_t) * (size_t)nfiles, cudaMemcpyDeviceToHost,
+                                c->stream));
+    AFP_CUDA(c, cudaMemcpyAsync(&total, c->d_file_off.as<int64_t>() + nfiles, sizeof(int64_t), cudaMemcpyDeviceToHost,
+                                c->stream));
+  }
+  AFP_CUDA(c, cudaStreamSynchronize(c->stream));   // also: the host vectors above outlive their copies
+  int first = -1;
+  for (int f = 0; f < nfiles; ++f) {
+    st[(size_t)f] = afp_peak_status_code(st[(size_t)f]);
+    if (file_status) file_status[f] = st[(size_t)f];
+    if (st[(size_t)f] && first < 0) first = f;
+  }
+  if (first >= 0) {
+    c->err = "file " + std::to_string(first) +
+             (st[(size_t)first] == AFP_ERR_INVALID
+                  ? ": peak rows must be (col, bin) in [0,T)x[0,256), column-major, bins ascending"
+                  : ": more peaks in one column than maxpksperframe");
+    return st[(size_t)first];
+  }
+  AFP_CUDA(c, c->d_hashes.reserve(sizeof(int32_t) * 2 * (size_t)(total + 1)));
+  if ((rc = afp_write_hashes(c))) return rc;
+  c->batch_valid = true;
+  c->total_hashes = total;
+  if (total_hashes) *total_hashes = total;
   return AFP_OK;
 }
 

@@ -196,24 +196,49 @@ __global__ void __launch_bounds__(1024) afp_scan_kernel(const int32_t* in, int64
   if (tid == 0) out[n] = s_run;
 }
 
-// ---- explicit peak list -> landmark rows (Analyzer.peaks2landmarks as a call) ---
-__global__ void afp_scatter_peaks_kernel(const int32_t* rows, int64_t n, int maxpks, int T, uint8_t* pk_bin,
-                                         uint8_t* pk_cnt, int* err) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
+// ---- explicit peak lists -> K2's output layout (peaks2landmarks / .afpk hashing as calls) ----
+// One thread per peak row of a ragged batch: rows[off[f] .. off[f+1]) are file f's (col, bin) pairs,
+// rows indexed absolutely (row off[0] is the first).  The row finds its file by binary search over
+// `off` (the largest f with off[f] <= row: empty files share their offset with the next file) and
+// lands at the file's frame_base + col in pk_bin / pk_cnt, in the slot its rank in the column gives.
+// status[f] collects PK_BAD_LAYOUT (a column outside [0, T_f) or a bin outside [0, 256), or rows not
+// column-major with bins ascending) and PK_TOO_MANY (more than maxpks peaks in one column); a row that
+// sets either writes nothing, so pk_cnt never exceeds maxpks whatever the input.
+constexpr int PK_BAD_LAYOUT = 1, PK_TOO_MANY = 2;
+
+__global__ void __launch_bounds__(256) afp_scatter_peaks_kernel(const int32_t* rows, const int64_t* off, int nfiles,
+                                                               const ItemDesc* items, int item_stride, int maxpks,
+                                                               uint8_t* pk_bin, uint8_t* pk_cnt, int32_t* status) {
+  const int64_t i = off[0] + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= off[nfiles]) return;
+  int f = 0, hi = nfiles;
+  while (hi - f > 1) {
+    const int mid = (f + hi) >> 1;
+    if (off[mid] <= i) f = mid; else hi = mid;
+  }
+  const int64_t b = off[f];
+  const ItemDesc it = items[(int64_t)f * item_stride];   // nframes = T_f = last peak column + 1
   const int col = rows[2 * i], bin = rows[2 * i + 1];
-  if (col < 0 || col >= T || bin < 0 || bin >= AFP_NBINS) { atomicExch(err, 1); return; }
-  if (i > 0 && (rows[2 * (i - 1)] > col || (rows[2 * (i - 1)] == col && rows[2 * (i - 1) + 1] >= bin))) {
-    atomicExch(err, 2);   // not sorted column-major / bins ascending
+  if (col < 0 || col >= it.nframes || bin < 0 || bin >= AFP_NBINS ||
+      (i > b && (rows[2 * (i - 1)] > col || (rows[2 * (i - 1)] == col && rows[2 * (i - 1) + 1] >= bin)))) {
+    atomicOr(&status[f], PK_BAD_LAYOUT);
     return;
   }
   int slot = 0;
-  while (i - slot - 1 >= 0 && rows[2 * (i - slot - 1)] == col) {
-    ++slot;
-    if (slot >= maxpks) { atomicExch(err, 3); return; }
+  while (i - slot - 1 >= b && rows[2 * (i - slot - 1)] == col) {
+    if (++slot >= maxpks) {
+      atomicOr(&status[f], PK_TOO_MANY);
+      return;
+    }
   }
-  pk_bin[(int64_t)col * maxpks + slot] = (uint8_t)bin;
-  if (i == n - 1 || rows[2 * (i + 1)] != col) pk_cnt[col] = (uint8_t)(slot + 1);
+  pk_bin[(it.frame_base + col) * maxpks + slot] = (uint8_t)bin;
+  if (i + 1 == off[f + 1] || rows[2 * (i + 1)] != col) pk_cnt[it.frame_base + col] = (uint8_t)(slot + 1);
+}
+
+// Column of each non-empty file's last row (-1 for an empty file): its T_f - 1 (:321).
+__global__ void afp_peak_last_col_kernel(const int32_t* rows, const int64_t* off, int nfiles, int32_t* out) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f < nfiles) out[f] = off[f + 1] > off[f] ? rows[2 * (off[f + 1] - 1)] : -1;
 }
 
 template <bool WRITE>
@@ -266,6 +291,29 @@ static HashArgs make_args(afp_ctx* c) {
   return a;
 }
 
+int afp_peak_status_code(int32_t bits) {
+  return (bits & PK_BAD_LAYOUT) ? AFP_ERR_INVALID : (bits & PK_TOO_MANY) ? AFP_ERR_UNSUPPORTED : AFP_OK;
+}
+
+int afp_launch_peak_last_cols(afp_ctx* c, const int32_t* rows, const int64_t* off, int32_t nfiles, int32_t* out) {
+  if (nfiles <= 0) return AFP_OK;
+  afp_peak_last_col_kernel<<<(nfiles + 255) / 256, 256, 0, c->stream>>>(rows, off, nfiles, out);
+  AFP_CUDA(c, cudaGetLastError());
+  c->launches++;
+  return AFP_OK;
+}
+
+int afp_launch_scatter_peaks(afp_ctx* c, const int32_t* rows, const int64_t* off, int64_t nrows, int32_t nfiles,
+                             int item_stride, int32_t* status) {
+  if (nrows <= 0) return AFP_OK;
+  afp_scatter_peaks_kernel<<<(unsigned)((nrows + 255) / 256), 256, 0, c->stream>>>(
+      rows, off, nfiles, c->d_items.as<ItemDesc>(), item_stride, c->ap.maxpksperframe, c->d_pk_bin.as<uint8_t>(),
+      c->d_pk_cnt.as<uint8_t>(), status);
+  AFP_CUDA(c, cudaGetLastError());
+  c->launches++;
+  return AFP_OK;
+}
+
 int afp_landmarks_from_peaks_impl(afp_ctx* c, const int32_t* rows_in, int64_t n, int on_host, int64_t* nlm) {
   c->batch_valid = false;
   c->nlandmarks = -1;
@@ -273,9 +321,10 @@ int afp_landmarks_from_peaks_impl(afp_ctx* c, const int32_t* rows_in, int64_t n,
   const int32_t* drows = rows_in;
   int32_t last[2];
   if (on_host) {
-    AFP_CUDA(c, c->d_q.reserve(sizeof(int32_t) * 2 * (size_t)n));
-    AFP_CUDA(c, cudaMemcpyAsync(c->d_q.p, rows_in, sizeof(int32_t) * 2 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
-    drows = c->d_q.as<int32_t>();
+    AFP_CUDA(c, c->d_pk_in.reserve(sizeof(int32_t) * 2 * (size_t)n));
+    AFP_CUDA(c, cudaMemcpyAsync(c->d_pk_in.p, rows_in, sizeof(int32_t) * 2 * (size_t)n, cudaMemcpyHostToDevice,
+                                c->stream));
+    drows = c->d_pk_in.as<int32_t>();
     last[0] = rows_in[2 * (n - 1)];
   } else {
     AFP_CUDA(c, cudaMemcpyAsync(last, rows_in + 2 * (n - 1), sizeof(last), cudaMemcpyDeviceToHost, c->stream));
@@ -294,17 +343,17 @@ int afp_landmarks_from_peaks_impl(afp_ctx* c, const int32_t* rows_in, int64_t n,
   AFP_CUDA(c, c->d_col_cnt.reserve(sizeof(int32_t) * fr));
   AFP_CUDA(c, c->d_file_tot.reserve(sizeof(int32_t) * 4));
   AFP_CUDA(c, c->d_file_col_base.reserve(sizeof(int64_t) * 2));
-  AFP_CUDA(c, c->d_tmp.reserve(64));
-  const int64_t fcb[2] = {0, T};
+  AFP_CUDA(c, c->d_pk_inoff.reserve(sizeof(int64_t) * 2));
+  AFP_CUDA(c, c->d_pk_status.reserve(sizeof(int32_t) * 2));
+  const int64_t fcb[2] = {0, T}, off[2] = {0, n};
   AFP_CUDA(c, cudaMemcpyAsync(c->d_items.p, &it, sizeof(it), cudaMemcpyHostToDevice, c->stream));
   AFP_CUDA(c, cudaMemcpyAsync(c->d_file_col_base.p, fcb, sizeof(fcb), cudaMemcpyHostToDevice, c->stream));
+  AFP_CUDA(c, cudaMemcpyAsync(c->d_pk_inoff.p, off, sizeof(off), cudaMemcpyHostToDevice, c->stream));
   AFP_CUDA(c, cudaMemcpyAsync(c->d_item_scols.p, &T, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
   AFP_CUDA(c, cudaMemsetAsync(c->d_pk_cnt.p, 0, fr, c->stream));
-  AFP_CUDA(c, cudaMemsetAsync(c->d_tmp.p, 0, sizeof(int), c->stream));
-  afp_scatter_peaks_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c->stream>>>(
-      drows, n, (int)P, T, c->d_pk_bin.as<uint8_t>(), c->d_pk_cnt.as<uint8_t>(), c->d_tmp.as<int>());
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
+  AFP_CUDA(c, cudaMemsetAsync(c->d_pk_status.p, 0, sizeof(int32_t), c->stream));
+  int rc = afp_launch_scatter_peaks(c, drows, c->d_pk_inoff.as<int64_t>(), n, 1, 1, c->d_pk_status.as<int32_t>());
+  if (rc) return rc;
   c->nfiles = 1; c->nitems = 1; c->total_frames = T; c->total_cols = T;
   HashArgs a = make_args(c);
   AFP_CUDA(c, cudaMemsetAsync(c->d_lm.p, 0xFF, sizeof(uint32_t) * P * F * fr, c->stream));
@@ -315,13 +364,13 @@ int afp_landmarks_from_peaks_impl(afp_ctx* c, const int32_t* rows_in, int64_t n,
   afp_file_scan_kernel<<<1, 256, 0, c->stream>>>(a);
   AFP_CUDA(c, cudaGetLastError());
   c->launches += 3;
-  int32_t total = 0;
-  int err = 0;
+  int32_t total = 0, err = 0;
   AFP_CUDA(c, cudaMemcpyAsync(&total, c->d_file_tot.p, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-  AFP_CUDA(c, cudaMemcpyAsync(&err, c->d_tmp.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  AFP_CUDA(c, cudaMemcpyAsync(&err, c->d_pk_status.p, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));
-  if (err == 3) AFP_FAIL(c, AFP_ERR_UNSUPPORTED, "more peaks in one column than maxpksperframe");
-  if (err) AFP_FAIL(c, AFP_ERR_INVALID, "peak rows must be (col, bin) in [0,T)x[0,256), column-major, bins ascending");
+  if (afp_peak_status_code(err) == AFP_ERR_INVALID)
+    AFP_FAIL(c, AFP_ERR_INVALID, "peak rows must be (col, bin) in [0,T)x[0,256), column-major, bins ascending");
+  if (err) AFP_FAIL(c, AFP_ERR_UNSUPPORTED, "more peaks in one column than maxpksperframe");
   AFP_CUDA(c, c->d_hashes.reserve(sizeof(int32_t) * 4 * (size_t)(total + 1)));
   if (total > 0) {
     afp_lm_rows_kernel<true><<<(T + 127) / 128, 128, 0, c->stream>>>(a.lm, T, (int)(P * F), a.col_cnt,

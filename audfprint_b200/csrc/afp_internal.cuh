@@ -119,6 +119,9 @@ struct afp_ctx {
   int64_t nlandmarks = -1;   // afp_landmarks_from_peaks result (rows in d_hashes)
   DevBuf d_pk_off;         // int64 [nfiles+1] (peak fetch)
   DevBuf d_pk_rows;        // int32 [total][2]
+  DevBuf d_pk_in;          // int32 [rows][2]  host peak rows staged for afp_fingerprint_from_peaks / afp_landmarks_from_peaks
+  DevBuf d_pk_inoff;       // int64 [nfiles+1] their per-file offsets
+  DevBuf d_pk_status;      // int32 [nfiles]   per-file PK_* flags of the peak scatter (afp_hash.cu)
   DevBuf d_tmp;            // misc
 
   // table + matching
@@ -199,6 +202,11 @@ int afp_launch_landmarks(afp_ctx* c, int item0, int nitems);
 int afp_launch_hashes(afp_ctx* c);   // merge / scans (all files)
 int afp_write_hashes(afp_ctx* c);
 int afp_landmarks_from_peaks_impl(afp_ctx* c, const int32_t* rows, int64_t n, int on_host, int64_t* nlm);
+// peak rows of a ragged batch -> pk_bin / pk_cnt at each file's item (items f * item_stride of d_items)
+int afp_launch_scatter_peaks(afp_ctx* c, const int32_t* rows, const int64_t* off, int64_t nrows, int32_t nfiles,
+                             int item_stride, int32_t* status);
+int afp_launch_peak_last_cols(afp_ctx* c, const int32_t* rows, const int64_t* off, int32_t nfiles, int32_t* out);
+int afp_peak_status_code(int32_t bits);   // a file's scatter flags -> AFP_OK / AFP_ERR_INVALID / AFP_ERR_UNSUPPORTED
 int afp_compact_peaks(afp_ctx* c, int shift);
 int afp_spread_peaks_impl(afp_ctx* c, const double* vector, int32_t n, const double* table, double width,
                           const double* base, double* out);

@@ -431,15 +431,27 @@ def ingest_sharded(analyzer, ht, names, signals, root=0, replicate=False, report
        as its device copy (afp_table_upload from device memory) with the same names and hashesperid.
        Otherwise the other ranks' `ht` are unchanged.  np.random advances on the root only.
     Returns the number of hashes stored for each of this rank's files."""
+    _check_root(root, group)
+    if len(names) != len(signals):
+        raise ValueError("%d names for %d signals" % (len(names), len(signals)))
+    return _ingest_and_merge(lambda local: analyzer.ingest_batch(local, list(names), list(signals)), ht, int(root),
+                             replicate, report, group, False)
+
+
+def _check_root(root, group):
+    rank, ws = _group_rank(group)
+    if not 0 <= int(root) < ws:
+        raise ValueError("root %d outside the group's %d ranks" % (int(root), ws))
+
+
+def _ingest_and_merge(ingest, ht, root, replicate, report, group, io_errors_everywhere):
+    """Steps 1-6 of ingest_sharded, with step 1 as `ingest(local_table)` -> this rank's result.  With
+    io_errors_everywhere an IOError raised by one rank's ingest is raised, with its message, on every
+    rank (an unreadable file under fail_on_error); otherwise the others raise a RuntimeError."""
     import torch
     from . import _lib
     from .hash_table import DeviceTable, HashTable
     rank, ws = _group_rank(group)
-    root = int(root)
-    if not 0 <= root < ws:
-        raise ValueError("root %d outside the group's %d ranks" % (root, ws))
-    if len(names) != len(signals):
-        raise ValueError("%d names for %d signals" % (len(names), len(signals)))
     ctx = _lib.context(ht.device)
     dev = torch.device("cuda", ctx.device)
     nccl = False
@@ -452,7 +464,7 @@ def ingest_sharded(analyzer, ht, names, signals, root=0, replicate=False, report
     local = HashTable(hashbits=hb, depth=depth, maxtime=1 << mtb, device=ht.device)
     err, mine, counts = None, None, []
     try:
-        counts = analyzer.ingest_batch(local, list(names), list(signals))
+        counts = ingest(local)
         mine = local.export_device()
     except Exception as e:          # raised on every rank after the all-gather
         err = e
@@ -462,7 +474,8 @@ def ingest_sharded(analyzer, ht, names, signals, root=0, replicate=False, report
     nhashes = int(mine.counts.sum(dtype=torch.int64)) if mine is not None else 0
 
     # 2. status, name and hash counts, the root's base and geometry, from every rank
-    info = np.array([0 if err is None else 1, len(mine.names) if mine is not None else 0, nhashes,
+    code = 0 if err is None else 2 if (io_errors_everywhere and isinstance(err, IOError)) else 1
+    info = np.array([code, len(mine.names) if mine is not None else 0, nhashes,
                      len(ht.names), hb, depth, mtb], np.int64)
     if ws > 1:
         t = torch.from_numpy(info).to(dev if nccl else "cpu")
@@ -473,8 +486,13 @@ def ingest_sharded(analyzer, ht, names, signals, root=0, replicate=False, report
         infos = info[None]
     failed = np.nonzero(infos[:, 0])[0]
     if len(failed):
+        msgs = [str(err) if err is not None else ""] * ws
+        if ws > 1 and (infos[:, 0] == 2).any():
+            dist.all_gather_object(msgs, msgs[0], group=group)
         if err is not None:
             raise err
+        if infos[failed[0], 0] == 2:
+            raise IOError(msgs[int(failed[0])])
         raise RuntimeError("ingest_sharded: rank %d failed to ingest its files" % int(failed[0]))
     if (infos[:, 4:] != infos[root, 4:]).any():
         raise ValueError("ingest_sharded: the ranks' tables disagree on hashbits / depth / maxtimebits")
@@ -603,3 +621,77 @@ def match_files_sharded(matcher, analyzer, ht, filenames, root=0, group=None):
             raise IOError(msg)
         raise RuntimeError("match_files_sharded: rank %d failed: %s" % (failed[0], msg))
     return gather_in_list_order(mine, n, root, group)
+
+
+# ---- new / add and precompute from a list of files (the reference's --ncores N) ----------------
+def ingest_files_sharded(analyzer, ht, filenames, root=0, replicate=False, report=None, group=None):
+    """`audfprint.py new / add --ncores N` from files: ingest_sharded with every rank reading its own
+    files.  Every rank passes the whole list and takes file j when j % world is its rank
+    (shard_indices, as multiproc_add deals), then runs Analyzer.ingest_files into a fresh table;
+    the status exchange, the tables' trip to the root, the one merge_batch, the report lines and
+    the optional replication are ingest_sharded's.  An unreadable file (fail_on_error) raises the
+    same IOError on every rank.  Returns ingest_files' (duration, hashes) of this rank's files."""
+    _check_root(root, group)
+    rank, ws = _group_rank(group)
+    idx = shard_indices(len(filenames), rank, ws)
+    mine = [filenames[i] for i in idx]
+    return _ingest_and_merge(lambda local: analyzer.ingest_files(local, mine), ht, int(root), replicate, report,
+                             group, True)
+
+
+def precompute_owners(opnames, world_size: int) -> np.ndarray:
+    """Rank that precomputes each file of a list whose output names are `opnames`: the rank of the
+    FIRST file naming that output (j % world), so that every file writing one output runs on one
+    rank in list order and the list-order effects of skip_existing and overwriting hold."""
+    first = {}
+    owners = np.empty(len(opnames), np.int64)
+    for j, name in enumerate(opnames):
+        owners[j] = first.setdefault(name, j % world_size)
+    return owners
+
+
+def precompute_files_sharded(analyzer, filenames, precompdir, type='hashes', skip_existing=False,
+                             strip_prefix=None, root=0, group=None):
+    """`audfprint.py precompute --ncores N` over the ranks of a process group, one GPU each.  Every
+    rank passes the whole list and runs Analyzer.precompute_files on the files it owns
+    (precompute_owners), in list order.  Failures are handled as in match_files_sharded: the same
+    IOError on every rank for an unreadable file, otherwise the failing rank's own exception and a
+    RuntimeError on the others.  The root returns one message list per file in list order; the other
+    ranks return None."""
+    from .analyzer import precompute_name
+    rank, ws = _group_rank(group)
+    _check_root(root, group)
+    root = int(root)
+    opnames = [precompute_name(f, precompdir, type == 'hashes', strip_prefix) for f in filenames]
+    idx = np.flatnonzero(precompute_owners(opnames, ws) == rank)
+    err, mine = None, []
+    try:
+        mine = analyzer.precompute_files([filenames[i] for i in idx], precompdir, type, skip_existing, strip_prefix)
+    except Exception as e:          # raised on every rank after the status exchange
+        err = e
+    status = (0, "") if err is None else ((1 if isinstance(err, IOError) else 2), str(err))
+    everyone = [status]
+    if ws > 1:
+        import torch.distributed as dist
+        everyone = [None] * ws
+        dist.all_gather_object(everyone, status, group=group)
+    failed = [r for r, st in enumerate(everyone) if st[0]]
+    if failed:
+        if err is not None:
+            raise err
+        kind, msg = everyone[failed[0]]
+        if kind == 1:
+            raise IOError(msg)
+        raise RuntimeError("precompute_files_sharded: rank %d failed: %s" % (failed[0], msg))
+    if ws == 1:
+        return list(mine)
+    import torch.distributed as dist
+    book = [None] * ws if rank == root else None
+    dist.gather_object((idx.tolist(), list(mine)), book, dst=_global_rank(group, root), group=group)
+    if rank != root:
+        return None
+    out = [None] * len(filenames)
+    for ids, msgs in book:
+        for i, m in zip(ids, msgs):
+            out[i] = m
+    return out

@@ -276,8 +276,9 @@ class HashTable(object):
             arrs = [np.asarray(h, dtype=np.int32).reshape(-1, 2) for h in hashes]
             roff = np.zeros(nfiles + 1, np.int64)
             roff[1:] = np.cumsum([len(a) for a in arrs])
-            rows = np.ascontiguousarray(np.concatenate(arrs)) if roff[-1] else np.zeros((0, 2), np.int32)
-            ctx.check(ctx.lib.afp_table_store_batch(ctx.h, rows.ctypes.data if len(rows) else None, 1,
+            # never NULL: NULL rows mean "the workspace's hashes", also when every track is empty
+            rows = np.ascontiguousarray(np.concatenate(arrs)) if roff[-1] else np.zeros((1, 2), np.int32)
+            ctx.check(ctx.lib.afp_table_store_batch(ctx.h, rows.ctypes.data, 1,
                                                     roff.ctypes.data_as(C.POINTER(C.c_int64)), nfiles,
                                                     ids.ctypes.data_as(C.POINTER(C.c_int64)), C.byref(nov)))
         n = int(nov.value)

@@ -196,6 +196,22 @@ int afp_fetch_peaks(afp_ctx* ctx, int32_t shift, int32_t* rows, int rows_on_host
 int afp_landmarks_from_peaks(afp_ctx* ctx, const int32_t* peak_rows, int64_t npeaks, int on_host,
                              int64_t* nlandmarks);
 int afp_fetch_landmarks(afp_ctx* ctx, int32_t* rows, int rows_on_host);
+/* wavfile2hashes of many precomputed-peak (.afpk) files in one pass (audfprint_analyze.py:385-426:
+ * peaks2landmarks, landmarks2hashes, sorted unique (time, hash) rows).
+ *   peak_rows     int32 [..][2] (col, bin), column-major with bins ascending per file, HOST or DEVICE
+ *   peak_offsets  HOST int64 [nfiles+1], non-decreasing: file f is rows [off[f], off[f+1]) of peak_rows
+ *   file_status   HOST int32 [nfiles] or NULL: 0, or the code afp_landmarks_from_peaks returns for that
+ *                 file alone (AFP_ERR_INVALID: a column outside [0, 2^28] or past the file's last
+ *                 column, a bin outside [0, 256), rows out of order; AFP_ERR_UNSUPPORTED: more peaks
+ *                 in one column than maxpksperframe)
+ * A file has last column + 1 columns (:321); an empty file has none and no hashes.  The result is
+ * left in the workspace exactly as afp_fingerprint_batch leaves it: afp_fetch_hashes,
+ * afp_table_store_batch(rows = NULL) and afp_fetch_peaks(shift 0, which returns the input) work on it,
+ * at any configured number of shifts.  When a file fails, the call returns the code of the lowest
+ * failing file and leaves no batch to fetch or store.  The workspace holds about
+ * (maxpksperframe * (1 + 4 maxpairsperpeak) + 5) bytes per column of the batch, plus 8 per hash. */
+int afp_fingerprint_from_peaks(afp_ctx* ctx, const int32_t* peak_rows, int rows_on_host, int32_t nfiles,
+                               const int64_t* peak_offsets, int32_t* file_status, int64_t* total_hashes);
 
 /* Analyzer.spreadpeaksinvector (audfprint_analyze.py:153-160) over spreadpeaks (:162-197):
  *   out[i] = max(base[i] (0 when base is NULL), max over the local maxima p of `vector`
