@@ -149,6 +149,15 @@ def ptr_of(x):
     raise AfpError("unsupported buffer type %r" % type(x))
 
 
+def pack_rows(arrays):
+    """A list of (n_i, 2) int32 arrays -> (rows int32 (sum n_i, 2) contiguous, offsets int64 [len + 1])."""
+    arrs = [np.asarray(a, dtype=np.int32).reshape(-1, 2) for a in arrays]
+    off = np.zeros(len(arrs) + 1, np.int64)
+    off[1:] = np.cumsum([len(a) for a in arrs])
+    rows = np.ascontiguousarray(np.concatenate(arrs)) if arrs else np.zeros((0, 2), np.int32)
+    return rows, off
+
+
 class Context:
     """One afp_ctx (one per process per GPU)."""
 

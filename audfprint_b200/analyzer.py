@@ -10,6 +10,7 @@ spectrogram, a peak or a hash on the CPU.
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import os
 import struct
@@ -407,21 +408,12 @@ class Analyzer(object):
     def fingerprint_batch(self, signals, shifts=None):
         """List of 1-D signals (int16 or float) -> list of int32 (U,2) hash arrays.
         Long lists are cut into device calls of at most `max_frames_per_call` frames."""
-        if len(signals) == 0:
-            return []
-        nsh = max(1, int(self.shifts if shifts is None else shifts))
-        frames = [nsh * (1 + len(x) // self.n_hop) for x in signals]
-        if sum(frames) > self.max_frames_per_call and len(signals) > 1:
-            out, start, acc = [], 0, 0
-            for i, f in enumerate(frames):
-                if acc + f > self.max_frames_per_call and i > start:
-                    out += self.fingerprint_batch(signals[start:i], shifts)
-                    start, acc = i, 0
-                acc += f
-            return out + self.fingerprint_batch(signals[start:], shifts)
-        packed, starts, lens = self._pack(signals)
-        rows, roff = self.fingerprint_packed(packed, starts, shifts, sample_lengths=lens)
-        return [rows[roff[i]:roff[i + 1]] for i in range(len(signals))]
+        out = []
+        for start, end in self._signal_chunks(signals, max(1, int(self.shifts if shifts is None else shifts))):
+            packed, starts, lens = self._pack(signals[start:end])
+            rows, roff = self.fingerprint_packed(packed, starts, shifts, sample_lengths=lens)
+            out += [rows[roff[i]:roff[i + 1]] for i in range(end - start)]
+        return out
 
     def ingest_batch(self, hashtable, names, signals, on_device=True):
         """Fingerprint many signals and add them to the table (batched Analyzer.ingest,
@@ -438,24 +430,24 @@ class Analyzer(object):
                 self._account(len(sig) / self.target_sr)
             return [len(h) for h in hashes]
         nsh = max(1, int(self.shifts))
-        counts, start, acc, pending = [], 0, 0, None
-        frames = [nsh * (1 + len(x) // self.n_hop) for x in signals]
-        for i in range(len(signals) + 1):
-            if i == len(signals) or (acc + frames[i] > self.max_frames_per_call and i > start):
-                if i > start:
-                    packed, starts, lens = self._pack(signals[start:i])
-                    self.fingerprint_packed(packed, starts, nsh, fetch=False, sample_lengths=lens)
-                    # the host-side RNG replay of the previous call's overflow runs while the GPU
-                    # fingerprints this one
-                    counts += hashtable.store_batch_finish(pending)
-                    pending = hashtable.store_batch_begin(names[start:i])
-                start, acc = i, 0
-            if i < len(signals):
-                acc += frames[i]
+        counts, pending = [], None
+        for start, end in self._signal_chunks(signals, nsh):
+            packed, starts, lens = self._pack(signals[start:end])
+            self.fingerprint_packed(packed, starts, nsh, fetch=False, sample_lengths=lens)
+            # the host-side RNG replay of the previous call's overflow runs while the GPU
+            # fingerprints this one
+            counts += hashtable.store_batch_finish(pending)
+            pending = hashtable.store_batch_begin(names[start:end])
         counts += hashtable.store_batch_finish(pending)
         for sig in signals:
             self._account(len(sig) / self.target_sr)
         return counts
+
+    def _signal_chunks(self, signals, nsh):
+        """[start, end) of the device calls that fingerprint `signals` at nsh shifts: at most
+        max_frames_per_call frames each, a longer signal alone."""
+        frames = [nsh * (1 + len(x) // self.n_hop) for x in signals]
+        return plan_chunks(frames, [0] * len(frames), self.max_frames_per_call, float('inf'))
 
     @staticmethod
     def _pack(signals):
@@ -479,12 +471,17 @@ class Analyzer(object):
         """Waveform -> list of (time_frame, freq_bin) (audfprint_analyze.py:255-308)."""
         if len(d) == 0:
             return []
+        return self._fetch_peaks(self._fingerprint_one(d, 1), 0, 1)[0]
+
+    def _fingerprint_one(self, d, shifts):
+        """Fingerprint one signal in one device call at `shifts`; the results stay in the workspace.
+        Returns the context."""
         a, dtype = _as_pcm(d)
-        ctx = self._configure(1)
+        ctx = self._configure(shifts)
         off = np.array([0, len(a)], np.int64)
         ctx.check(ctx.lib.afp_fingerprint_batch(ctx.h, a.ctypes.data, dtype, 1, 1,
                                                 off.ctypes.data_as(C.POINTER(C.c_int64)), None, None))
-        return self._fetch_peaks(ctx, 0, 1)[0]
+        return ctx
 
     def _fetch_peaks(self, ctx, shift, nfiles):
         poff = np.empty(nfiles + 1, np.int64)
@@ -538,6 +535,16 @@ class Analyzer(object):
             raise IOError(message)
         print(message, "skipping")
 
+    @contextlib.contextmanager
+    def _counters_restored_on_error(self):
+        """Leave soundfiledur / soundfiletotaldur / soundfilecount as they were if the body raises."""
+        saved = (self.soundfiledur, self.soundfiletotaldur, self.soundfilecount)
+        try:
+            yield
+        except BaseException:
+            self.soundfiledur, self.soundfiletotaldur, self.soundfilecount = saved
+            raise
+
     def _account(self, dur):
         self.soundfiledur = dur
         self.soundfiletotaldur += dur
@@ -559,11 +566,7 @@ class Analyzer(object):
                 peaks = [[] for _ in range(shifts)]
             else:
                 # NB the reference takes the offsets from self.shifts (:375)
-                a, dtype = _as_pcm(d)
-                ctx = self._configure(self.shifts)
-                off = np.array([0, len(a)], np.int64)
-                ctx.check(ctx.lib.afp_fingerprint_batch(ctx.h, a.ctypes.data, dtype, 1, 1,
-                                                        off.ctypes.data_as(C.POINTER(C.c_int64)), None, None))
+                ctx = self._fingerprint_one(d, self.shifts)
                 peaks = [self._fetch_peaks(ctx, s, 1)[0] for s in range(min(shifts, self.shifts))]
         self._account(dur)
         return peaks
@@ -619,27 +622,32 @@ class Analyzer(object):
     def _hashes_of_files(self, filenames, rows_on_device=False):
         """wavfiles2hashes; with rows_on_device the fingerprinted files' hashes stay on the device
         (afp_fetch_hashes into a torch tensor) as DeviceHashes."""
-        saved = (self.soundfiledur, self.soundfiletotaldur, self.soundfilecount)
+        def collect(kind, idx, results):
+            # the reference returns [] when a WAV has no peaks (:401-402)
+            self._collect_hashes(idx, results, rows_on_device, kind == 'pcm' and self.shifts < 2)
+        return self._analyse_files(filenames, False, max(1, int(self.shifts)), collect, list)
+
+    def _analyse_files(self, filenames, peaks_mode, nsh, collect, empty):
+        """The list forms' driver: read `filenames` in rounds (_file_rounds), run each device round at
+        nsh shifts and hand it to `collect(kind, indices, results)`, which puts the round's results at
+        their indices.  A file whose result is known on the host takes it as it is, or `empty()` when
+        it has no samples.  The counters end as the per-file loop leaves them, or as they were if
+        anything raises; the files' durations go to `last_batch_durations`."""
         n = len(filenames)
         results, durs = [None] * n, [0.0] * n
-        try:
-            for kind, items in self._file_rounds(filenames, False, max(1, int(self.shifts)), False):
-                idx = [it[0] for it in items]
+        with self._counters_restored_on_error():
+            for kind, items in self._file_rounds(filenames, peaks_mode, nsh, False):
                 if kind == 'host':
                     for i, value, dur in items:
-                        results[i], durs[i] = ([] if value is None else value), dur
-                elif kind == 'pcm':
-                    self._fingerprint_pcm(items, self.shifts, durs)
-                    # the reference returns [] when a WAV has no peaks (:401-402)
-                    self._collect_hashes(idx, results, rows_on_device, self.shifts < 2)
+                        results[i], durs[i] = (empty() if value is None else value), dur
+                    continue
+                if kind == 'pcm':
+                    self._fingerprint_pcm(items, nsh, durs)
                 else:
                     self._fingerprint_peaks([it[1] for it in items])
                     for i, _, dur in items:
                         durs[i] = dur
-                    self._collect_hashes(idx, results, rows_on_device, False)
-        except BaseException:
-            self.soundfiledur, self.soundfiletotaldur, self.soundfilecount = saved
-            raise
+                collect(kind, [it[0] for it in items], results)
         for dur in durs:
             self._account(dur)
         self.last_batch_durations = durs
@@ -793,33 +801,14 @@ class Analyzer(object):
         reads them.  Failures behave as in wavfiles2hashes."""
         multi = not (shifts is None or shifts < 2)
         nsh = max(1, int(self.shifts)) if multi else 1
-        saved = (self.soundfiledur, self.soundfiletotaldur, self.soundfilecount)
-        n = len(filenames)
-        results, durs = [None] * n, [0.0] * n
-        try:
-            for kind, items in self._file_rounds(filenames, True, nsh, False):
-                if kind == 'host':
-                    for i, value, dur in items:
-                        if value is None:
-                            value = [[] for _ in range(shifts)] if multi else []
-                        results[i], durs[i] = value, dur
-                    continue
-                self._fingerprint_pcm(items, nsh, durs)
-                ctx = _lib.context(self.device)
-                if multi:
-                    per_shift = [self._fetch_peaks(ctx, s, len(items)) for s in range(min(shifts, nsh))]
-                    for k, it in enumerate(items):
-                        results[it[0]] = [p[k] for p in per_shift]
-                else:
-                    for it, pk in zip(items, self._fetch_peaks(ctx, 0, len(items))):
-                        results[it[0]] = pk
-        except BaseException:
-            self.soundfiledur, self.soundfiletotaldur, self.soundfilecount = saved
-            raise
-        for dur in durs:
-            self._account(dur)
-        self.last_batch_durations = durs
-        return results
+
+        def collect(kind, idx, results):
+            ctx = _lib.context(self.device)
+            per_shift = [self._fetch_peaks(ctx, s, len(idx)) for s in range(min(shifts, nsh) if multi else 1)]
+            for k, i in enumerate(idx):
+                results[i] = [p[k] for p in per_shift] if multi else per_shift[0][k]
+        return self._analyse_files(filenames, True, nsh, collect,
+                                   (lambda: [[] for _ in range(shifts)]) if multi else list)
 
     def ingest(self, hashtable, filename):
         """Read a file and add it to the table (audfprint_analyze.py:430-457)."""

@@ -29,15 +29,67 @@ from __future__ import annotations
 import numpy as np
 
 
-def world():
-    """(rank, world_size) of the default process group, (0, 1) when not initialised."""
+def world(group=None):
+    """(rank, world_size) in `group` (None: the default process group), (0, 1) when torch.distributed
+    is not initialised."""
     try:
         import torch.distributed as dist
         if dist.is_available() and dist.is_initialized():
-            return dist.get_rank(), dist.get_world_size()
+            return dist.get_rank(group), dist.get_world_size(group)
     except ImportError:
         pass
     return 0, 1
+
+
+def _collective_device(group, device=None):
+    """Where the buffers of a collective over `group` live: CUDA device `device` (None: torch's current
+    one) under NCCL, host memory under gloo, which the device data reaches by a round trip."""
+    import torch
+    import torch.distributed as dist
+    if dist.get_backend(group) != "nccl":
+        return torch.device("cpu")
+    return torch.device("cuda", torch.cuda.current_device() if device is None else device)
+
+
+def _global_rank(group, r):
+    import torch.distributed as dist
+    return r if group is None else dist.get_global_rank(group, r)
+
+
+def _check_root(root, group):
+    rank, ws = world(group)
+    if not 0 <= int(root) < ws:
+        raise ValueError("root %d outside the group's %d ranks" % (int(root), ws))
+
+
+# status of one rank's part of an entry point, exchanged before any result moves
+_OK, _IO_ERROR, _FAILED = 0, 1, 2
+
+
+def _status_code(err, io_errors_everywhere=True):
+    """This rank's status: _OK without an exception, _IO_ERROR for an IOError that every rank is to
+    raise (with io_errors_everywhere), _FAILED otherwise."""
+    if err is None:
+        return _OK
+    return _IO_ERROR if io_errors_everywhere and isinstance(err, IOError) else _FAILED
+
+
+def _raise_if_failed(err, codes, what, group=None):
+    """Raise the same thing on every rank of `group` when one failed; `err` is this rank's exception
+    (or None) and `codes` the _status_code of every rank, in rank order, gathered by the caller.  The
+    messages are gathered only when a rank failed, by every rank.  The failing rank raises its own
+    exception; the others raise the first failing rank's IOError when its code is _IO_ERROR, else a
+    RuntimeError naming `what`, that rank and its message."""
+    failed = [r for r, c in enumerate(codes) if int(c) != _OK]
+    if not failed:
+        return
+    msgs = gather_objects("" if err is None else str(err), group)
+    if err is not None:
+        raise err
+    r = failed[0]
+    if int(codes[r]) == _IO_ERROR:
+        raise IOError(msgs[r])
+    raise RuntimeError("%s: rank %d failed: %s" % (what, r, msgs[r]))
 
 
 def shard_indices(n: int, rank: int, world_size: int) -> np.ndarray:
@@ -54,7 +106,7 @@ def id_range(nids: int, rank: int, world_size: int):
 
 def gather_objects(obj, group=None):
     """all_gather of small host objects (result lists); identity without a process group."""
-    rank, ws = world()
+    rank, ws = world(group)
     if ws == 1:
         return [obj]
     import torch.distributed as dist
@@ -156,14 +208,15 @@ def unpack_shard_records(buf: np.ndarray, search_depth: int = None, row_cap: int
     return recs
 
 
-def _allgather_bytes(mine: np.ndarray, group=None) -> np.ndarray:
-    """all_gather of one structured array per rank -> (world, nq) structured array."""
-    rank, ws = world()
+def _allgather_bytes(mine: np.ndarray, group=None, device=None) -> np.ndarray:
+    """all_gather of one 1-D array per rank (a structured one included), with buffers where
+    _collective_device puts them -> (world, len) array."""
+    rank, ws = world(group)
     if ws == 1:
         return mine[None]
     import torch
     import torch.distributed as dist
-    dev = torch.device("cuda", torch.cuda.current_device()) if dist.get_backend(group) == "nccl" else torch.device("cpu")
+    dev = _collective_device(group, device)
     t = torch.from_numpy(np.ascontiguousarray(mine).view(np.uint8).reshape(len(mine), -1)).to(dev)
     out = torch.empty((ws * t.shape[0], t.shape[1]), dtype=torch.uint8, device=dev)
     dist.all_gather_into_tensor(out, t, group=group)
@@ -185,13 +238,10 @@ def match_sharded(matcher, ht, queries, row_cap: int = 16, group=None):
     below is the throughput path).  With exact_count or find_time_range set the queries go through
     match_sharded_batch, which finishes them on the device."""
     if matcher.exact_count or matcher.find_time_range:
-        arrs = [np.asarray(q, dtype=np.int32).reshape(-1, 2) for q in queries]
-        qoff = np.zeros(len(arrs) + 1, np.int64)
-        if arrs:
-            qoff[1:] = np.cumsum([len(a) for a in arrs])
-        packed = np.ascontiguousarray(np.concatenate(arrs)) if arrs else np.zeros((0, 2), np.int32)
+        from ._lib import pack_rows
+        packed, qoff = pack_rows(queries)
         rows, roff = match_sharded_batch(matcher, ht, (packed, qoff), row_cap, group)
-        return [r[(-r[:, 1]).argsort(), ] for r in (rows[roff[i]:roff[i + 1]] for i in range(len(arrs)))]
+        return [r[(-r[:, 1]).argsort(), ] for r in (rows[roff[i]:roff[i + 1]] for i in range(len(qoff) - 1))]
     mine = matcher.match_batch_shard(ht, queries)
     shards = allgather_shard_records(mine, matcher.search_depth, row_cap, group)
     out = []
@@ -344,7 +394,7 @@ def match_sharded_batch(matcher, ht, packed_queries, row_cap: int = 16, group=No
     if rb < 0:
         raise ValueError("row_cap must be even and >= 2")
     dev = torch.device("cuda", ctx.device)
-    rank, ws = world()
+    rank, ws = world(group)
     if not options:
         matcher._run(ctx, p, qrows, nq, qoff)
     else:
@@ -353,12 +403,10 @@ def match_sharded_batch(matcher, ht, packed_queries, row_cap: int = 16, group=No
                      shard_qmax=qmax.data_ptr())
         if ws > 1:
             import torch.distributed as dist
-            if dist.get_backend(group) == "nccl":
-                dist.all_reduce(qmax, op=dist.ReduceOp.MAX, group=group)
-            else:                                # gloo: through host memory
-                h = qmax.cpu()
-                dist.all_reduce(h, op=dist.ReduceOp.MAX, group=group)
-                qmax.copy_(h)
+            buf = qmax.to(_collective_device(group, ctx.device))         # in place under NCCL
+            dist.all_reduce(buf, op=dist.ReduceOp.MAX, group=group)
+            if buf is not qmax:
+                qmax.copy_(buf)
             torch.cuda.current_stream(dev).synchronize()
         ctx.check(ctx.lib.afp_match_options_shard_finish(ctx.h, C.c_void_p(qmax.data_ptr()), None))
     mine = torch.empty((max(nq, 1), rb), dtype=torch.uint8, device=dev)
@@ -372,39 +420,19 @@ def match_sharded_batch(matcher, ht, packed_queries, row_cap: int = 16, group=No
         gathered = mine
     else:
         import torch.distributed as dist
-        if dist.get_backend(group) == "nccl":
-            gathered = torch.empty((ws * mine.shape[0], rb), dtype=torch.uint8, device=dev)
-            dist.all_gather_into_tensor(gathered, mine, group=group)
-        else:                                    # gloo: same bytes through host memory
-            h = mine.cpu()
-            g = torch.empty((ws * h.shape[0], rb), dtype=torch.uint8)
-            dist.all_gather_into_tensor(g, h, group=group)
-            gathered = g.to(dev)
+        cdev = _collective_device(group, ctx.device)
+        g = torch.empty((ws * mine.shape[0], rb), dtype=torch.uint8, device=cdev)
+        dist.all_gather_into_tensor(g, mine.to(cdev), group=group)
+        gathered = g.to(dev)
         torch.cuda.current_stream(dev).synchronize()
     total = C.c_int64(0)
     ctx.check(ctx.lib.afp_shard_merge(ctx.h, gathered.data_ptr(), ws, nq, sd, int(row_cap), C.byref(total)))
     if not fetch:
         return None, None
-    rows = np.empty((int(total.value), 7), np.int32)
-    roff = np.zeros(nq + 1, np.int64)
-    ctx.check(ctx.lib.afp_fetch_match_rows(ctx.h, rows.ctypes.data if len(rows) else None, 1,
-                                           roff.ctypes.data_as(C.POINTER(C.c_int64))))
-    return rows, roff
+    return matcher._fetch_rows(ctx, int(total.value), nq)
 
 
 # ---- one table from a multi-GPU ingest (the reference's multiproc_add) --------------------
-def _group_rank(group):
-    import torch.distributed as dist
-    if not (dist.is_available() and dist.is_initialized()):
-        return 0, 1
-    return dist.get_rank(group), dist.get_world_size(group)
-
-
-def _global_rank(group, r):
-    import torch.distributed as dist
-    return r if group is None else dist.get_global_rank(group, r)
-
-
 def ingest_sharded(analyzer, ht, names, signals, root=0, replicate=False, report=None, group=None):
     """`audfprint.py new / add --ncores N` (multiproc_add, audfprint.py:199-235) over the ranks of
     a process group, one GPU each.  `names` / `signals` are this rank's own files, dealt as the
@@ -438,12 +466,6 @@ def ingest_sharded(analyzer, ht, names, signals, root=0, replicate=False, report
                              replicate, report, group, False)
 
 
-def _check_root(root, group):
-    rank, ws = _group_rank(group)
-    if not 0 <= int(root) < ws:
-        raise ValueError("root %d outside the group's %d ranks" % (int(root), ws))
-
-
 def _ingest_and_merge(ingest, ht, root, replicate, report, group, io_errors_everywhere):
     """Steps 1-6 of ingest_sharded, with step 1 as `ingest(local_table)` -> this rank's result.  With
     io_errors_everywhere an IOError raised by one rank's ingest is raised, with its message, on every
@@ -451,13 +473,12 @@ def _ingest_and_merge(ingest, ht, root, replicate, report, group, io_errors_ever
     import torch
     from . import _lib
     from .hash_table import DeviceTable, HashTable
-    rank, ws = _group_rank(group)
+    rank, ws = world(group)
     ctx = _lib.context(ht.device)
     dev = torch.device("cuda", ctx.device)
-    nccl = False
     if ws > 1:
         import torch.distributed as dist
-        nccl = dist.get_backend(group) == "nccl"
+        cdev = _collective_device(group, ctx.device)
     hb, depth, mtb = int(ht.hashbits), int(ht.depth), int(ht.maxtimebits)
 
     # 1. this rank's files into a fresh table
@@ -468,32 +489,15 @@ def _ingest_and_merge(ingest, ht, root, replicate, report, group, io_errors_ever
         mine = local.export_device()
     except Exception as e:          # raised on every rank after the all-gather
         err = e
-    if ctx.table_owner is not None and ctx.table_owner() is local:
-        ctx.table_owner = None      # its rows live on in `mine`: no pull to the host when `ht` takes the device
+    local._disown_device()          # its rows live on in `mine`: no pull to the host when `ht` takes the device
     del local
     nhashes = int(mine.counts.sum(dtype=torch.int64)) if mine is not None else 0
 
     # 2. status, name and hash counts, the root's base and geometry, from every rank
-    code = 0 if err is None else 2 if (io_errors_everywhere and isinstance(err, IOError)) else 1
-    info = np.array([code, len(mine.names) if mine is not None else 0, nhashes,
+    info = np.array([_status_code(err, io_errors_everywhere), len(mine.names) if mine is not None else 0, nhashes,
                      len(ht.names), hb, depth, mtb], np.int64)
-    if ws > 1:
-        t = torch.from_numpy(info).to(dev if nccl else "cpu")
-        g = torch.empty(ws * len(info), dtype=torch.int64, device=t.device)
-        dist.all_gather_into_tensor(g, t, group=group)
-        infos = g.cpu().numpy().reshape(ws, len(info))
-    else:
-        infos = info[None]
-    failed = np.nonzero(infos[:, 0])[0]
-    if len(failed):
-        msgs = [str(err) if err is not None else ""] * ws
-        if ws > 1 and (infos[:, 0] == 2).any():
-            dist.all_gather_object(msgs, msgs[0], group=group)
-        if err is not None:
-            raise err
-        if infos[failed[0], 0] == 2:
-            raise IOError(msgs[int(failed[0])])
-        raise RuntimeError("ingest_sharded: rank %d failed to ingest its files" % int(failed[0]))
+    infos = _allgather_bytes(info, group, ctx.device)
+    _raise_if_failed(err, infos[:, 0], "ingest_sharded", group)
     if (infos[:, 4:] != infos[root, 4:]).any():
         raise ValueError("ingest_sharded: the ranks' tables disagree on hashbits / depth / maxtimebits")
     nn = int(infos[root, 3])
@@ -516,13 +520,11 @@ def _ingest_and_merge(ingest, ht, root, replicate, report, group, io_errors_ever
             if r == rank:
                 tables.append(mine)
                 continue
-            tab = torch.empty((nb, depth), dtype=torch.int32, device=dev if nccl else "cpu")
-            cnt = torch.empty(nb, dtype=torch.int32, device=tab.device)
+            tab = torch.empty((nb, depth), dtype=torch.int32, device=cdev)
+            cnt = torch.empty(nb, dtype=torch.int32, device=cdev)
             dist.recv(tab, src=_global_rank(group, r), group=group)
             dist.recv(cnt, src=_global_rank(group, r), group=group)
-            if not nccl:
-                tab, cnt = tab.to(dev), cnt.to(dev)
-            tables.append(DeviceTable(tab, cnt, book[r][0], book[r][1], hb, depth, mtb))
+            tables.append(DeviceTable(tab.to(dev), cnt.to(dev), book[r][0], book[r][1], hb, depth, mtb))
         if report is not None:
             for r in range(ws):
                 report(["hash_table %d has %d files %d hashes" % (r, int(infos[r, 1]), int(infos[r, 2]))])
@@ -530,8 +532,8 @@ def _ingest_and_merge(ingest, ht, root, replicate, report, group, io_errors_ever
         del tables
     else:
         dst = _global_rank(group, root)
-        dist.send(mine.table if nccl else mine.table.cpu(), dst=dst, group=group)
-        dist.send(mine.counts if nccl else mine.counts.cpu(), dst=dst, group=group)
+        dist.send(mine.table.to(cdev), dst=dst, group=group)
+        dist.send(mine.counts.to(cdev), dst=dst, group=group)
     del mine
 
     # 6. the merged table to every rank
@@ -540,11 +542,11 @@ def _ingest_and_merge(ingest, ht, root, replicate, report, group, io_errors_ever
         if rank == root:
             snap = ht.export_device()
             obj = [(snap.names, snap.hashesperid)]
-            tab, cnt = (snap.table, snap.counts) if nccl else (snap.table.cpu(), snap.counts.cpu())
+            tab, cnt = snap.table.to(cdev), snap.counts.to(cdev)
         else:
             obj = [None]
-            tab = torch.empty((nb, depth), dtype=torch.int32, device=dev if nccl else "cpu")
-            cnt = torch.empty(nb, dtype=torch.int32, device=tab.device)
+            tab = torch.empty((nb, depth), dtype=torch.int32, device=cdev)
+            cnt = torch.empty(nb, dtype=torch.int32, device=cdev)
         dist.broadcast_object_list(obj, src=src, group=group)
         dist.broadcast(tab, src=src, group=group)
         dist.broadcast(cnt, src=src, group=group)
@@ -557,13 +559,26 @@ def _ingest_and_merge(ingest, ht, root, replicate, report, group, io_errors_ever
 def gather_in_list_order(mine, n, root=0, group=None):
     """Rank r's results of items r, r + world, r + 2 world, ... (shard_indices) -> the whole list of
     n results in list order on the root, None on the other ranks: one gather_object."""
-    rank, ws = _group_rank(group)
+    rank, ws = world(group)
+    return _gather_by_index(shard_indices(n, rank, ws), mine, n, root, group)
+
+
+def _gather_by_index(idx, mine, n, root, group):
+    """This rank's results `mine` of the list positions `idx` -> the whole list of n results on the
+    root, None on the other ranks: one gather_object."""
+    rank, ws = world(group)
     if ws == 1:
         return list(mine)
     import torch.distributed as dist
     book = [None] * ws if rank == root else None
-    dist.gather_object(list(mine), book, dst=_global_rank(group, root), group=group)
-    return interleave_shards(book, n) if rank == root else None
+    dist.gather_object((np.asarray(idx).tolist(), list(mine)), book, dst=_global_rank(group, root), group=group)
+    if rank != root:
+        return None
+    out = [None] * n
+    for ids, results in book:
+        for i, m in zip(ids, results):
+            out[i] = m
+    return out
 
 
 def match_files_sharded(matcher, analyzer, ht, filenames, root=0, group=None):
@@ -580,22 +595,12 @@ def match_files_sharded(matcher, analyzer, ht, filenames, root=0, group=None):
        own exception and the others a RuntimeError naming it.  No rank is left in a collective.
     4. The root returns the message lists in list order, as joblib returns them; the other ranks
        return None."""
-    import torch
-    rank, ws = _group_rank(group)
-    root = int(root)
-    if not 0 <= root < ws:
-        raise ValueError("root %d outside the group's %d ranks" % (root, ws))
+    from . import _lib
+    _check_root(root, group)
+    rank, ws = world(group)
     n = len(filenames)
     info = np.array([int(ht.hashbits), int(ht.depth), int(ht.maxtimebits), len(ht.names)], np.int64)
-    infos = info[None]
-    if ws > 1:
-        import torch.distributed as dist
-        from . import _lib
-        dev = torch.device("cuda", _lib.context(ht.device).device) if dist.get_backend(group) == "nccl" else "cpu"
-        t = torch.from_numpy(info).to(dev)
-        g = torch.empty(ws * len(info), dtype=torch.int64, device=dev)
-        dist.all_gather_into_tensor(g, t, group=group)
-        infos = g.cpu().numpy().reshape(ws, len(info))
+    infos = _allgather_bytes(info, group, _lib.context(ht.device).device if ws > 1 else None)
     if (infos != infos[0]).any():
         raise ValueError("match_files_sharded: the ranks' tables disagree on hashbits / depth / maxtimebits / "
                          "number of names: %s" % infos.tolist())
@@ -605,22 +610,8 @@ def match_files_sharded(matcher, analyzer, ht, filenames, root=0, group=None):
         mine = matcher._files_msgs(analyzer, ht, [filenames[i] for i in idx], [int(i) for i in idx])
     except Exception as e:          # raised on every rank after the status exchange
         err = e
-    status = (0, "") if err is None else ((1 if isinstance(err, IOError) else 2), str(err))
-    if ws > 1:
-        import torch.distributed as dist
-        everyone = [None] * ws
-        dist.all_gather_object(everyone, status, group=group)
-    else:
-        everyone = [status]
-    failed = [r for r, st in enumerate(everyone) if st[0]]
-    if failed:
-        if err is not None:
-            raise err
-        kind, msg = everyone[failed[0]]
-        if kind == 1:
-            raise IOError(msg)
-        raise RuntimeError("match_files_sharded: rank %d failed: %s" % (failed[0], msg))
-    return gather_in_list_order(mine, n, root, group)
+    _raise_if_failed(err, gather_objects(_status_code(err), group), "match_files_sharded", group)
+    return _gather_by_index(idx, mine, n, int(root), group)
 
 
 # ---- new / add and precompute from a list of files (the reference's --ncores N) ----------------
@@ -632,7 +623,7 @@ def ingest_files_sharded(analyzer, ht, filenames, root=0, replicate=False, repor
     the optional replication are ingest_sharded's.  An unreadable file (fail_on_error) raises the
     same IOError on every rank.  Returns ingest_files' (duration, hashes) of this rank's files."""
     _check_root(root, group)
-    rank, ws = _group_rank(group)
+    rank, ws = world(group)
     idx = shard_indices(len(filenames), rank, ws)
     mine = [filenames[i] for i in idx]
     return _ingest_and_merge(lambda local: analyzer.ingest_files(local, mine), ht, int(root), replicate, report,
@@ -659,9 +650,8 @@ def precompute_files_sharded(analyzer, filenames, precompdir, type='hashes', ski
     RuntimeError on the others.  The root returns one message list per file in list order; the other
     ranks return None."""
     from .analyzer import precompute_name
-    rank, ws = _group_rank(group)
     _check_root(root, group)
-    root = int(root)
+    rank, ws = world(group)
     opnames = [precompute_name(f, precompdir, type == 'hashes', strip_prefix) for f in filenames]
     idx = np.flatnonzero(precompute_owners(opnames, ws) == rank)
     err, mine = None, []
@@ -669,29 +659,5 @@ def precompute_files_sharded(analyzer, filenames, precompdir, type='hashes', ski
         mine = analyzer.precompute_files([filenames[i] for i in idx], precompdir, type, skip_existing, strip_prefix)
     except Exception as e:          # raised on every rank after the status exchange
         err = e
-    status = (0, "") if err is None else ((1 if isinstance(err, IOError) else 2), str(err))
-    everyone = [status]
-    if ws > 1:
-        import torch.distributed as dist
-        everyone = [None] * ws
-        dist.all_gather_object(everyone, status, group=group)
-    failed = [r for r, st in enumerate(everyone) if st[0]]
-    if failed:
-        if err is not None:
-            raise err
-        kind, msg = everyone[failed[0]]
-        if kind == 1:
-            raise IOError(msg)
-        raise RuntimeError("precompute_files_sharded: rank %d failed: %s" % (failed[0], msg))
-    if ws == 1:
-        return list(mine)
-    import torch.distributed as dist
-    book = [None] * ws if rank == root else None
-    dist.gather_object((idx.tolist(), list(mine)), book, dst=_global_rank(group, root), group=group)
-    if rank != root:
-        return None
-    out = [None] * len(filenames)
-    for ids, msgs in book:
-        for i, m in zip(ids, msgs):
-            out[i] = m
-    return out
+    _raise_if_failed(err, gather_objects(_status_code(err), group), "precompute_files_sharded", group)
+    return _gather_by_index(idx, mine, len(filenames), int(root), group)

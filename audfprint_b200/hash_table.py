@@ -273,11 +273,10 @@ class HashTable(object):
             ctx.check(ctx.lib.afp_table_store_batch(ctx.h, None, 0, None, nfiles, ids.ctypes.data_as(C.POINTER(C.c_int64)),
                                                     C.byref(nov)))
         else:
-            arrs = [np.asarray(h, dtype=np.int32).reshape(-1, 2) for h in hashes]
-            roff = np.zeros(nfiles + 1, np.int64)
-            roff[1:] = np.cumsum([len(a) for a in arrs])
+            rows, roff = _lib.pack_rows(hashes)
             # never NULL: NULL rows mean "the workspace's hashes", also when every track is empty
-            rows = np.ascontiguousarray(np.concatenate(arrs)) if roff[-1] else np.zeros((1, 2), np.int32)
+            if not roff[-1]:
+                rows = np.zeros((1, 2), np.int32)
             ctx.check(ctx.lib.afp_table_store_batch(ctx.h, rows.ctypes.data, 1,
                                                     roff.ctypes.data_as(C.POINTER(C.c_int64)), nfiles,
                                                     ids.ctypes.data_as(C.POINTER(C.c_int64)), C.byref(nov)))
@@ -286,10 +285,7 @@ class HashTable(object):
         if n:
             ctx.check(ctx.lib.afp_table_fetch_overflow_counts(ctx.h, cnt.ctypes.data))
         # from here on the device table is ahead of the host arrays, whatever happens next
-        self._touch()
-        self._dev_newer = True
-        ctx.table_key = self._dev_key = self._stamp()
-        ctx.table_owner = weakref.ref(self)
+        self._device_leads(ctx)
         self._store_pending = True
         return (ctx, ids, roff, cnt)
 
@@ -316,8 +312,7 @@ class HashTable(object):
             ctx.check(ctx.lib.afp_table_set_hashesperid(ctx.h, hpi.ctypes.data if len(hpi) else None, len(hpi)))
         finally:
             self._store_pending = False       # a failed finish must not lock the table against every later edit
-        self._touch()
-        ctx.table_key = self._dev_key = self._stamp()      # the device copy IS this version
+        self._device_is_current(ctx)
         return [int(x) for x in per_track]
 
     def _plan_ids(self, names):
@@ -470,10 +465,7 @@ class HashTable(object):
         for i in ids:
             self.names[i] = None
             hpi[i] = 0
-        self._touch()
-        self._dev_newer = True
-        ctx.table_key = self._dev_key = self._stamp()      # the device copy IS this version
-        ctx.table_owner = weakref.ref(self)
+        self._device_leads(ctx)
         for name, n in zip(names, removed):
             print("Removed", name, "(", int(n), "hashes).")
 
@@ -583,10 +575,7 @@ class HashTable(object):
         for t, _, _, _ in plan:
             self.names += t.names
         self.__dict__["_hashesperid"] = hpi
-        self._touch()
-        self._dev_newer = True
-        ctx.table_key = self._dev_key = self._stamp()      # the device copy IS this version
-        ctx.table_owner = weakref.ref(self)
+        self._device_leads(ctx)
         return total
 
     def _check_snapshot(self, t, nb):
@@ -627,10 +616,7 @@ class HashTable(object):
         import torch
         self._check_device_edit("install a device table")
         ctx = _lib.context(self.device)
-        owner = ctx.table_owner() if getattr(ctx, "table_owner", None) else None
-        if owner is not None and owner is not self and getattr(owner, "_dev_newer", False):
-            owner._pull_device()
-        ctx.table_owner = None
+        self._evict_device_owner(ctx)
         ctx.table_key = None
         self._shard = None
         dev = torch.device("cuda", ctx.device)
@@ -644,10 +630,36 @@ class HashTable(object):
         self.__dict__["_table"] = self.__dict__["_counts"] = None     # pulled from the device when read
         self.names = list(snap.names)
         self.__dict__["_hashesperid"] = hpi.copy()
+        self._device_leads(ctx)
+
+    def _device_is_current(self, ctx):
+        """After an edit made on the device copy: the host state is a new version (and dirty), and
+        the device copy IS that version."""
         self._touch()
+        ctx.table_key = self._dev_key = self._stamp()
+
+    def _device_leads(self, ctx):
+        """_device_is_current, where the device copy also holds this table's only copy of the edit:
+        the host arrays refresh from it when read, and this table owns the device copy, so another
+        table's upload pulls it first (_evict_device_owner)."""
+        self._device_is_current(ctx)
         self._dev_newer = True
-        ctx.table_key = self._dev_key = self._stamp()      # the device copy IS this version
         ctx.table_owner = weakref.ref(self)
+
+    def _evict_device_owner(self, ctx):
+        """Before this table overwrites the device copy: if that copy holds another table's only copy
+        of its device-side edits, pull them into that table's host arrays first."""
+        owner = ctx.table_owner() if ctx.table_owner is not None else None
+        if owner is not None and owner is not self and owner._dev_newer:
+            owner._pull_device()
+        ctx.table_owner = None
+
+    def _disown_device(self):
+        """Give up the device copy without pulling it to the host, for a caller that keeps its rows
+        elsewhere (an export_device snapshot) and drops this table: the next upload overwrites them."""
+        ctx = _lib.context(self.device)
+        if ctx.table_owner is not None and ctx.table_owner() is self:
+            ctx.table_owner = None
 
     def _check_device_edit(self, what):
         # a shard stamp left behind after another table took the device is no shard: _sync_device
@@ -800,11 +812,7 @@ class HashTable(object):
             return ctx              # device copy is this table's shard
         if ctx.table_key != self._stamp():
             self._shard = None
-            # the device may hold ANOTHER table's only copy of its device-side inserts: save it first
-            owner = ctx.table_owner() if getattr(ctx, "table_owner", None) else None
-            if owner is not None and owner is not self and getattr(owner, "_dev_newer", False):
-                owner._pull_device()
-            ctx.table_owner = None
+            self._evict_device_owner(ctx)
             table = np.ascontiguousarray(self.table, dtype=np.uint32)     # (pulls the device copy first if it is newer)
             counts = np.ascontiguousarray(self.counts, dtype=np.int32)
             hpi = np.ascontiguousarray(self.hashesperid, dtype=np.uint32)

@@ -141,21 +141,14 @@ class Matcher(object):
                 packed = np.ascontiguousarray(packed, dtype=np.int32).reshape(-1, 2)
             qoff = np.ascontiguousarray(qoff, dtype=np.int64)
         else:
-            arrs = [np.asarray(q, dtype=np.int32).reshape(-1, 2) for q in queries]
-            qoff = np.zeros(len(arrs) + 1, np.int64)
-            if arrs:
-                qoff[1:] = np.cumsum([len(a) for a in arrs])
-            packed = np.ascontiguousarray(np.concatenate(arrs)) if arrs else np.zeros((0, 2), np.int32)
+            packed, qoff = _lib.pack_rows(queries)
         nq = len(qoff) - 1
         p = self._params()
         if (self.exact_count or self.find_time_range) and hasattr(ht, "_sync_device"):
             # one device call: ranking in publish mode, then the options' finish on the device
             ctx = ht._sync_device()
-            rows = np.empty((self._run(ctx, p, packed, nq, qoff, (self.exact_count, self.find_time_range,
-                                                                   self.time_quantile)), 7), np.int32)
-            roff = np.zeros(nq + 1, np.int64)
-            ctx.check(ctx.lib.afp_fetch_match_rows(ctx.h, rows.ctypes.data if len(rows) else None, 1,
-                                                   roff.ctypes.data_as(C.POINTER(C.c_int64))))
+            total = self._run(ctx, p, packed, nq, qoff, (self.exact_count, self.find_time_range, self.time_quantile))
+            rows, roff = self._fetch_rows(ctx, total, nq)
             if sort and len(rows):
                 rows = self._sort_by_count(rows, roff)
             return [rows[roff[i]:roff[i + 1]] for i in range(nq)]
@@ -183,13 +176,19 @@ class Matcher(object):
                 out.append(self._match_with_options(ht, packed[qoff[i]:qoff[i + 1]], device_results=pre))
             return [r[(-r[:, 1]).argsort(), ] for r in out] if sort else out
         ctx = ht._sync_device()
-        rows = np.empty((self._run(ctx, p, packed, nq, qoff), 7), np.int32)
-        roff = np.zeros(nq + 1, np.int64)
-        ctx.check(ctx.lib.afp_fetch_match_rows(ctx.h, rows.ctypes.data if len(rows) else None, 1,
-                                               roff.ctypes.data_as(C.POINTER(C.c_int64))))
+        rows, roff = self._fetch_rows(ctx, self._run(ctx, p, packed, nq, qoff), nq)
         if sort and len(rows):
             rows = self._sort_by_count(rows, roff)
         return [rows[roff[i]:roff[i + 1]] for i in range(nq)]
+
+    @staticmethod
+    def _fetch_rows(ctx, total, nq):
+        """The `total` result rows of the last match call (int32 (total, 7)) and their query offsets."""
+        rows = np.empty((total, 7), np.int32)
+        roff = np.zeros(nq + 1, np.int64)
+        ctx.check(ctx.lib.afp_fetch_match_rows(ctx.h, rows.ctypes.data if total else None, 1,
+                                               roff.ctypes.data_as(C.POINTER(C.c_int64))))
+        return rows, roff
 
     @staticmethod
     def _sort_by_count(rows, roff):
@@ -419,10 +418,7 @@ class Matcher(object):
         p = self._params()
         p.publish_candidates = 1
         ctx = ht._sync_device()
-        rows = np.empty((self._run(ctx, p, qrows, nq, qoff), 7), np.int32)
-        roff = np.zeros(nq + 1, np.int64)
-        ctx.check(ctx.lib.afp_fetch_match_rows(ctx.h, rows.ctypes.data if len(rows) else None, 1,
-                                               roff.ctypes.data_as(C.POINTER(C.c_int64))))
+        rows, roff = self._fetch_rows(ctx, self._run(ctx, p, qrows, nq, qoff), nq)
         cand = np.zeros((nq, max(int(self.search_depth), 1), 3), np.float64)
         cnts = np.zeros((nq, 2), np.int32)
         if nq:
@@ -433,14 +429,10 @@ class Matcher(object):
         """Table-shard side of a sharded match (SURVEY.md §8e): `ht`'s device copy holds only
         this rank's id range.  Returns one record per query for dist.merge_sharded_results:
         {"n_above", "cand" (k,3) [id, raw, weight], "rows" (r,7) with LOCAL ranks}."""
-        arrs = [np.asarray(q, dtype=np.int32).reshape(-1, 2) for q in queries]
-        qoff = np.zeros(len(arrs) + 1, np.int64)
-        if arrs:
-            qoff[1:] = np.cumsum([len(a) for a in arrs])
-        packed = np.ascontiguousarray(np.concatenate(arrs)) if arrs else np.zeros((0, 2), np.int32)
+        packed, qoff = _lib.pack_rows(queries)
         rows, roff, cand, cnts = self._publish_call(ht, packed, qoff)
         return [{"n_above": int(cnts[i, 1]), "cand": cand[i, :cnts[i, 0]].copy(),
-                 "rows": rows[roff[i]:roff[i + 1]].copy()} for i in range(len(arrs))]
+                 "rows": rows[roff[i]:roff[i + 1]].copy()} for i in range(len(qoff) - 1)]
 
     def match_batch_shard_packed(self, ht, packed_queries, row_cap=16):
         """match_batch_shard for a packed (rows, offsets) query batch, returning the fixed-size
@@ -498,11 +490,10 @@ class Matcher(object):
 
     def _match_files(self, analyzer, ht, filenames, numbers):
         self._params()                     # illustrate raises before any file is read
-        saved = (analyzer.soundfiledur, analyzer.soundfiletotaldur, analyzer.soundfilecount)
         durs = []
         on_device = hasattr(ht, "_sync_device") and _lib.context(ht.device) is _lib.context(analyzer.device)
         out = []
-        try:
+        with analyzer._counters_restored_on_error():
             for c0 in range(0, len(filenames), max(1, int(self.max_files_per_call))):
                 names = filenames[c0:c0 + max(1, int(self.max_files_per_call))]
                 queries = analyzer._hashes_of_files(names, rows_on_device=on_device)
@@ -518,9 +509,6 @@ class Matcher(object):
                     if self.sort_by_time:
                         rows = rows[(-rows[:, 2]).argsort(), :]
                     out.append((rows[:self.max_returns, :], sec, len(q)))
-        except BaseException:
-            analyzer.soundfiledur, analyzer.soundfiletotaldur, analyzer.soundfilecount = saved
-            raise
         analyzer.last_batch_durations = durs
         return out
 
