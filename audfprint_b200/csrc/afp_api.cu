@@ -8,8 +8,6 @@
 
 #include "afp_internal.cuh"
 
-int afp_write_hashes(afp_ctx* c);
-
 extern "C" {
 
 int afp_abi_version(void) { return AFP_ABI_VERSION; }
@@ -70,9 +68,9 @@ void afp_destroy(afp_ctx* c) {
   for (int i = 0; i <= AFP_NSTAGES; ++i)
     if (c->ev[i]) cudaEventDestroy(c->ev[i]);
   DevBuf* bufs[] = {&c->d_window, &c->d_window_f, &c->d_twid_f, &c->d_gauss, &c->d_twid, &c->d_pcm_stage, &c->d_items, &c->d_tile_item, &c->d_file_col_base,
-                    &c->d_logs, &c->d_nyq, &c->d_tile_stats, &c->d_item_stats, &c->d_fwd_val, &c->d_fwd_bin,
+                    &c->d_logs, &c->d_nyq, &c->d_tile_stats, &c->d_item_stats, &c->d_stats_ticket, &c->d_fwd_val, &c->d_fwd_bin,
                     &c->d_fwd_cnt, &c->d_pk_bin, &c->d_pk_cnt, &c->d_item_scols, &c->d_item_npeaks, &c->d_lm,
-                    &c->d_col_cnt, &c->d_file_tot, &c->d_file_off, &c->d_hashes, &c->d_pk_off, &c->d_pk_rows,
+                    &c->d_col_cnt, &c->d_hash_stage, &c->d_file_tot, &c->d_file_off, &c->d_hashes, &c->d_pk_off, &c->d_pk_rows,
                     &c->d_pk_in, &c->d_pk_inoff, &c->d_pk_status, &c->d_tmp, &c->tab.table, &c->tab.counts, &c->tab.hashesperid, &c->d_q, &c->d_qoff,
                     &c->d_hit_off, &c->d_hits, &c->d_st_off, &c->d_st_ids, &c->d_st_eval, &c->d_st_seq, &c->d_st_ovf,
                     &c->d_st_cnt, &c->d_st_seg, &c->d_st_heavy, &c->d_st_part, &c->d_st_scan, &c->d_st_obkt,
@@ -186,7 +184,7 @@ int afp_set_analyzer(afp_ctx* c, const afp_analyzer_params* p, const double* win
 // (afp_fingerprint_batch, afp_sgram, afp_fingerprint_from_logs), and upload its item table.
 static int reserve_batch(afp_ctx* c) {
   const int32_t nfiles = c->nfiles;
-  const int64_t frames = c->total_frames, tiles = c->total_tiles, cols = c->total_cols;
+  const int64_t frames = c->total_frames, tiles = c->total_tiles;
   const size_t P = (size_t)c->ap.maxpksperframe, F = (size_t)c->ap.maxpairsperpeak;
   const size_t fr = (size_t)frames + 1;
   AFP_CUDA(c, c->d_items.reserve(sizeof(ItemDesc) * (size_t)(c->nitems + 1)));
@@ -196,6 +194,7 @@ static int reserve_batch(afp_ctx* c) {
   AFP_CUDA(c, c->d_nyq.reserve(sizeof(double) * fr));
   AFP_CUDA(c, c->d_tile_stats.reserve(sizeof(double) * 3 * (size_t)(tiles + 1)));
   AFP_CUDA(c, c->d_item_stats.reserve(sizeof(ItemStats) * (size_t)(c->nitems + 1)));
+  AFP_CUDA(c, c->d_stats_ticket.reserve(sizeof(int32_t) * (size_t)(c->nitems + 1)));
   AFP_CUDA(c, c->d_fwd_val.reserve(sizeof(double) * P * fr));
   AFP_CUDA(c, c->d_fwd_bin.reserve(P * fr));
   AFP_CUDA(c, c->d_fwd_cnt.reserve(fr));
@@ -203,17 +202,29 @@ static int reserve_batch(afp_ctx* c) {
   AFP_CUDA(c, c->d_pk_cnt.reserve(fr));
   AFP_CUDA(c, c->d_item_scols.reserve(sizeof(int32_t) * (size_t)(c->nitems + 1)));
   AFP_CUDA(c, c->d_item_npeaks.reserve(sizeof(int32_t) * (size_t)(c->nitems + 1)));
-  AFP_CUDA(c, c->d_lm.reserve(sizeof(uint32_t) * P * F * fr));
-  AFP_CUDA(c, c->d_col_cnt.reserve(sizeof(int32_t) * (size_t)(cols + 1)));
   AFP_CUDA(c, c->d_file_tot.reserve(sizeof(int32_t) * (size_t)(nfiles + 1)));
   AFP_CUDA(c, c->d_file_off.reserve(sizeof(int64_t) * (size_t)(nfiles + 1)));
   // upper bound on the output: every hash slot distinct
+  AFP_CUDA(c, c->d_hash_stage.reserve(sizeof(int32_t) * 2 * P * F * fr));
   AFP_CUDA(c, c->d_hashes.reserve(sizeof(int32_t) * 2 * (P * F * fr + 1)));
-  if (c->nitems > 0)
+  // a caller that fingerprints batch after batch of one layout (files of equal lengths) uploads the
+  // item table once: it is compared with what the buffer holds, not re-sent, and the tile table stays
+  if (c->nitems > 0 && !(c->items_tag.is(c->d_items) && c->up_items.size() == c->h_items.size() &&
+                         memcmp(c->up_items.data(), c->h_items.data(), sizeof(ItemDesc) * c->h_items.size()) == 0)) {
+    c->items_tag.clear();
+    c->tile_tag.clear();
     AFP_CUDA(c, cudaMemcpyAsync(c->d_items.p, c->h_items.data(), sizeof(ItemDesc) * (size_t)c->nitems,
                                 cudaMemcpyHostToDevice, c->stream));
-  AFP_CUDA(c, cudaMemcpyAsync(c->d_file_col_base.p, c->h_file_col_base.data(),
-                              sizeof(int64_t) * (size_t)(nfiles + 1), cudaMemcpyHostToDevice, c->stream));
+    c->up_items = c->h_items;
+    c->items_tag.set(c->d_items);
+  }
+  if (!(c->fcb_tag.is(c->d_file_col_base) && c->up_file_col_base == c->h_file_col_base)) {
+    c->fcb_tag.clear();
+    AFP_CUDA(c, cudaMemcpyAsync(c->d_file_col_base.p, c->h_file_col_base.data(),
+                                sizeof(int64_t) * (size_t)(nfiles + 1), cudaMemcpyHostToDevice, c->stream));
+    c->up_file_col_base = c->h_file_col_base;
+    c->fcb_tag.set(c->d_file_col_base);
+  }
   return AFP_OK;
 }
 
@@ -329,7 +340,7 @@ static int run_chunked(afp_ctx* c, const void* pcm, int dtype, int32_t nfiles, c
     if (!rc) rc = afp_launch_stft(c, dpcm, dtype, nullptr, t0, t1 - t0);
     if (!rc) rc = afp_launch_stats(c, i0, i1 - i0);
     if (!rc) rc = afp_launch_peaks(c, i0, i1 - i0);
-    if (!rc) rc = afp_launch_landmarks(c, i0, i1 - i0);
+    if (!rc) rc = afp_launch_file_hashes(c, f0, f1 - f0);
     c->stream = user;
     if (rc) return rc;
   }
@@ -369,7 +380,7 @@ int afp_fingerprint_batch(afp_ctx* c, const void* pcm, int pcm_dtype, int pcm_on
     AFP_MARK(3);
     if ((rc = afp_launch_peaks(c, 0, c->nitems))) return rc;
     AFP_MARK(4);
-    if ((rc = afp_launch_landmarks(c, 0, c->nitems))) return rc;
+    if ((rc = afp_launch_file_hashes(c, 0, c->nfiles))) return rc;
     if ((rc = afp_launch_hashes(c))) return rc;
     if ((rc = afp_write_hashes(c))) return rc;
     AFP_MARK(5);
@@ -438,7 +449,7 @@ int afp_fingerprint_from_logs(afp_ctx* c, const void* logs, int logs_on_host, in
     AFP_CUDA(c, cudaMemcpyAsync(c->d_item_stats.p, st.data(), sizeof(ItemStats) * st.size(), cudaMemcpyHostToDevice,
                                 c->stream));
   if ((rc = afp_launch_peaks(c, 0, c->nitems))) return rc;
-  if ((rc = afp_launch_landmarks(c, 0, c->nitems))) return rc;
+  if ((rc = afp_launch_file_hashes(c, 0, c->nfiles))) return rc;
   if ((rc = afp_launch_hashes(c))) return rc;
   if ((rc = afp_write_hashes(c))) return rc;
   c->batch_valid = true;
@@ -522,7 +533,7 @@ int afp_fingerprint_from_peaks(afp_ctx* c, const int32_t* peak_rows, int rows_on
   c->total_frames = cols;
   c->total_tiles = 0;
   c->total_cols = cols;
-  // only what the scatter and K3 read: pk slots, landmark slots, column counts, file offsets
+  // only what the scatter and K3 use: pk slots, staged rows, file counts and offsets
   const size_t fr = (size_t)cols + 1;
   AFP_CUDA(c, c->d_items.reserve(sizeof(ItemDesc) * (size_t)(c->nitems + 1)));
   AFP_CUDA(c, c->d_file_col_base.reserve(sizeof(int64_t) * (size_t)(nfiles + 1)));
@@ -530,10 +541,12 @@ int afp_fingerprint_from_peaks(afp_ctx* c, const int32_t* peak_rows, int rows_on
   AFP_CUDA(c, c->d_item_npeaks.reserve(sizeof(int32_t) * npeaks.size()));
   AFP_CUDA(c, c->d_pk_bin.reserve(P * fr));
   AFP_CUDA(c, c->d_pk_cnt.reserve(fr));
-  AFP_CUDA(c, c->d_lm.reserve(sizeof(uint32_t) * P * F * fr));
-  AFP_CUDA(c, c->d_col_cnt.reserve(sizeof(int32_t) * fr));
+  AFP_CUDA(c, c->d_hash_stage.reserve(sizeof(int32_t) * 2 * P * F * fr));
   AFP_CUDA(c, c->d_file_tot.reserve(sizeof(int32_t) * (size_t)(nfiles + 1)));
   AFP_CUDA(c, c->d_file_off.reserve(sizeof(int64_t) * (size_t)(nfiles + 1)));
+  c->items_tag.clear();   // written here, not by reserve_batch
+  c->fcb_tag.clear();
+  c->tile_tag.clear();
   if (c->nitems > 0)
     AFP_CUDA(c, cudaMemcpyAsync(c->d_items.p, c->h_items.data(), sizeof(ItemDesc) * (size_t)c->nitems,
                                 cudaMemcpyHostToDevice, c->stream));
@@ -549,7 +562,7 @@ int afp_fingerprint_from_peaks(afp_ctx* c, const int32_t* peak_rows, int rows_on
   // the scatter never writes pk_cnt above maxpks, so K3 runs safely before the status is read: one sync
   int rc = afp_launch_scatter_peaks(c, drows, c->d_pk_inoff.as<int64_t>(), nrows, nfiles, S,
                                     c->d_pk_status.as<int32_t>());
-  if (!rc) rc = afp_launch_landmarks(c, 0, c->nitems);
+  if (!rc) rc = afp_launch_file_hashes(c, 0, nfiles);
   if (!rc) rc = afp_launch_hashes(c);
   if (rc) return rc;
   std::vector<int32_t> st((size_t)nfiles + 1, 0);

@@ -17,129 +17,206 @@ namespace {
 
 struct HashArgs {
   const ItemDesc* items;
-  int item0;
-  int nitems, nfiles, shifts, maxpks, fanout, targetdf, mindt, targetdt;
+  int file0;                    // first file of the launch
+  int shifts, maxpks, fanout, targetdf, mindt, targetdt;
+  int win;                      // source columns per window
   const uint8_t* pk_bin;
   const uint8_t* pk_cnt;
   const int32_t* item_scols;
-  uint32_t* lm;                 // [frames][maxpks][fanout]
-  const int64_t* file_col_base; // [nfiles+1]
-  int64_t total_cols;
-  int32_t* col_cnt;             // [total_cols] counts, then exclusive per-file offsets
-  int32_t* file_tot;            // [nfiles]
+  uint32_t* lm;                 // [frames][maxpks][fanout]      (afp_landmarks_from_peaks)
+  const int64_t* file_col_base; // [nfiles+1]                    (afp_landmarks_from_peaks)
+  int32_t* col_cnt;             // [cols] counts, then offsets   (afp_landmarks_from_peaks)
+  int32_t* file_tot;            // [nfiles] rows of each file
   const int64_t* file_off;      // [nfiles+1]
+  int32_t* stage;               // [P*F*frames][2] file f's rows from row P*F*(frame_base of its shift-0 item)
   int32_t* hashes;              // [total][2]
 };
 
-// One CTA per item.  The item's peaks are first compacted (window by window) into a
-// shared-memory list sorted by (column, bin) — the order the reference visits them in —
-// then one thread per SOURCE PEAK scans the following list entries: ~18 candidates on
-// average instead of 61 mostly-empty columns, and no thread is spent on empty slots.
-// The hash slots of `lm` are pre-filled with AFP_NO_HASH by a memset.
-constexpr int LM_THREADS = 256;
-// Peak entries per window, packed (col - w0):20 | slot:4 | bin:8.  The column is stored relative to
-// the window start: a window spans at most W + targetdt <= PCAP columns, whatever the item's length.
-constexpr int PCAP = 11264;
+constexpr int K3_THREADS = 256;
+
+// Exclusive prefix of v over the CTA's K3_THREADS threads in thread order; *total gets the sum.
+// s_w holds K3_THREADS / 32 ints.
+__device__ __forceinline__ int block_excl_scan(int v, int* s_w, int* total) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  int x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) s_w[w] = x;
+  __syncthreads();
+  int before = 0, tot = 0;
+#pragma unroll
+  for (int k = 0; k < K3_THREADS / 32; ++k) {
+    const int t = s_w[k];
+    before += (k < w) ? t : 0;
+    tot += t;
+  }
+  *total = tot;
+  __syncthreads();   // s_w is rewritten by the next call
+  return before + x - v;
+}
+
+// The peaks of a window of S items, compacted into shared memory in the order the reference visits
+// them: item by item, each sorted by (column, bin).  Item s (last peak column + 1 s_scols[s], first
+// frame s_fb[s], both in shared memory so that a column's count is the only dependent load) contributes
+// its columns [w0, min(s_scols[s], w0 + span)); its entries are s_pk[s_seg[s] .. s_seg[s+1]), packed
+// (col - w0):20 | slot:4 | bin:8.  The column is stored relative to the window start, so a window of
+// any item's length fits the 20-bit field.  Ends with a barrier.
+__device__ __forceinline__ void compact_window(const HashArgs& a, const int* s_scols, const int64_t* s_fb, int S,
+                                               int w0, int span, uint32_t* s_pk, int* s_seg, int* s_w) {
+  const int P = a.maxpks;
+  int run = 0;
+  for (int j0 = 0; j0 < S * span; j0 += K3_THREADS) {
+    const int j = j0 + threadIdx.x;
+    const int s = j / span, c = w0 + (j - s * span);
+    int n = 0;
+    int64_t fc = 0;
+    if (j < S * span && c < s_scols[s]) {
+      fc = s_fb[s] + c;
+      n = a.pk_cnt[fc];
+    }
+    int tot;
+    const int at = run + block_excl_scan(n, s_w, &tot);
+    if (j < S * span && c == w0) s_seg[s] = at;
+    for (int k = 0; k < n; ++k) s_pk[at + k] = ((uint32_t)(c - w0) << 12) | ((uint32_t)k << 8) | a.pk_bin[fc * P + k];
+    run += tot;
+  }
+  if (threadIdx.x == 0) s_seg[S] = run;
+  __syncthreads();
+}
+
+// The hashes of source entry i of one item's window list s_pk[.. end) (column < scols): its pairs with
+// the entries that follow it, in (column, bin) order, at most `fanout` (audfprint_analyze.py:325-343),
+// packed as landmarks2hashes packs them (:92-95).  Returns how many were written to out.
+__device__ __forceinline__ int pair_source(const HashArgs& a, const uint32_t* s_pk, int i, int end, int w0, int scols,
+                                           uint32_t* out) {
+  const uint32_t e = s_pk[i];
+  const int col = w0 + (int)(e >> 12), slot = (int)((e >> 8) & 15), b1 = (int)(e & 255);
+  const int c2lo = col + a.mindt, c2hi = min(scols, col + a.targetdt);     // :331-332
+  int n = 0;
+  for (int j = (a.mindt > 0) ? i + 1 : i - slot; j < end && n < a.fanout; ++j) {
+    const uint32_t t = s_pk[j];
+    const int c2 = w0 + (int)(t >> 12);
+    if (c2 >= c2hi) break;
+    if (c2 < c2lo) continue;
+    const int b2 = (int)(t & 255);
+    if (abs(b2 - b1) < a.targetdf)                                          // :335
+      out[n++] = ((uint32_t)(b1 & 0xFF) << 12) | ((uint32_t)((b2 - b1) & 0x3F) << 6) | (uint32_t)((c2 - col) & 0x3F);
+  }
+  return n;
+}
+
+// Landmarks of one item (afp_landmarks_from_peaks): every peak owns `fanout` slots of lm, pre-filled
+// with AFP_NO_HASH by a memset.  One thread per source peak.
+constexpr int PCAP = 11264;   // peak entries per window
 static_assert(PCAP <= (1 << 20), "a window's relative column must fit the 20-bit field");
 
-__global__ void __launch_bounds__(LM_THREADS) afp_landmark_kernel(HashArgs a) {
+__global__ void __launch_bounds__(K3_THREADS) afp_landmark_kernel(HashArgs a) {
   __shared__ uint32_t s_pk[PCAP];
-  __shared__ int s_scan[LM_THREADS];
-  __shared__ int s_run;
-  const ItemDesc it = a.items[a.item0 + blockIdx.x];
-  const int scols = a.item_scols[a.item0 + blockIdx.x];   // last peak column + 1 (:321)
-  const int P = a.maxpks, F = a.fanout, tid = threadIdx.x;
-  const int64_t base = it.frame_base;
-  const int W = max(64, PCAP / P - a.targetdt - 1);       // source columns per window
+  __shared__ int s_seg[2];
+  __shared__ int s_w[K3_THREADS / 32];
+  __shared__ int s_scols[1];
+  __shared__ int64_t s_fb[1];
+  const int scols = a.item_scols[0];                       // last peak column + 1 (:321)
+  const int P = a.maxpks, F = a.fanout;
+  const int64_t base = a.items[0].frame_base;
+  const int W = max(64, PCAP / P - a.targetdt - 1);       // source columns per window: P * (W + targetdt) <= PCAP
+  if (threadIdx.x == 0) {
+    s_scols[0] = scols;
+    s_fb[0] = base;
+  }
+  __syncthreads();
   for (int w0 = 0; w0 < scols; w0 += W) {
-    const int wend = min(scols, w0 + W + a.targetdt);     // sources in [w0, w0+W), targets up to +targetdt
-    if (tid == 0) s_run = 0;
-    __syncthreads();
-    for (int c0 = w0; c0 < wend; c0 += LM_THREADS) {      // compaction, column order
-      const int c = c0 + tid;
-      const int n = (c < wend) ? a.pk_cnt[base + c] : 0;
-      s_scan[tid] = n;
-      __syncthreads();
-      for (int o = 1; o < LM_THREADS; o <<= 1) {
-        const int v = (tid >= o) ? s_scan[tid - o] : 0;
-        __syncthreads();
-        s_scan[tid] += v;
-        __syncthreads();
-      }
-      const int at = s_run + s_scan[tid] - n;
-      for (int k = 0; k < n; ++k)
-        s_pk[at + k] = ((uint32_t)(c - w0) << 12) | ((uint32_t)k << 8) | a.pk_bin[(base + c) * P + k];
-      __syncthreads();
-      if (tid == LM_THREADS - 1) s_run += s_scan[tid];
-      __syncthreads();
-    }
-    const int np = s_run;
-    for (int i = tid; i < np; i += LM_THREADS) {
+    compact_window(a, s_scols, s_fb, 1, w0, W + a.targetdt, s_pk, s_seg, s_w);
+    const int np = s_seg[1];
+    for (int i = threadIdx.x; i < np; i += K3_THREADS) {
       const uint32_t e = s_pk[i];
-      const int col = w0 + (int)(e >> 12), slot = (int)((e >> 8) & 15), b1 = (int)(e & 255);
+      const int col = w0 + (int)(e >> 12);
       if (col >= w0 + W) break;                           // entries are column-sorted: only targets remain
-      uint32_t* out = a.lm + ((base + col) * P + slot) * F;
-      const int c2lo = col + a.mindt, c2hi = min(scols, col + a.targetdt);     // :331-332
-      int n = 0;
-      for (int j = (a.mindt > 0) ? i + 1 : i - slot; j < np && n < F; ++j) {
-        const uint32_t t = s_pk[j];
-        const int c2 = w0 + (int)(t >> 12);
-        if (c2 >= c2hi) break;
-        if (c2 < c2lo) continue;
-        const int b2 = (int)(t & 255);
-        if (abs(b2 - b1) < a.targetdf)                                          // :335
-          out[n++] = ((uint32_t)(b1 & 0xFF) << 12) | ((uint32_t)((b2 - b1) & 0x3F) << 6) |
-                     (uint32_t)((c2 - col) & 0x3F);                             // :92-95
-      }
+      pair_source(a, s_pk, i, np, w0, scols, a.lm + ((base + col) * P + ((e >> 8) & 15)) * F);
     }
     __syncthreads();
   }
 }
 
-__device__ __forceinline__ int find_file(const int64_t* fcb, int nfiles, int64_t gcol) {
-  int lo = 0, hi = nfiles;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (fcb[mid] <= gcol) lo = mid; else hi = mid;
+// K3 of the fingerprint batch: one CTA per file, window by window over its columns.  The peaks of the
+// file's `shifts` items are compacted (compact_window) and paired into hash slots in shared memory,
+// [column][shift][slot][fanout] (AFP_NO_HASH = empty).  All hashes of a file that carry the same time
+// value live in one column, so its (time, hash)-sorted unique rows (the concatenate / sort / unique
+// tail of wavfile2hashes, :401-422) are, column by column, the sorted unique union of that column's
+// slots: an insertion sort in place, one thread per column.  The rows go to the file's staging region,
+// whose P*F slots per frame of all its items bound its row count; file_tot gets the count.
+constexpr int K3_SLOTS = 4096;   // hash slots of a window: W * shifts * maxpks * fanout <= K3_SLOTS
+
+// 8 CTAs per SM (32 registers, no spills; 27 KB of shared memory each at the default settings, with the
+// carveout at its maximum): a batch of 1024 files is one wave on 132 SMs
+__global__ void __launch_bounds__(K3_THREADS, 8) afp_file_hash_kernel(HashArgs a) {
+  extern __shared__ uint32_t s_pk[];          // shifts * maxpks * (W + targetdt) entries
+  __shared__ uint32_t s_slot[K3_SLOTS];
+  __shared__ int s_seg[AFP_MAX_MERGE + 1];
+  __shared__ int s_w[K3_THREADS / 32];
+  __shared__ int s_scols[AFP_MAX_MERGE];     // shifts <= AFP_MAX_MERGE
+  __shared__ int64_t s_fb[AFP_MAX_MERGE];
+  const int f = a.file0 + blockIdx.x, S = a.shifts, it0 = f * S, tid = threadIdx.x;
+  const int P = a.maxpks, F = a.fanout, SPF = S * P * F, W = a.win;
+  for (int s = tid; s < S; s += K3_THREADS) {
+    s_scols[s] = a.item_scols[it0 + s];
+    s_fb[s] = a.items[it0 + s].frame_base;
   }
-  return lo;
+  __syncthreads();
+  int scols = 0;
+  for (int s = 0; s < S; ++s) scols = max(scols, s_scols[s]);
+  int2* out = reinterpret_cast<int2*>(a.stage) + (int64_t)P * F * s_fb[0];
+  int run = 0;
+  for (int w0 = 0; w0 < scols; w0 += W) {
+    const int ncol = min(W, scols - w0);
+    for (int e = tid; e < ncol * SPF; e += K3_THREADS) s_slot[e] = AFP_NO_HASH;
+    compact_window(a, s_scols, s_fb, S, w0, W + a.targetdt, s_pk, s_seg, s_w);
+    for (int s = 0; s < S; ++s) {
+      const int end = s_seg[s + 1], sc = s_scols[s];
+      for (int i = s_seg[s] + tid; i < end; i += K3_THREADS) {
+        const uint32_t e = s_pk[i];
+        const int cc = (int)(e >> 12);
+        if (cc >= W) break;                       // entries are column-sorted: only targets remain
+        pair_source(a, s_pk, i, end, w0, sc, s_slot + ((cc * S + s) * P + (int)((e >> 8) & 15)) * F);
+      }
+    }
+    __syncthreads();
+    for (int c0 = 0; c0 < ncol; c0 += K3_THREADS) {
+      const int cc = c0 + tid;
+      uint32_t* buf = s_slot + cc * SPF;
+      int n = 0;
+      if (cc < ncol)
+        for (int e = 0; e < SPF; ++e) {           // reads slot e, writes slots < n <= e
+          const uint32_t h = buf[e];
+          if (h == AFP_NO_HASH) continue;
+          int i = n;
+          while (i > 0 && buf[i - 1] > h) --i;
+          if (i > 0 && buf[i - 1] == h) continue; // duplicate across shifts (:417)
+          for (int k = n; k > i; --k) buf[k] = buf[k - 1];
+          buf[i] = h;
+          ++n;
+        }
+      int tot;
+      const int at = run + block_excl_scan(n, s_w, &tot);
+      for (int k = 0; k < n; ++k) out[at + k] = make_int2(w0 + cc, (int)buf[k]);
+      run += tot;
+    }
+    __syncthreads();                              // s_slot and s_pk are refilled by the next window
+  }
+  if (tid == 0) a.file_tot[f] = run;
 }
 
-// Sorted unique union of the hash slots of one (file, column) over all shifts.
-template <bool WRITE>
-__global__ void __launch_bounds__(128) afp_merge_kernel(HashArgs a) {
-  const int64_t gcol = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (gcol >= a.total_cols) return;
-  const int f = find_file(a.file_col_base, a.nfiles, gcol);
-  const int col = (int)(gcol - a.file_col_base[f]);
-  uint32_t buf[AFP_MAX_MERGE];
-  int n = 0;
-  const int PF = a.maxpks * a.fanout;
-  for (int s = 0; s < a.shifts; ++s) {
-    const ItemDesc it = a.items[f * a.shifts + s];
-    if (col >= it.nframes) continue;
-    if (a.pk_cnt[it.frame_base + col] == 0) continue;
-    const uint32_t* src = a.lm + (it.frame_base + col) * PF;
-    for (int e = 0; e < PF; ++e) {
-      const uint32_t h = src[e];
-      if (h == AFP_NO_HASH) continue;
-      int i = n;
-      while (i > 0 && buf[i - 1] > h) --i;
-      if (i > 0 && buf[i - 1] == h) continue;        // duplicate across shifts (:417)
-      for (int k = n; k > i; --k) buf[k] = buf[k - 1];
-      buf[i] = h;
-      ++n;
-    }
-  }
-  if (!WRITE) {
-    a.col_cnt[gcol] = n;
-  } else {
-    int32_t* out = a.hashes + 2 * (a.file_off[f] + a.col_cnt[gcol]);
-    for (int i = 0; i < n; ++i) {
-      out[2 * i] = col;
-      out[2 * i + 1] = (int32_t)buf[i];
-    }
-  }
+// Each file's rows from its staging region to their place in the dense output.
+__global__ void __launch_bounds__(256) afp_gather_rows_kernel(HashArgs a) {
+  const int f = blockIdx.x;
+  const int64_t n = a.file_off[f + 1] - a.file_off[f];
+  const int2* src = reinterpret_cast<const int2*>(a.stage) +
+                    (int64_t)a.maxpks * a.fanout * a.items[(int64_t)f * a.shifts].frame_base;
+  int2* dst = reinterpret_cast<int2*>(a.hashes) + a.file_off[f];
+  for (int64_t i = threadIdx.x; i < n; i += 256) dst[i] = src[i];
 }
 
 // In-place exclusive scan of col_cnt inside each file; file totals out.
@@ -264,29 +341,28 @@ __global__ void afp_lm_rows_kernel(const uint32_t* lm, int T, int PF, int32_t* c
 
 }  // namespace
 
-// Runs landmark -> count -> scans.  The write pass needs the total (to size the
-// output) and is issued by afp_finish_hashes.
 static HashArgs make_args(afp_ctx* c) {
   HashArgs a;
   a.items = c->d_items.as<ItemDesc>();
-  a.item0 = 0;
-  a.nitems = c->nitems;
-  a.nfiles = c->nfiles;
+  a.file0 = 0;
   a.shifts = c->ap.shifts;
   a.maxpks = c->ap.maxpksperframe;
   a.fanout = c->ap.maxpairsperpeak;
   a.targetdf = c->ap.targetdf;
   a.mindt = c->ap.mindt;
   a.targetdt = c->ap.targetdt;
+  // source columns per window of afp_file_hash_kernel: whole passes of K3_THREADS columns when they fit
+  const int w = K3_SLOTS / (a.shifts * a.maxpks * a.fanout);
+  a.win = w >= K3_THREADS ? w / K3_THREADS * K3_THREADS : w;
   a.pk_bin = c->d_pk_bin.as<uint8_t>();
   a.pk_cnt = c->d_pk_cnt.as<uint8_t>();
   a.item_scols = c->d_item_scols.as<int32_t>();
   a.lm = c->d_lm.as<uint32_t>();
   a.file_col_base = c->d_file_col_base.as<int64_t>();
-  a.total_cols = c->total_cols;
   a.col_cnt = c->d_col_cnt.as<int32_t>();
   a.file_tot = c->d_file_tot.as<int32_t>();
   a.file_off = c->d_file_off.as<int64_t>();
+  a.stage = c->d_hash_stage.as<int32_t>();
   a.hashes = c->d_hashes.as<int32_t>();
   return a;
 }
@@ -346,6 +422,9 @@ int afp_landmarks_from_peaks_impl(afp_ctx* c, const int32_t* rows_in, int64_t n,
   AFP_CUDA(c, c->d_pk_inoff.reserve(sizeof(int64_t) * 2));
   AFP_CUDA(c, c->d_pk_status.reserve(sizeof(int32_t) * 2));
   const int64_t fcb[2] = {0, T}, off[2] = {0, n};
+  c->items_tag.clear();   // written here, not by reserve_batch
+  c->fcb_tag.clear();
+  c->tile_tag.clear();
   AFP_CUDA(c, cudaMemcpyAsync(c->d_items.p, &it, sizeof(it), cudaMemcpyHostToDevice, c->stream));
   AFP_CUDA(c, cudaMemcpyAsync(c->d_file_col_base.p, fcb, sizeof(fcb), cudaMemcpyHostToDevice, c->stream));
   AFP_CUDA(c, cudaMemcpyAsync(c->d_pk_inoff.p, off, sizeof(off), cudaMemcpyHostToDevice, c->stream));
@@ -357,7 +436,7 @@ int afp_landmarks_from_peaks_impl(afp_ctx* c, const int32_t* rows_in, int64_t n,
   c->nfiles = 1; c->nitems = 1; c->total_frames = T; c->total_cols = T;
   HashArgs a = make_args(c);
   AFP_CUDA(c, cudaMemsetAsync(c->d_lm.p, 0xFF, sizeof(uint32_t) * P * F * fr, c->stream));
-  afp_landmark_kernel<<<1, LM_THREADS, 0, c->stream>>>(a);
+  afp_landmark_kernel<<<1, K3_THREADS, 0, c->stream>>>(a);
   AFP_CUDA(c, cudaGetLastError());
   afp_lm_rows_kernel<false><<<(T + 127) / 128, 128, 0, c->stream>>>(a.lm, T, (int)(P * F), a.col_cnt, nullptr);
   AFP_CUDA(c, cudaGetLastError());
@@ -390,18 +469,16 @@ int afp_launch_scan_i32_to_i64(afp_ctx* c, const int32_t* in, int64_t* out, int6
   return AFP_OK;
 }
 
-int afp_launch_landmarks(afp_ctx* c, int item0, int nitems) {
-  if (nitems <= 0 || c->total_frames == 0) return AFP_OK;
+int afp_launch_file_hashes(afp_ctx* c, int file0, int nfiles) {
+  if (nfiles <= 0) return AFP_OK;
   HashArgs a = make_args(c);
-  a.item0 = item0;
-  {   // empty hash slots = AFP_NO_HASH (0xFFFFFFFF): byte fill of this launch's slot range
-    const ItemDesc& i0 = c->h_items[item0];
-    const ItemDesc& i1 = c->h_items[item0 + nitems - 1];
-    const size_t per_frame = (size_t)c->ap.maxpksperframe * c->ap.maxpairsperpeak * sizeof(uint32_t);
-    const size_t f0 = (size_t)i0.frame_base, f1 = (size_t)i1.frame_base + i1.nframes;
-    if (f1 > f0) AFP_CUDA(c, cudaMemsetAsync((char*)c->d_lm.p + f0 * per_frame, 0xFF, (f1 - f0) * per_frame, c->stream));
-  }
-  afp_landmark_kernel<<<nitems, LM_THREADS, 0, c->stream>>>(a);
+  a.file0 = file0;
+  const size_t smem = sizeof(uint32_t) * a.shifts * a.maxpks * (a.win + a.targetdt);
+  AFP_CUDA(c, cudaFuncSetAttribute(afp_file_hash_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                   cudaSharedmemCarveoutMaxShared));
+  if (smem > 48 * 1024)
+    AFP_CUDA(c, cudaFuncSetAttribute(afp_file_hash_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  afp_file_hash_kernel<<<nfiles, K3_THREADS, smem, c->stream>>>(a);
   AFP_CUDA(c, cudaGetLastError());
   c->launches++;
   return AFP_OK;
@@ -409,22 +486,12 @@ int afp_launch_landmarks(afp_ctx* c, int item0, int nitems) {
 
 int afp_launch_hashes(afp_ctx* c) {
   if (c->nfiles == 0) return AFP_OK;
-  HashArgs a = make_args(c);
-  if (c->total_cols > 0) {
-    afp_merge_kernel<false><<<(unsigned)((c->total_cols + 127) / 128), 128, 0, c->stream>>>(a);
-    AFP_CUDA(c, cudaGetLastError());
-    c->launches++;
-  }
-  afp_file_scan_kernel<<<c->nfiles, 256, 0, c->stream>>>(a);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
   return afp_launch_scan_i32_to_i64(c, c->d_file_tot.as<int32_t>(), c->d_file_off.as<int64_t>(), c->nfiles);
 }
 
 int afp_write_hashes(afp_ctx* c) {
-  if (c->total_cols == 0) return AFP_OK;
-  HashArgs a = make_args(c);
-  afp_merge_kernel<true><<<(unsigned)((c->total_cols + 127) / 128), 128, 0, c->stream>>>(a);
+  if (c->nfiles == 0 || c->total_cols == 0) return AFP_OK;
+  afp_gather_rows_kernel<<<c->nfiles, 256, 0, c->stream>>>(make_args(c));
   AFP_CUDA(c, cudaGetLastError());
   c->launches++;
   return AFP_OK;

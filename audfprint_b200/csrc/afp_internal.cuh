@@ -35,6 +35,16 @@ struct DevBuf {
   template <class T> T* as() const { return reinterpret_cast<T*>(p); }
 };
 
+// Which allocation of a DevBuf some content was written to: a buffer that grows is reallocated with a
+// larger capacity, so (pointer, capacity) names one allocation even if the pointer is reused.
+struct BufTag {
+  const void* p = nullptr;
+  size_t cap = 0;
+  bool is(const DevBuf& b) const { return p != nullptr && p == b.p && cap == b.cap; }
+  void set(const DevBuf& b) { p = b.p; cap = b.cap; }
+  void clear() { p = nullptr; cap = 0; }
+};
+
 // Per-item (file x shift) descriptor built on the host for each batch.
 struct ItemDesc {
   int64_t sample_start;   // index of the item's first sample in the packed PCM buffer
@@ -95,6 +105,13 @@ struct afp_ctx {
   bool batch_valid = false;
   int pcm_dtype = 0;
 
+  // What d_items / d_file_col_base hold (uploaded by reserve_batch) and whether d_tile_item was built from
+  // them: a batch with the same layout as the last one skips both uploads and the tile table.  Code that
+  // writes these buffers otherwise clears the tags.
+  std::vector<ItemDesc> up_items;
+  std::vector<int64_t> up_file_col_base;
+  BufTag items_tag, fcb_tag, tile_tag;
+
   DevBuf d_pcm_stage;      // host->device staging when pcm_on_host
   DevBuf d_items;          // ItemDesc[nitems]
   DevBuf d_tile_item;      // int32[total_tiles] item of every K1 tile
@@ -103,6 +120,7 @@ struct afp_ctx {
   DevBuf d_nyq;            // double [total_frames]        log|S| of the Nyquist bin
   DevBuf d_tile_stats;     // double [total_tiles][3]      (max |S|^2, min log, sum log)
   DevBuf d_item_stats;     // ItemStats[nitems]
+  DevBuf d_stats_ticket;   // int32 [nitems]  CTAs of an item that finished its floored tile sums
   DevBuf d_fwd_val;        // double [total_frames][maxpks]
   DevBuf d_fwd_bin;        // uint8  [total_frames][maxpks]
   DevBuf d_fwd_cnt;        // uint8  [total_frames]
@@ -110,10 +128,11 @@ struct afp_ctx {
   DevBuf d_pk_cnt;         // uint8  [total_frames]
   DevBuf d_item_scols;     // int32 [nitems]  last peak column + 1
   DevBuf d_item_npeaks;    // int32 [nitems]
-  DevBuf d_lm;             // uint32 [total_frames][maxpks][fanout] landmark hashes (AFP_NO_HASH = none)
-  DevBuf d_col_cnt;        // int32 [total_cols]   unique hashes per (file, column); then exclusive offsets
-  DevBuf d_file_tot;       // int32 [nfiles]
+  DevBuf d_lm;             // uint32 [frames][maxpks][fanout] landmark hashes (AFP_NO_HASH = none), afp_landmarks_from_peaks
+  DevBuf d_col_cnt;        // int32 [frames]       landmarks per column; then exclusive offsets, afp_landmarks_from_peaks
+  DevBuf d_file_tot;       // int32 [nfiles]       rows of each file
   DevBuf d_file_off;       // int64 [nfiles+1]
+  DevBuf d_hash_stage;     // int32 [maxpks*fanout*total_frames][2]  K3's rows, file by file at maxpks*fanout*frame_base
   DevBuf d_hashes;         // int32 [total][2]
   int64_t total_hashes = -1;
   int64_t nlandmarks = -1;   // afp_landmarks_from_peaks result (rows in d_hashes)
@@ -198,9 +217,9 @@ int afp_launch_stft(afp_ctx* c, const void* pcm, int dtype, double* mag_out /* o
 int afp_launch_stats(afp_ctx* c, int item0, int nitems);
 int afp_launch_sgram(afp_ctx* c, double* sgram_out);
 int afp_launch_peaks(afp_ctx* c, int item0, int nitems);
-int afp_launch_landmarks(afp_ctx* c, int item0, int nitems);
-int afp_launch_hashes(afp_ctx* c);   // merge / scans (all files)
-int afp_write_hashes(afp_ctx* c);
+int afp_launch_file_hashes(afp_ctx* c, int file0, int nfiles);   // K3 of files file0 .. file0+nfiles-1, to d_hash_stage
+int afp_launch_hashes(afp_ctx* c);   // file row counts -> d_file_off (all files)
+int afp_write_hashes(afp_ctx* c);    // d_hash_stage -> dense d_hashes
 int afp_landmarks_from_peaks_impl(afp_ctx* c, const int32_t* rows, int64_t n, int on_host, int64_t* nlm);
 // peak rows of a ragged batch -> pk_bin / pk_cnt at each file's item (items f * item_stride of d_items)
 int afp_launch_scatter_peaks(afp_ctx* c, const int32_t* rows, const int64_t* off, int64_t nrows, int32_t nfiles,

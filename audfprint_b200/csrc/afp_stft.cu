@@ -441,37 +441,31 @@ __global__ void __launch_bounds__(K1_THREADS, K1Traits<R>::MIN_CTAS)
   }
 }
 
-// tile -> item table (one thread per item)
-__global__ void afp_tile_table_kernel(const ItemDesc* items, int nitems, int32_t* tile_item) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= nitems) return;
+// tile -> item table: one CTA per item, one thread per tile
+__global__ void __launch_bounds__(128) afp_tile_table_kernel(const ItemDesc* items, int32_t* tile_item) {
+  const int i = blockIdx.x;
   const ItemDesc it = items[i];
   const int nt = (it.nframes + FT - 1) / FT;
-  for (int k = 0; k < nt; ++k) tile_item[it.tile_base + k] = i;
+  for (int k = threadIdx.x; k < nt; k += blockDim.x) tile_item[it.tile_base + k] = i;
 }
 
 // ---- per-item statistics: floor, mean (audfprint_analyze.py:283-286) ----------
-// Three tiny launches.  (1) one WARP per item reduces the tile partials in a fixed order
-// (deterministic): floor, all-zero flag, mean of the un-floored logs, and whether anything
-// may sit below the floor.  (2) For such items only (digital silence, or the rare file whose
-// smallest bin is 120 dB below its largest) the tile sums are recomputed with the floor
-// applied, one CTA per tile so that a single long file cannot serialise the batch.
-// (3) the means of those items are re-reduced.
-__global__ void __launch_bounds__(256) afp_stats_kernel(const ItemDesc* items, int item0, int nitems,
-                                                        const double* tile_stats, ItemStats* out, int phase) {
-  const int lane = threadIdx.x & 31;
-  const int w = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (w >= nitems) return;
-  const int item = item0 + w;
-  if (phase == 1 && !out[item].floored) return;       // only items whose tile sums were floored
+// Two launches.  (1) One WARP per item reduces the tile partials in a fixed order (deterministic):
+// floor, all-zero flag, mean of the un-floored logs, and whether anything may sit below the floor.
+// (2) For such items only (digital silence, or a file whose smallest bin is 120 dB below its largest:
+// about one bench file in eight) the tile sums are recomputed with the floor applied, FS_SPLIT CTAs per
+// item so that a single long file cannot serialise the batch, and the last of an item's CTAs to finish
+// (a per-item ticket) re-reduces it with (1)'s code.
+__device__ __forceinline__ void reduce_item(const ItemDesc* items, int item, const double* tile_stats, ItemStats* out,
+                                            bool first, int lane, int* ticket) {
   const ItemDesc it = items[item];
   const int ntiles = (it.nframes + FT - 1) / FT;
   double m = 0.0, mn = INFINITY, sm = 0.0;
   for (int i = lane; i < ntiles; i += 32) {
     const double* ts = tile_stats + (size_t)(it.tile_base + i) * 3;
-    m = fmax(m, ts[0]);
-    mn = fmin(mn, ts[1]);
-    sm += ts[2];
+    m = fmax(m, __ldcg(ts));        // L2: the floored sums are written by other CTAs
+    mn = fmin(mn, __ldcg(ts + 1));
+    sm += __ldcg(ts + 2);
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
@@ -485,29 +479,44 @@ __global__ void __launch_bounds__(256) afp_stats_kernel(const ItemDesc* items, i
     st.logfloor = allzero ? 0.0 : log(sqrt(m) / 1e6);
     st.mean = (allzero || it.nframes == 0) ? 0.0 : sm / ((double)it.nframes * 257.0);
     st.allzero = allzero ? 1 : 0;
-    st.floored = (phase == 0 && !allzero && mn < st.logfloor) ? 1 : 0;   // needs the floored sums
+    st.floored = (first && !allzero && mn < st.logfloor) ? 1 : 0;   // needs the floored sums
     out[item] = st;
+    if (st.floored) ticket[item] = 0;
   }
 }
 
-// floored tile sums of the flagged items: grid (items, FS_SPLIT); un-flagged items leave after
-// one load, a flagged item's tiles are dealt round-robin to its FS_SPLIT CTAs
+__global__ void __launch_bounds__(256) afp_stats_kernel(const ItemDesc* items, int item0, int nitems,
+                                                        const double* tile_stats, ItemStats* out, int* ticket) {
+  const int w = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (w >= nitems) return;
+  reduce_item(items, item0 + w, tile_stats, out, true, threadIdx.x & 31, ticket);
+}
+
+// floored tile sums of the flagged items: grid (items, FS_SPLIT) of AFP_NBINS threads; un-flagged items
+// leave after one load, a flagged item's tiles are dealt round-robin to its FS_SPLIT CTAs
 constexpr int FS_SPLIT = 8;
 template <typename R>
-__global__ void __launch_bounds__(256) afp_floorsum_kernel(const ItemDesc* items, int item0, const ItemStats* stats,
-                                                           const R* logs, const double* nyq,
-                                                           double* tile_stats) {
-  __shared__ double s_part[8];
+__global__ void __launch_bounds__(AFP_NBINS) afp_floorsum_kernel(const ItemDesc* items, int item0, ItemStats* stats,
+                                                                 const R* logs, const double* nyq, double* tile_stats,
+                                                                 int* ticket) {
+  __shared__ double s_part[AFP_NBINS / 32];
+  __shared__ bool s_last;
   const int item = item0 + blockIdx.x;
   const ItemStats st = stats[item];
   if (!st.floored) return;                        // uniform
   const ItemDesc it = items[item];
   const int ntiles = (it.nframes + FT - 1) / FT;
+  if ((int)blockIdx.y >= ntiles) return;
   for (int k = blockIdx.y; k < ntiles; k += FS_SPLIT) {
     const int t0 = k * FT, nft = min(FT, it.nframes - t0);
-    const R* L = logs + (size_t)(it.frame_base + t0) * AFP_NBINS;
+    const R* L = logs + (size_t)(it.frame_base + t0) * AFP_NBINS + threadIdx.x;
+    R x[FT];                                      // bin threadIdx.x of the tile's frames: loads first,
+#pragma unroll                                    // then the sum in frame order
+    for (int r = 0; r < FT; ++r) x[r] = r < nft ? L[(size_t)r * AFP_NBINS] : R(0);
     double acc = 0.0;
-    for (int i = threadIdx.x; i < nft * AFP_NBINS; i += 256) acc += fmax((double)L[i], st.logfloor);
+#pragma unroll
+    for (int r = 0; r < FT; ++r)
+      if (r < nft) acc += fmax((double)x[r], st.logfloor);
     if ((int)threadIdx.x < nft) acc += fmax(nyq[it.frame_base + t0 + threadIdx.x], st.logfloor);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
@@ -516,9 +525,18 @@ __global__ void __launch_bounds__(256) afp_floorsum_kernel(const ItemDesc* items
     __syncthreads();
     if (threadIdx.x == 0) {
       double t = 0.0;
-      for (int w = 0; w < 8; ++w) t += s_part[w];
+      for (int w = 0; w < AFP_NBINS / 32; ++w) t += s_part[w];
       tile_stats[(size_t)(it.tile_base + k) * 3 + 2] = t;
     }
+  }
+  if (threadIdx.x == 0) {   // the last of the item's min(FS_SPLIT, ntiles) CTAs sees every floored sum
+    __threadfence();
+    s_last = atomicAdd(&ticket[item], 1) == min(FS_SPLIT, ntiles) - 1;
+  }
+  __syncthreads();
+  if (s_last && threadIdx.x < 32) {
+    __threadfence();
+    reduce_item(items, item, tile_stats, stats, false, threadIdx.x, nullptr);
   }
 }
 
@@ -545,11 +563,11 @@ __global__ void afp_sgram_kernel(const ItemDesc* items, const ItemStats* stats, 
 }  // namespace
 
 int afp_launch_tile_table(afp_ctx* c) {
-  if (c->nitems == 0) return AFP_OK;
-  afp_tile_table_kernel<<<(c->nitems + 255) / 256, 256, 0, c->stream>>>(c->d_items.as<ItemDesc>(), c->nitems,
-                                                                       c->d_tile_item.as<int32_t>());
+  if (c->nitems == 0 || c->tile_tag.is(c->d_tile_item)) return AFP_OK;   // already built for these items
+  afp_tile_table_kernel<<<c->nitems, 128, 0, c->stream>>>(c->d_items.as<ItemDesc>(), c->d_tile_item.as<int32_t>());
   AFP_CUDA(c, cudaGetLastError());
   c->launches++;
+  c->tile_tag.set(c->d_tile_item);
   return AFP_OK;
 }
 
@@ -613,18 +631,18 @@ int afp_launch_stats(afp_ctx* c, int item0, int nitems) {
   const ItemDesc* items = c->d_items.as<ItemDesc>();
   ItemStats* st = c->d_item_stats.as<ItemStats>();
   double* ts = c->d_tile_stats.as<double>();
-  afp_stats_kernel<<<(nitems + 7) / 8, 256, 0, c->stream>>>(items, item0, nitems, ts, st, 0);
+  int* ticket = c->d_stats_ticket.as<int>();
+  afp_stats_kernel<<<(nitems + 7) / 8, 256, 0, c->stream>>>(items, item0, nitems, ts, st, ticket);
   AFP_CUDA(c, cudaGetLastError());
+  const dim3 grid((unsigned)nitems, FS_SPLIT);
   if (c->ap.spectrogram_fp32)
-    afp_floorsum_kernel<float><<<dim3((unsigned)nitems, FS_SPLIT), 256, 0, c->stream>>>(
-        items, item0, st, c->d_logs.as<float>(), c->d_nyq.as<double>(), ts);
+    afp_floorsum_kernel<float><<<grid, AFP_NBINS, 0, c->stream>>>(items, item0, st, c->d_logs.as<float>(),
+                                                                  c->d_nyq.as<double>(), ts, ticket);
   else
-    afp_floorsum_kernel<double><<<dim3((unsigned)nitems, FS_SPLIT), 256, 0, c->stream>>>(
-        items, item0, st, c->d_logs.as<double>(), c->d_nyq.as<double>(), ts);
+    afp_floorsum_kernel<double><<<grid, AFP_NBINS, 0, c->stream>>>(items, item0, st, c->d_logs.as<double>(),
+                                                                   c->d_nyq.as<double>(), ts, ticket);
   AFP_CUDA(c, cudaGetLastError());
-  afp_stats_kernel<<<(nitems + 7) / 8, 256, 0, c->stream>>>(items, item0, nitems, ts, st, 1);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches += 3;
+  c->launches += 2;
   return AFP_OK;
 }
 
