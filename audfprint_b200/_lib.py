@@ -2,6 +2,7 @@
 the library is missing or no CUDA device is present every call fails loudly."""
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import os
 import re
@@ -44,6 +45,7 @@ _SIGS = {
     "afp_destroy": (None, [_P]),
     "afp_last_error": (C.c_char_p, [_P]),
     "afp_set_stream": (C.c_int, [_P, _P]),
+    "afp_get_stream": (C.c_int, [_P, C.POINTER(_P)]),
     "afp_sync": (C.c_int, [_P]),
     "afp_launch_count": (C.c_int64, [_P]),
     "afp_set_profiling": (C.c_int, [_P, C.c_int]),
@@ -173,6 +175,9 @@ class Context:
         self.analyzer_key = None
         self.table_key = None
         self.table_owner = None      # weakref to the HashTable whose device copy is newer than its host arrays
+        self._ext = None             # torch.cuda.ExternalStream of the context's stream (after_torch)
+        self._ready = self._done = None     # after_torch's events: torch's stream ready / calls passed
+        self._held = []              # tensors after_torch keeps alive until _done completes
 
     def check(self, rc):
         if rc != 0:
@@ -187,10 +192,61 @@ class Context:
             raise AfpError("libafp status %d: %s" % (rc, msg))
 
     def set_stream(self, cuda_stream: int | None):
+        """Run the context's calls on `cuda_stream` (a cudaStream_t handle; None or 0: the library's
+        own stream).  Returns once the work queued on the outgoing stream has finished."""
         self.check(self.lib.afp_set_stream(self.h, _P(cuda_stream) if cuda_stream else None))
+        self._release_finished()
+
+    def stream(self) -> int:
+        """The cudaStream_t handle the context's calls run on."""
+        s = _P()
+        self.check(self.lib.afp_get_stream(self.h, C.byref(s)))
+        return s.value or 0
 
     def sync(self):
         self.check(self.lib.afp_sync(self.h))
+        self._release_finished()
+
+    @contextlib.contextmanager
+    def after_torch(self, *tensors):
+        """Order the library calls made inside the block after torch's work on the torch tensors among
+        `tensors` (the tensors the calls read or write; other values are ignored):
+          - the context's stream first waits, on the device, for everything queued so far on torch's
+            current stream of this device (an event: the host does not wait);
+          - the tensors are then held until the context's stream has passed the calls, so that
+            torch's caching allocator cannot give their memory to new work while a call that returned
+            without synchronising (afp_fingerprint_batch with fetch=False) still reads it.
+        Nothing is done when no torch tensor is given, or when the context runs on torch's current
+        stream: stream order alone then orders both sides."""
+        tensors = [t for t in tensors if hasattr(t, "data_ptr") and not isinstance(t, np.ndarray)]
+        if not tensors:
+            yield
+            return
+        import torch
+        cur = torch.cuda.current_stream(self.device)
+        handle = self.stream()
+        if handle == cur.cuda_stream:
+            yield
+            return
+        if self._ext is None or self._ext.cuda_stream != handle:
+            self._ext = torch.cuda.ExternalStream(handle, device=torch.device("cuda", self.device))
+        if self._ready is None:
+            self._ready, self._done = torch.cuda.Event(), torch.cuda.Event()
+        self._release_finished()
+        self._ready.record(cur)
+        self._ext.wait_event(self._ready)
+        try:
+            yield
+        finally:
+            self._held.append(tensors)
+            self._done.record(self._ext)
+
+    def _release_finished(self):
+        """Drop the tensors held by after_torch once the context's stream has passed the last call
+        that held any (its event covers every earlier one: the holds of a stream that was switched
+        away from were synchronised by the switch)."""
+        if self._held and self._done.query():
+            self._held = []
 
     def set_profiling(self, on: bool):
         self.check(self.lib.afp_set_profiling(self.h, 1 if on else 0))

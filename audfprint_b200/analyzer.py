@@ -89,10 +89,11 @@ def pcm_frontend(raw, channels, src_rate, dst_rate=None, device=None, to_host=Tr
         import torch
         out = torch.empty(nout, dtype=torch.float32, device=torch.device("cuda", ctx.device))
         optr, on_host = out.data_ptr(), 0
-    ctx.check(ctx.lib.afp_pcm_frontend(ctx.h, raw.ctypes.data if nframes else None, 1, nframes, int(channels), up, down,
-                                       taps.ctypes.data if taps is not None else None,
-                                       len(taps) if taps is not None else 0, optr if nout else None, on_host,
-                                       C.byref(n)))
+    with ctx.after_torch(out):            # torch's pending reads of out's memory come first
+        ctx.check(ctx.lib.afp_pcm_frontend(ctx.h, raw.ctypes.data if nframes else None, 1, nframes, int(channels), up,
+                                           down, taps.ctypes.data if taps is not None else None,
+                                           len(taps) if taps is not None else 0, optr if nout else None, on_host,
+                                           C.byref(n)))
     return out
 
 
@@ -178,8 +179,8 @@ def pcm_frontend_batch(raws, channels, src_rates, dst_rate, device=None):
     ctx.check(ctx.lib.afp_pcm_frontend_batch(*args, None, 0, off.ctypes.data_as(P), lens.ctypes.data_as(P)))
     # 16 bytes of zeros past the last file, as Analyzer._pack leaves
     out = torch.zeros(int(off[-1]) + 4, dtype=torch.float32, device=torch.device("cuda", ctx.device))
-    torch.cuda.current_stream(out.device).synchronize()         # the zeros land before the library's stream writes
-    ctx.check(ctx.lib.afp_pcm_frontend_batch(*args, out.data_ptr(), out.numel(), None, None))
+    with ctx.after_torch(out):            # the zeros land before the library's stream writes
+        ctx.check(ctx.lib.afp_pcm_frontend_batch(*args, out.data_ptr(), out.numel(), None, None))
     return out, off, lens
 
 
@@ -389,15 +390,18 @@ class Analyzer(object):
         else:
             dtype = _lib.PCM_I16 if pcm.element_size() == 2 else _lib.PCM_F32
         total = C.c_int64(-1)
-        ctx.check(ctx.lib.afp_fingerprint_batch(ctx.h, ptr, dtype, on_host, nfiles,
-                                                off.ctypes.data_as(C.POINTER(C.c_int64)), lens_p,
-                                                C.byref(total) if fetch else None))
-        if not fetch:
-            return None, None
-        rows = host_rows if host_rows is not None else np.empty((max(int(total.value), 0), 2), np.int32)
-        roff = np.empty(nfiles + 1, np.int64)
-        rptr, r_on_host = _lib.ptr_of(rows)
-        ctx.check(ctx.lib.afp_fetch_hashes(ctx.h, rptr, r_on_host, roff.ctypes.data_as(C.POINTER(C.c_int64))))
+        # torch tensors: written on torch's stream, read (and host_rows written) on the context's; with
+        # fetch=False the call returns while the device still reads pcm, which after_torch keeps alive
+        with ctx.after_torch(pcm, host_rows):
+            ctx.check(ctx.lib.afp_fingerprint_batch(ctx.h, ptr, dtype, on_host, nfiles,
+                                                    off.ctypes.data_as(C.POINTER(C.c_int64)), lens_p,
+                                                    C.byref(total) if fetch else None))
+            if not fetch:
+                return None, None
+            rows = host_rows if host_rows is not None else np.empty((max(int(total.value), 0), 2), np.int32)
+            roff = np.empty(nfiles + 1, np.int64)
+            rptr, r_on_host = _lib.ptr_of(rows)
+            ctx.check(ctx.lib.afp_fetch_hashes(ctx.h, rptr, r_on_host, roff.ctypes.data_as(C.POINTER(C.c_int64))))
         if host_rows is not None:
             rows = rows[:int(total.value)]
         return rows, roff
@@ -773,9 +777,8 @@ class Analyzer(object):
         if rows_on_device:
             import torch
             rows = torch.empty((max(total, 1), 2), dtype=torch.int32, device=torch.device("cuda", ctx.device))
-            # the library writes `rows` on its own stream: torch's earlier work on this memory is done first
-            torch.cuda.current_stream(rows.device).synchronize()
-            ctx.check(ctx.lib.afp_fetch_hashes(ctx.h, C.c_void_p(rows.data_ptr()), 0, None))
+            with ctx.after_torch(rows):   # torch's pending reads of rows' memory come first
+                ctx.check(ctx.lib.afp_fetch_hashes(ctx.h, C.c_void_p(rows.data_ptr()), 0, None))
             ends = np.maximum(roff[1:] - 1, 0)
             last = rows[torch.from_numpy(ends).to(rows.device), 0].cpu().numpy() if total else np.zeros(len(idx), np.int32)
         else:

@@ -101,10 +101,11 @@ const char* afp_last_error(afp_ctx* c) { return c ? c->err.c_str() : "null conte
 int afp_set_stream(afp_ctx* c, void* s) {
   if (!c) return AFP_ERR_INVALID;
   AFP_CUDA(c, cudaSetDevice(c->device));
-  if (c->own_stream && c->stream) {
-    cudaStreamSynchronize(c->stream);
-    cudaStreamDestroy(c->stream);
-  }
+  // work queued on the outgoing stream uses the workspace the next call reuses, whoever owns that
+  // stream: it finishes before the switch
+  if (c->stream) AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+  if (c->own_stream && c->stream) cudaStreamDestroy(c->stream);
+  c->stream = nullptr;
   if (s) {
     c->stream = static_cast<cudaStream_t>(s);
     c->own_stream = false;
@@ -112,6 +113,12 @@ int afp_set_stream(afp_ctx* c, void* s) {
     AFP_CUDA(c, cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
     c->own_stream = true;
   }
+  return AFP_OK;
+}
+
+int afp_get_stream(afp_ctx* c, void** s) {
+  if (!c || !s) return AFP_ERR_INVALID;
+  *s = static_cast<void*>(c->stream);
   return AFP_OK;
 }
 

@@ -400,18 +400,19 @@ def match_sharded_batch(matcher, ht, packed_queries, row_cap: int = 16, group=No
     else:
         qmax = torch.empty(max(nq, 1), dtype=torch.int32, device=dev)      # written by the ranking call
         matcher._run(ctx, p, qrows, nq, qoff, (matcher.exact_count, matcher.find_time_range, matcher.time_quantile),
-                     shard_qmax=qmax.data_ptr())
+                     shard_qmax=qmax)
         if ws > 1:
             import torch.distributed as dist
             buf = qmax.to(_collective_device(group, ctx.device))         # in place under NCCL
             dist.all_reduce(buf, op=dist.ReduceOp.MAX, group=group)
             if buf is not qmax:
                 qmax.copy_(buf)
-            torch.cuda.current_stream(dev).synchronize()
-        ctx.check(ctx.lib.afp_match_options_shard_finish(ctx.h, C.c_void_p(qmax.data_ptr()), None))
+        with ctx.after_torch(qmax):
+            ctx.check(ctx.lib.afp_match_options_shard_finish(ctx.h, C.c_void_p(qmax.data_ptr()), None))
     mine = torch.empty((max(nq, 1), rb), dtype=torch.uint8, device=dev)
     try:
-        ctx.check(ctx.lib.afp_shard_pack(ctx.h, int(row_cap), mine.data_ptr()))
+        with ctx.after_torch(mine):               # torch's pending reads of its memory come first
+            ctx.check(ctx.lib.afp_shard_pack(ctx.h, int(row_cap), mine.data_ptr()))
     except _lib.AfpError as e:
         if "row capacity" in str(e):
             raise ValueError("a shard produced more than row_cap=%d rows for one query" % row_cap)
@@ -424,9 +425,9 @@ def match_sharded_batch(matcher, ht, packed_queries, row_cap: int = 16, group=No
         g = torch.empty((ws * mine.shape[0], rb), dtype=torch.uint8, device=cdev)
         dist.all_gather_into_tensor(g, mine.to(cdev), group=group)
         gathered = g.to(dev)
-        torch.cuda.current_stream(dev).synchronize()
     total = C.c_int64(0)
-    ctx.check(ctx.lib.afp_shard_merge(ctx.h, gathered.data_ptr(), ws, nq, sd, int(row_cap), C.byref(total)))
+    with ctx.after_torch(gathered):
+        ctx.check(ctx.lib.afp_shard_merge(ctx.h, gathered.data_ptr(), ws, nq, sd, int(row_cap), C.byref(total)))
     if not fetch:
         return None, None
     return matcher._fetch_rows(ctx, int(total.value), nq)

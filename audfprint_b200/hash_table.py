@@ -495,8 +495,8 @@ class HashTable(object):
         `for t in tables: self.merge(t)` does (`random` is not used).  An entry of the list is a
         HashTable or a DeviceTable snapshot (export_device) on this table's device.  Each incoming
         HashTable's host arrays are read first (a table whose device copy leads pulls it); a
-        snapshot's rows are read where they lie (afp_table_merge_device), after the current torch
-        stream of its device is synchronised.  The merges run on
+        snapshot's rows are read where they lie (afp_table_merge_device), after the work queued on
+        torch's current stream of its device (Context.after_torch).  The merges run on
         this table's device copy: buckets whose pool fits are appended in place, the overflowing
         ones are drawn by a C replay of np.random.permutation on the host, chunk by chunk while
         the device applies the previous chunk.  Afterwards the DEVICE copy is the current one (as
@@ -549,23 +549,23 @@ class HashTable(object):
         if not plan:
             return 0
         ctx = self._sync_device()
-        if any(table is None for _, table, _, _ in plan):
-            import torch
-            torch.cuda.current_stream(torch.device("cuda", ctx.device)).synchronize()
+        snaps = [x for t, table, _, _ in plan if table is None for x in (t.table, t.counts)]
         st = np.random.get_state()
         state = np.empty(625, np.uint32)
         state[:624], state[624] = st[1], st[2]
         novf, total = C.c_int64(0), 0
         try:
-            for t, table, counts, offset in plan:
-                if table is None:
-                    ctx.check(ctx.lib.afp_table_merge_device(ctx.h, t.table.data_ptr(), t.counts.data_ptr(),
-                                                             t.hashbits, t.depth, offset, state.ctypes.data,
-                                                             C.byref(novf), None))
-                else:
-                    ctx.check(ctx.lib.afp_table_merge(ctx.h, table.ctypes.data, counts.ctypes.data, int(t.hashbits),
-                                                      int(t.depth), offset, state.ctypes.data, C.byref(novf), None))
-                total += int(novf.value)
+            with ctx.after_torch(*snaps):         # the snapshots' rows as torch's stream last wrote them
+                for t, table, counts, offset in plan:
+                    if table is None:
+                        ctx.check(ctx.lib.afp_table_merge_device(ctx.h, t.table.data_ptr(), t.counts.data_ptr(),
+                                                                 t.hashbits, t.depth, offset, state.ctypes.data,
+                                                                 C.byref(novf), None))
+                    else:
+                        ctx.check(ctx.lib.afp_table_merge(ctx.h, table.ctypes.data, counts.ctypes.data,
+                                                          int(t.hashbits), int(t.depth), offset, state.ctypes.data,
+                                                          C.byref(novf), None))
+                    total += int(novf.value)
             hpi = np.concatenate([self.hashesperid] + [np.asarray(t.hashesperid) for t, _, _, _ in plan]).astype(np.uint32)
             ctx.check(ctx.lib.afp_table_set_hashesperid(ctx.h, hpi.ctypes.data if len(hpi) else None, len(hpi)))
         except BaseException:
@@ -606,7 +606,8 @@ class HashTable(object):
         nb = 1 << int(self.hashbits)
         table = torch.empty((nb, int(self.depth)), dtype=torch.int32, device=dev)
         counts = torch.empty(nb, dtype=torch.int32, device=dev)
-        ctx.check(ctx.lib.afp_table_export(ctx.h, table.data_ptr(), counts.data_ptr()))
+        with ctx.after_torch(table, counts):      # torch's pending reads of their memory come first
+            ctx.check(ctx.lib.afp_table_export(ctx.h, table.data_ptr(), counts.data_ptr()))
         return DeviceTable(table, counts, self.names, self.hashesperid, self.hashbits, self.depth, self.maxtimebits)
 
     def _install_device(self, snap):
@@ -622,10 +623,10 @@ class HashTable(object):
         dev = torch.device("cuda", ctx.device)
         hpi = np.ascontiguousarray(snap.hashesperid, dtype=np.uint32)
         hpi_dev = torch.from_numpy(hpi.view(np.int32)).to(dev) if len(hpi) else None
-        torch.cuda.current_stream(dev).synchronize()
-        ctx.check(ctx.lib.afp_table_upload(ctx.h, snap.table.data_ptr(), snap.counts.data_ptr(), snap.hashbits,
-                                           snap.depth, snap.maxtimebits,
-                                           hpi_dev.data_ptr() if hpi_dev is not None else None, len(hpi), 0))
+        with ctx.after_torch(snap.table, snap.counts, hpi_dev):
+            ctx.check(ctx.lib.afp_table_upload(ctx.h, snap.table.data_ptr(), snap.counts.data_ptr(), snap.hashbits,
+                                               snap.depth, snap.maxtimebits,
+                                               hpi_dev.data_ptr() if hpi_dev is not None else None, len(hpi), 0))
         self.hashbits, self.depth, self.maxtimebits = snap.hashbits, snap.depth, snap.maxtimebits
         self.__dict__["_table"] = self.__dict__["_counts"] = None     # pulled from the device when read
         self.names = list(snap.names)

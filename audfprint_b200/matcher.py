@@ -75,13 +75,20 @@ class Matcher(object):
     def _run(ctx, p, packed, nq, qoff, options=None, shard_qmax=None):
         """afp_match_batch - or afp_match_options_batch with options = (exact_count,
         find_time_range, time_quantile) - growing the per-query row capacity of the approximate
-        rows when a query overflows it.  With shard_qmax (the address of a device int32
-        [nq]) the options call is afp_match_options_shard_rank instead: the ranking of one shard,
+        rows when a query overflows it.  With shard_qmax (a device int32 [nq] tensor, or its
+        address) the options call is afp_match_options_shard_rank instead: the ranking of one shard,
         whose finish waits for the all-reduce of shard_qmax."""
+        with ctx.after_torch(packed, shard_qmax):          # torch tensors: written / read on torch's stream
+            return Matcher._run_ordered(ctx, p, packed, nq, qoff, options, shard_qmax)
+
+    @staticmethod
+    def _run_ordered(ctx, p, packed, nq, qoff, options, shard_qmax):
         total = C.c_int64(0)
         cap = 256
         ptr, on_host = _lib.ptr_of(packed) if len(packed) else (None, 1)     # NumPy (host) or torch CUDA tensor
         qp = qoff.ctypes.data_as(C.POINTER(C.c_int64))
+        if hasattr(shard_qmax, "data_ptr"):
+            shard_qmax = shard_qmax.data_ptr()
         if options is not None:
             breaks = timebits_breaks()
         while True:
@@ -439,7 +446,8 @@ class Matcher(object):
         float64 records (nq, W) that dist.allgather exchanges — no per-query Python work."""
         from . import dist as afd
         qrows, qoff = packed_queries
-        qrows = np.ascontiguousarray(qrows, dtype=np.int32).reshape(-1, 2)
+        if not getattr(qrows, "is_cuda", False):        # a torch CUDA tensor (int32 [R][2]) is used in place
+            qrows = np.ascontiguousarray(qrows, dtype=np.int32).reshape(-1, 2)
         qoff = np.ascontiguousarray(qoff, dtype=np.int64)
         rows, roff, cand, cnts = self._publish_call(ht, qrows, qoff)
         return afd.pack_shard_batch(cand, cnts, rows, roff, row_cap)
@@ -526,11 +534,8 @@ class Matcher(object):
         qoff = np.zeros(len(parts) + 1, np.int64)
         qoff[1:] = np.cumsum([len(p) for p in parts])
         packed = torch.cat([p.to(dev) for p in parts]) if qoff[-1] else torch.zeros((0, 2), dtype=torch.int32, device=dev)
-        packed = packed.contiguous()
-        # the library reads `packed` in place on its own (non-blocking) stream: the copies and the
-        # concatenation on torch's stream must be done first
-        torch.cuda.current_stream(dev).synchronize()
-        return packed, qoff
+        # match_batch orders its read of `packed` after the copies and the concatenation on torch's stream
+        return packed.contiguous(), qoff
 
     def file_match_to_msgs(self, analyzer, ht, qry, number=None):
         """Match one file and format the reference's report lines

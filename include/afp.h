@@ -19,6 +19,14 @@
  *   - buffers are caller-owned; the context owns only its internal workspace.
  *   - one context per process per GPU; calls are asynchronous on the context's
  *     stream except where a result count must be returned to the host.
+ *   - stream order is the caller's to keep at the boundary.  A device buffer a
+ *     call reads must be complete with respect to the context's stream: if other
+ *     streams wrote it, make the context's stream wait for them (e.g. an event)
+ *     before the call.  A device buffer a call writes must no longer be in use
+ *     by work on other streams.  A buffer (device or pinned host) read by a call
+ *     that returns without synchronising (afp_fingerprint_batch with
+ *     total_hashes = NULL) must stay unchanged and allocated until the next call
+ *     that synchronises the context's stream (afp_sync, any fetch).
  *   - there is no CPU fallback: every call needs a CUDA device.
  */
 #ifndef AFP_H_
@@ -94,8 +102,12 @@ int afp_abi_version(void);
 int afp_create(afp_ctx** out, int device);
 void afp_destroy(afp_ctx* ctx);
 const char* afp_last_error(afp_ctx* ctx);
-/* Use the caller's CUDA stream (cudaStream_t as void*); NULL = library-owned. */
+/* Use the caller's CUDA stream (cudaStream_t as void*); NULL = library-owned.  Waits for the work
+ * queued on the outgoing stream (the caller's or the library's) first, so that no call on the new
+ * stream overtakes it in the shared workspace; the outgoing stream must still exist. */
 int afp_set_stream(afp_ctx* ctx, void* cuda_stream);
+/* The stream the context's calls run on: the caller's (afp_set_stream) or the library-owned one. */
+int afp_get_stream(afp_ctx* ctx, void** cuda_stream);
 int afp_sync(afp_ctx* ctx);
 /* Number of kernel launches issued by this context so far (bench accounting). */
 int64_t afp_launch_count(afp_ctx* ctx);

@@ -27,6 +27,7 @@ def test_library_exports_every_declared_symbol():
     assert len(syms) >= 20
     for s in syms:
         assert hasattr(lib, s), s
+    assert "afp_get_stream" in syms and "afp_set_stream" in syms
     assert lib.afp_abi_version() == 2
 
 
