@@ -37,6 +37,11 @@ class MatcherParams(C.Structure):
                 ("row_capacity", C.c_int32), ("force_general", C.c_int32)]
 
 
+class FlacStream(C.Structure):
+    _fields_ = [("byte_offset", C.c_int64), ("nbytes", C.c_int64), ("sample_rate", C.c_int32),
+                ("channels", C.c_int32), ("bits_per_sample", C.c_int32), ("max_blocksize", C.c_int32)]
+
+
 _P = C.c_void_p
 _I64P = C.POINTER(C.c_int64)
 _SIGS = {
@@ -54,6 +59,8 @@ _SIGS = {
                                    C.c_int, _I64P]),
     "afp_pcm_frontend_batch": (C.c_int, [_P, _P, C.c_int, C.c_int64, C.c_int32, _I64P, _I64P, _P, _P, _P, C.c_int32,
                                          _P, _I64P, _P, _P, C.c_int64, _I64P, _I64P]),
+    "afp_flac_locate_batch": (C.c_int, [_P, _P, C.c_int, C.c_int64, C.c_int32, C.POINTER(FlacStream), _I64P, _P]),
+    "afp_flac_decode_batch": (C.c_int, [_P, _P, C.c_int64, _I64P, _P]),
     "afp_set_analyzer": (C.c_int, [_P, C.POINTER(AnalyzerParams), _P, _P, C.c_double]),
     "afp_fingerprint_batch": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int32, _I64P, _I64P, _I64P]),
     "afp_fetch_hashes": (C.c_int, [_P, _P, C.c_int, _I64P]),

@@ -19,7 +19,7 @@ import wave
 
 import numpy as np
 
-from . import _lib
+from . import _lib, flac
 
 # Special extensions of precomputed files (audfprint_analyze.py:29-32)
 PRECOMPEXT = '.afpt'
@@ -108,14 +108,31 @@ def _wav_read_raw(filename):
     return raw, nch, fs
 
 
+def _audio_read_raw(filename):
+    """The host half of the default reader, by content rather than extension: a native FLAC stream
+    (after optional ID3v2 tags) -> (flac.FlacStream, channels, rate); anything else goes to
+    _wav_read_raw, which reads a RIFF WAV or raises what it raises for other files."""
+    with open(filename, 'rb') as f:
+        head = f.read(10)
+        if head[:3] == b'ID3' or head[:4] == flac.MAGIC:
+            data = head + f.read()
+            if flac.is_flac(data):
+                stream = flac.parse(data)
+                return stream, stream.channels, stream.sample_rate
+    return _wav_read_raw(filename)
+
+
 def _wav_reader(filename, sr=None, channels=None, device=None):
-    """PCM-WAV reader standing in for audio_read.audio_read (audio_read.py:56-68; ffmpeg decoding
-    is out of scope, SURVEY §2 #9).  Returns (float32 samples in [-1,1), sr) like the reference
-    reader does (audio_read.py:139-145).  The file is parsed on the host; the arithmetic the
-    reference hands to ffmpeg - down-mix to mono, resampling to `sr` - runs on the device
-    (afp_pcm_frontend, SURVEY.md 8f-2).  No two resamplers agree bit for bit, so parity statements
-    in this repo are made on 11025 Hz PCM."""
-    raw, nch, fs = _wav_read_raw(filename)
+    """PCM-WAV and FLAC reader standing in for audio_read.audio_read (audio_read.py:56-68; ffmpeg
+    decoding of other formats is out of scope, SURVEY §2 #9).  Returns (float32 samples in [-1,1), sr)
+    like the reference reader does (audio_read.py:139-145).  A WAV is parsed on the host; a FLAC file's
+    frames are decoded on the device (flac.decode) to the int16 samples ffmpeg's decoder gives.  The
+    arithmetic the reference hands to ffmpeg - down-mix to mono, resampling to `sr` - runs on the
+    device (afp_pcm_frontend, SURVEY.md 8f-2).  No two resamplers agree bit for bit, so parity
+    statements in this repo are made on 11025 Hz PCM."""
+    raw, nch, fs = _audio_read_raw(filename)
+    if isinstance(raw, flac.FlacStream):
+        raw = flac.decode(raw, device)
     if nch == 1 and (sr is None or fs == sr):
         # nothing to do but the reader's own scaling (exact in float32)
         return raw.astype(np.float32) * np.float32(1.0 / 32768.0), fs
@@ -154,34 +171,83 @@ def pcm_frontend_batch(raws, channels, src_rates, dst_rate, device=None):
     Returns (out torch CUDA float32, offsets int64 [n+1], lengths int64 [n]): file i is
     out[offsets[i]:offsets[i] + lengths[i]], starting on a 16-byte boundary - the layout
     Analyzer.fingerprint_packed(out, offsets, sample_lengths=lengths) takes as it is."""
+    raws = [np.ascontiguousarray(r, dtype=np.int16).reshape(-1) for r in raws]
+    inoff = np.zeros(len(raws) + 1, np.int64)
+    inoff[1:] = np.cumsum([len(r) for r in raws])
+    nfr = [len(r) // max(1, int(c)) for r, c in zip(raws, channels)]
+    packed = np.concatenate(raws) if raws else np.zeros(0, np.int16)
+    return _frontend_packed(_lib.context(device), packed, inoff, nfr, channels, src_rates, dst_rate)
+
+
+def _frontend_packed(ctx, pcm, inoff, nfr, channels, src_rates, dst_rate):
+    """afp_pcm_frontend_batch over files packed in `pcm`, a host int16 array or a device int16 tensor:
+    file i's nfr[i] frames of channels[i] channels start at pcm[inoff[i]].  -> (out, offsets, lengths)
+    as pcm_frontend_batch returns them."""
     import torch
     from math import gcd
-    n = len(raws)
-    raws = [np.ascontiguousarray(r, dtype=np.int16).reshape(-1) for r in raws]
+    n = len(nfr)
     ch = np.array([int(c) for c in channels], np.int32)
-    nfr = np.array([len(r) // max(1, int(c)) for r, c in zip(raws, ch)], np.int64)
+    nfr = np.ascontiguousarray(nfr, dtype=np.int64)
+    inoff = np.ascontiguousarray(inoff, dtype=np.int64)
     up, down = np.ones(n, np.int32), np.ones(n, np.int32)
     for i, fs in enumerate(src_rates):
         if dst_rate is not None and int(dst_rate) != int(fs):
             g = gcd(int(dst_rate), int(fs))
             up[i], down[i] = int(dst_rate) // g, int(fs) // g
     rates, toff, taps = taps_table(zip(up, down))
-    inoff = np.zeros(n + 1, np.int64)
-    inoff[1:] = np.cumsum([len(r) for r in raws])
-    packed = np.concatenate(raws) if n else np.zeros(0, np.int16)
-    ctx = _lib.context(device)
     off = np.zeros(n + 1, np.int64)
     lens = np.zeros(n, np.int64)
     P = C.POINTER(C.c_int64)
-    args = [ctx.h, packed.ctypes.data if len(packed) else None, 1, len(packed), n, inoff.ctypes.data_as(P),
+    ptr, on_host = _lib.ptr_of(pcm)
+    plen = len(pcm) if isinstance(pcm, np.ndarray) else pcm.numel()
+    args = [ctx.h, ptr if plen else None, on_host, plen, n, inoff.ctypes.data_as(P),
             nfr.ctypes.data_as(P), ch.ctypes.data, up.ctypes.data, down.ctypes.data, len(rates), rates.ctypes.data,
             toff.ctypes.data_as(P), taps.ctypes.data]
     ctx.check(ctx.lib.afp_pcm_frontend_batch(*args, None, 0, off.ctypes.data_as(P), lens.ctypes.data_as(P)))
     # 16 bytes of zeros past the last file, as Analyzer._pack leaves
     out = torch.zeros(int(off[-1]) + 4, dtype=torch.float32, device=torch.device("cuda", ctx.device))
-    with ctx.after_torch(out):            # the zeros land before the library's stream writes
+    with ctx.after_torch(out, pcm):       # the zeros (and a device pcm) land before the library's stream
         ctx.check(ctx.lib.afp_pcm_frontend_batch(*args, out.data_ptr(), out.numel(), None, None))
     return out, off, lens
+
+
+def _frontend_sources(sources, channels, src_rates, dst_rate, device=None):
+    """pcm_frontend_batch over files given as int16 PCM or as flac.FlacStream.  With FLAC files among
+    them, the round's int16 buffer is built on the device: the PCM files go up in one copy, the FLAC
+    files are located (one call) and decoded in place after them (one call), and one front-end call
+    runs over all.  -> (out, offsets, lengths, status int32 [n]): 0, or the AFP_FLAC_* code of a FLAC
+    file the device refused, which then has no samples."""
+    import torch
+    n = len(sources)
+    status = np.zeros(n, np.int32)
+    fl = [k for k, s in enumerate(sources) if isinstance(s, flac.FlacStream)]
+    if not fl:
+        return pcm_frontend_batch(sources, channels, src_rates, dst_rate, device=device) + (status,)
+    ctx = _lib.context(device)
+    nsamples, _ = flac.locate(ctx, [sources[k] for k in fl])
+    is_flac = set(fl)
+    raws = [np.ascontiguousarray(sources[k], dtype=np.int16).reshape(-1) for k in range(n) if k not in is_flac]
+    inoff, nfr = np.zeros(n, np.int64), np.zeros(n, np.int64)
+    pos, r = 0, iter(raws)
+    for k in range(n):
+        if k not in is_flac:
+            raw = next(r)
+            inoff[k], nfr[k] = pos, len(raw) // max(1, int(channels[k]))
+            pos += len(raw)
+    wav_len, fl_off = pos, []
+    for j, k in enumerate(fl):
+        inoff[k], nfr[k] = pos, nsamples[j]
+        fl_off.append(pos)
+        pos += int(nsamples[j]) * int(channels[k])
+    pcm = torch.empty(max(pos, 1), dtype=torch.int16, device=torch.device("cuda", ctx.device))
+    if wav_len:
+        pcm[:wav_len].copy_(torch.from_numpy(np.concatenate(raws)))
+    with ctx.after_torch(pcm):            # the PCM copy lands before the decode writes after it
+        fst = flac.decode_into(ctx, pcm, fl_off)
+    for j, k in enumerate(fl):
+        if fst[j]:
+            status[k], nfr[k] = fst[j], 0
+    return _frontend_packed(ctx, pcm, inoff, nfr, channels, src_rates, dst_rate) + (status,)
 
 
 class _ChunkPlanner(object):
@@ -611,7 +677,9 @@ class Analyzer(object):
 
         WAVs read by the default reader are parsed on the host (_wav_read_raw); the raw PCM of a
         chunk of files is staged once, down-mixed and resampled by ONE afp_pcm_frontend_batch call
-        into a device buffer, and fingerprinted there in place (fingerprint_packed).  A custom
+        into a device buffer, and fingerprinted there in place (fingerprint_packed).  FLAC files are
+        decoded on the device into the same staging buffer first (_frontend_sources); one the device
+        refuses is an unreadable file.  A custom
         `reader` is called per file and its output packed as it is.  Runs of .afpk files are loaded
         on the host and hashed by ONE afp_fingerprint_from_peaks call per chunk; .afpt files are
         loaded as they are.  Chunks follow max_frames_per_call and max_pcm_bytes_per_call (a file
@@ -645,13 +713,17 @@ class Analyzer(object):
                     for i, value, dur in items:
                         results[i], durs[i] = (empty() if value is None else value), dur
                     continue
+                refused = []
                 if kind == 'pcm':
-                    self._fingerprint_pcm(items, nsh, durs)
+                    refused = self._fingerprint_pcm(items, nsh, durs)
+                    self._refuse(filenames, items, refused)
                 else:
                     self._fingerprint_peaks([it[1] for it in items])
                     for i, _, dur in items:
                         durs[i] = dur
                 collect(kind, [it[0] for it in items], results)
+                for k, _ in refused:
+                    results[items[k][0]] = empty()      # what the per-file call gives an unreadable file
         for dur in durs:
             self._account(dur)
         self.last_batch_durations = durs
@@ -712,39 +784,61 @@ class Analyzer(object):
             return 'peaks', (i, rows, dur), max(1, int(rows[-1, 0]) + 1), rows.nbytes
         if self.reader is _wav_reader:
             try:
-                raw, nch, fs = _wav_read_raw(fn)
+                raw, nch, fs = _audio_read_raw(fn)
                 if fs < 1:
                     # the per-file reader fails here in the device front-end (down < 1)
                     raise ValueError("%s: sample rate %d" % (fn, fs))
+                nframes = len(raw) // nch if isinstance(raw, np.ndarray) else self._flac_frames(raw)
             except Exception as e:
                 self._read_failed(fn, e)
-                raw, nch, fs = np.zeros(0, np.int16), 1, self.target_sr
-            nout = -(-(len(raw) // nch) * self.target_sr // fs)      # ceil(nframes * up / down)
+                raw, nch, fs, nframes = np.zeros(0, np.int16), 1, self.target_sr, 0
+            nout = -(-nframes * self.target_sr // fs)      # ceil(nframes * up / down)
             if nout == 0:
                 return 'host', (i, None, 0.0), 0, 0
-            return 'pcm', (i, (raw, nch, fs), nout, None), nsh * (1 + nout // self.n_hop), raw.nbytes
+            nbytes = raw.nbytes if isinstance(raw, np.ndarray) else 2 * nframes * nch     # decoded int16
+            return 'pcm', (i, (raw, nch, fs), nout, None), nsh * (1 + nout // self.n_hop), nbytes
         d, sr = self._read(fn)
         if len(d) == 0:
             return 'host', (i, None, len(d) / sr), 0, 0
         a = _as_pcm(d)[0]
         return 'pcm', (i, a, len(d), len(d) / sr), nsh * (1 + len(d) // self.n_hop), a.nbytes
 
+    def _flac_frames(self, stream):
+        """Samples per channel of a FLAC file for the round planner: STREAMINFO's count, or when that
+        is 0 (unknown) the count the device finds by locating the file's frames.  Raises for a file
+        the device refuses."""
+        if stream.total_samples:
+            return stream.total_samples
+        nsamples, status = flac.locate(_lib.context(self.device), [stream])
+        if status[0]:
+            raise flac.failure(status[0])
+        return int(nsamples[0])
+
     def _fingerprint_pcm(self, items, shifts, durs):
         """Fingerprint one 'pcm' round in one device call at `shifts`; the results stay in the
-        workspace.  Each file's duration goes to durs[i]."""
+        workspace.  Each file's duration goes to durs[i].  Returns [(position in items, AFP_FLAC_*
+        code)] of the FLAC files the device refused; they are fingerprinted as files without samples,
+        and the caller reports them (_refuse)."""
         idx = [it[0] for it in items]
         if self.reader is _wav_reader:
             raws = [it[1] for it in items]
-            out, off, lens = pcm_frontend_batch([r[0] for r in raws], [r[1] for r in raws], [r[2] for r in raws],
-                                                self.target_sr, device=self.device)
+            out, off, lens, status = _frontend_sources([r[0] for r in raws], [r[1] for r in raws],
+                                                       [r[2] for r in raws], self.target_sr, device=self.device)
             for i, ln in zip(idx, lens):
                 durs[i] = int(ln) / self.target_sr
             self.fingerprint_packed(out, off, shifts, fetch=False, sample_lengths=lens)
-        else:
-            for it in items:
-                durs[it[0]] = it[3]
-            packed, starts, lens = self._pack([it[1] for it in items])
-            self.fingerprint_packed(packed, starts, shifts, fetch=False, sample_lengths=lens)
+            return [(k, int(c)) for k, c in enumerate(status) if c]
+        for it in items:
+            durs[it[0]] = it[3]
+        packed, starts, lens = self._pack([it[1] for it in items])
+        self.fingerprint_packed(packed, starts, shifts, fetch=False, sample_lengths=lens)
+        return []
+
+    def _refuse(self, filenames, items, refused):
+        """Report the files _fingerprint_pcm refused as unreadable, in list order: under fail_on_error
+        the first raises _read_failed's IOError."""
+        for k, code in refused:
+            self._read_failed(filenames[items[k][0]], flac.failure(code))
 
     def _fingerprint_peaks(self, arrays):
         """wavfile2hashes of many .afpk peak lists (int32 (n,2) each, n >= 1) in ONE
@@ -859,7 +953,15 @@ class Analyzer(object):
                     begin(idx, [[] if it[1] is None else it[1] for it in items])
                     continue
                 if kind == 'pcm':
-                    self._fingerprint_pcm(items, self.shifts, durs)
+                    refused = self._fingerprint_pcm(items, self.shifts, durs)
+                    if refused and self.fail_on_error:
+                        # the loop stores the files before the refused one; it is not counted
+                        k = refused[0][0]
+                        if k:
+                            self._fingerprint_pcm(items[:k], self.shifts, durs)
+                            begin(idx[:k], None)
+                        finish()
+                    self._refuse(filenames, items, refused)
                 else:
                     for i, _, dur in items:
                         durs[i] = dur

@@ -81,7 +81,8 @@ void afp_destroy(afp_ctx* c) {
                     &c->d_ed_rows, &c->d_lg_key, &c->d_lg_cub, &c->d_lg_id, &c->d_lg_w, &c->d_lg_cand,
                     &c->d_lg_dts, &c->d_lg_hist, &c->d_op_slot, &c->d_op_hit, &c->d_op_mode, &c->d_op_sup,
                     &c->d_op_key, &c->d_op_tq, &c->d_op_cub, &c->d_op_rows, &c->d_mg_in, &c->d_mg_flag,
-                    &c->d_mg_off, &c->d_mg_bkt, &c->d_mg_idx, &c->d_mg_row, &c->d_op_qfail};
+                    &c->d_mg_off, &c->d_mg_bkt, &c->d_mg_idx, &c->d_mg_row, &c->d_op_qfail,
+                    &c->d_fl_in, &c->d_fl_cand, &c->d_fl_file, &c->d_fl_res, &c->d_fl_frame, &c->d_fl_scratch};
   for (DevBuf* b : bufs) b->release();
   if (c->copy_stream) {
     cudaStreamDestroy(c->copy_stream);

@@ -193,6 +193,17 @@ struct afp_ctx {
     const int32_t* dq = nullptr;
   } sopt;
   DevBuf d_op_qfail;
+  // FLAC decoding (afp_flac.cu): staged compressed bytes, per-byte header candidates, file descriptors,
+  // per-file locate results, the frame tables and the int32 samples before decorrelation
+  DevBuf d_fl_in, d_fl_cand, d_fl_file, d_fl_res, d_fl_frame, d_fl_scratch;
+  struct {
+    bool valid = false;              // afp_flac_locate_batch ran and its batch has not been decoded over
+    int32_t nfiles = 0;
+    const uint8_t* bytes = nullptr;  // device bytes the frame table points into
+    std::vector<int64_t> nsamples;   // per file, per channel (0 for a failed file)
+    std::vector<int32_t> nframes, status;
+    std::vector<char> desc;          // the FlacFile descriptors of the batch
+  } fl;
 };
 
 #define AFP_CUDA(ctx, call)                                                        \

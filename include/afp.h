@@ -162,6 +162,72 @@ int afp_pcm_frontend_batch(afp_ctx* ctx, const int16_t* pcm, int pcm_on_host, in
                            const int64_t* tap_offsets, const double* taps, float* out, int64_t out_capacity,
                            int64_t* out_offsets, int64_t* out_lengths);
 
+/* ---- FLAC decoding -----------------------------------------------------------
+ * What the reference's `ffmpeg -i F -f s16le` does for a FLAC file, up to the int16 stream the PCM
+ * front-end takes: the frames of a list of FLAC streams are decoded on the device into interleaved
+ * int16, in the layout afp_pcm_frontend_batch takes as its device input.  Two calls:
+ *   afp_flac_locate_batch  finds every file's frames and returns its sample count (one synchronise);
+ *   afp_flac_decode_batch  decodes the located files into a caller-owned DEVICE buffer.
+ * The host parses the metadata blocks and passes, per file, the byte range of its frames (everything
+ * after the last metadata block) and the STREAMINFO fields below.
+ *
+ * Locate: every byte that starts a frame header (sync code, no reserved value, fields consistent with
+ * STREAMINFO, correct CRC-8) is a candidate.  From the first byte of the file, a frame ends at the next
+ * candidate whose frame number (fixed block size) or first-sample number (variable block size)
+ * follows on and where the CRC-16 over [frame start, candidate) is right; the last frame ends at the
+ * end of the file's bytes.  So a sync pattern inside compressed data never splits a frame.  STREAMINFO's
+ * total sample count is not used (it may be 0): the count is the sum of the frames' block sizes.
+ *
+ * Decode: CONSTANT, VERBATIM, FIXED (orders 0-4) and LPC (orders 1-32, int64 accumulation)
+ * subframes, wasted bits, Rice partitions with 4- and 5-bit parameters and escape partitions,
+ * independent, left/side, right/side and mid/side channels, block sizes 1-65535, fixed or variable;
+ * 4-24 bits per sample, 1-8 channels.  A b-bit sample x becomes the int16 FFmpeg's decoder and
+ * libswresample give: x << (16 - b) for b <= 16, x >> (b - 16) (arithmetic) above.
+ * The STREAMINFO MD5 signature is not checked (ffmpeg does not check it by default either).
+ *
+ * A file is refused, with its own code in file_status, for a depth outside 4-24 bits, a frame chain
+ * that does not follow on, a CRC-16 mismatch, a reserved code, a last frame cut short, or subframe data
+ * that does not fit its frame.  ffmpeg would conceal a bad frame and go on; here the whole file is
+ * refused.  A refused file gets no samples (count 0) and nothing is written for it; nothing outside a
+ * file's output range is written.  Both calls return AFP_OK when no file failed, else the code of the
+ * lowest failing file: AFP_ERR_UNSUPPORTED for a depth, AFP_ERR_INVALID for the others. */
+typedef struct {
+  int64_t byte_offset;      /* first byte of the file's frames in the packed bytes */
+  int64_t nbytes;           /* bytes of frames (to the end of the file) */
+  int32_t sample_rate;      /* STREAMINFO fields */
+  int32_t channels;         /* 1-8 */
+  int32_t bits_per_sample;  /* 4-24 decodable */
+  int32_t max_blocksize;    /* a frame header with a larger block size is not a candidate (if >= 16) */
+} afp_flac_stream;
+
+enum {
+  AFP_FLAC_OK = 0,
+  AFP_FLAC_DEPTH = 1,       /* bits per sample outside 4-24 (25-32 are not decoded) */
+  AFP_FLAC_CHAIN = 2,       /* no frame at the start, or a frame followed by one that does not follow on */
+  AFP_FLAC_CRC = 3,         /* a frame's CRC-16 does not match */
+  AFP_FLAC_RESERVED = 4,    /* a reserved code in a frame or subframe header */
+  AFP_FLAC_TRUNCATED = 5,   /* the last frame does not end in its CRC-16 (cut short, or damaged: no
+                             * later header tells the two apart) */
+  AFP_FLAC_CORRUPT = 6      /* subframe data that does not fit its frame (residual past the frame's
+                             * end, a partition order the block size cannot take, a negative LPC shift) */
+};
+
+/*   bytes         packed FLAC frame bytes of all files, HOST or DEVICE, nbytes_total of them.  A DEVICE
+ *                 buffer is read by both calls and must stay unchanged until afp_flac_decode_batch
+ *                 returns.
+ *   files         HOST [nfiles]
+ *   nsamples      HOST int64 [nfiles] or NULL: samples per channel of every file (0 when it fails)
+ *   file_status   HOST int32 [nfiles] or NULL: AFP_FLAC_* of every file */
+int afp_flac_locate_batch(afp_ctx* ctx, const uint8_t* bytes, int bytes_on_host, int64_t nbytes_total,
+                          int32_t nfiles, const afp_flac_stream* files, int64_t* nsamples, int32_t* file_status);
+/* Decode the files of the last afp_flac_locate_batch: file i's nsamples[i] * channels interleaved int16
+ * go to out_dev[out_offsets[i] ...] (HOST int64 [nfiles]); out_dev holds out_capacity int16.  Files that
+ * failed to locate are skipped.  file_status (HOST [nfiles] or NULL) receives the codes of both calls;
+ * a file that fails here may have had part of its own range written.  AFP_ERR_STATE without a located
+ * batch; every range is checked against out_capacity before anything is launched.  Synchronises. */
+int afp_flac_decode_batch(afp_ctx* ctx, int16_t* out_dev, int64_t out_capacity, const int64_t* out_offsets,
+                          int32_t* file_status);
+
 /* ---- Analyzer --------------------------------------------------------------
  * Replaces stft.stft (stft.py:62-94) + Analyzer.find_peaks
  * (audfprint_analyze.py:255-308) + peaks2landmarks (:310-343) +
