@@ -67,23 +67,6 @@ void afp_destroy(afp_ctx* c) {
   if (c->stream) cudaStreamSynchronize(c->stream);
   for (int i = 0; i <= AFP_NSTAGES; ++i)
     if (c->ev[i]) cudaEventDestroy(c->ev[i]);
-  DevBuf* bufs[] = {&c->d_window, &c->d_window_f, &c->d_twid_f, &c->d_gauss, &c->d_twid, &c->d_pcm_stage, &c->d_items, &c->d_tile_item, &c->d_file_col_base,
-                    &c->d_logs, &c->d_nyq, &c->d_tile_stats, &c->d_item_stats, &c->d_stats_ticket, &c->d_fwd_val, &c->d_fwd_bin,
-                    &c->d_fwd_cnt, &c->d_pk_bin, &c->d_pk_cnt, &c->d_item_scols, &c->d_item_npeaks, &c->d_lm,
-                    &c->d_col_cnt, &c->d_hash_stage, &c->d_file_tot, &c->d_file_off, &c->d_hashes, &c->d_pk_off, &c->d_pk_rows,
-                    &c->d_pk_in, &c->d_pk_inoff, &c->d_pk_status, &c->d_tmp, &c->tab.table, &c->tab.counts, &c->tab.hashesperid, &c->d_q, &c->d_qoff,
-                    &c->d_hit_off, &c->d_hits, &c->d_st_off, &c->d_st_ids, &c->d_st_eval, &c->d_st_seq, &c->d_st_ovf,
-                    &c->d_st_cnt, &c->d_st_seg, &c->d_st_heavy, &c->d_st_part, &c->d_st_scan, &c->d_st_obkt,
-                    &c->d_st_opos, &c->d_st_oval, &c->d_st_slot, &c->d_st_last, &c->d_mfast, &c->d_mqlist, &c->d_mscratch, &c->d_mrows, &c->d_mrow_cnt,
-                    &c->d_mrow_off, &c->d_mrows_packed, &c->d_mcand, &c->d_mcand_cnt,
-                    &c->d_ed_ids, &c->d_ed_bits, &c->d_ed_slot, &c->d_ed_cnt, &c->d_ed_off, &c->d_ed_key,
-                    &c->d_ed_key2, &c->d_ed_val, &c->d_ed_val2, &c->d_ed_cub, &c->d_ed_uoff, &c->d_ed_req,
-                    &c->d_ed_rows, &c->d_lg_key, &c->d_lg_cub, &c->d_lg_id, &c->d_lg_w, &c->d_lg_cand,
-                    &c->d_lg_dts, &c->d_lg_hist, &c->d_op_slot, &c->d_op_hit, &c->d_op_mode, &c->d_op_sup,
-                    &c->d_op_key, &c->d_op_tq, &c->d_op_cub, &c->d_op_rows, &c->d_mg_in, &c->d_mg_flag,
-                    &c->d_mg_off, &c->d_mg_bkt, &c->d_mg_idx, &c->d_mg_row, &c->d_op_qfail,
-                    &c->d_fl_in, &c->d_fl_cand, &c->d_fl_file, &c->d_fl_res, &c->d_fl_frame, &c->d_fl_scratch};
-  for (DevBuf* b : bufs) b->release();
   if (c->copy_stream) {
     cudaStreamDestroy(c->copy_stream);
     for (auto& e : c->ev_chunk) if (e) cudaEventDestroy(e);
@@ -397,9 +380,7 @@ int afp_fingerprint_batch(afp_ctx* c, const void* pcm, int pcm_dtype, int pcm_on
 #undef AFP_MARK
   c->batch_valid = true;
   if (total_hashes) {
-    AFP_CUDA(c, cudaMemcpyAsync(&c->total_hashes, c->d_file_off.as<int64_t>() + nfiles, sizeof(int64_t),
-                                cudaMemcpyDeviceToHost, c->stream));
-    AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+    if ((rc = afp_read_back(c, &c->total_hashes, c->d_file_off.as<int64_t>() + nfiles, 1))) return rc;
     *total_hashes = c->total_hashes;
   }
   return AFP_OK;
@@ -451,8 +432,8 @@ int afp_fingerprint_from_logs(afp_ctx* c, const void* logs, int logs_on_host, in
   // K2 bulk-copies its columns out of d_logs, as it does after K1
   const size_t esz = c->ap.spectrogram_fp32 ? sizeof(float) : sizeof(double);
   if (frames > 0)
-    AFP_CUDA(c, cudaMemcpyAsync(c->d_logs.p, logs, esz * AFP_NBINS * (size_t)frames,
-                                logs_on_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, c->stream));
+    AFP_CUDA(c, afp_copy_in(c, c->d_logs.as<char>(), static_cast<const char*>(logs), esz * AFP_NBINS * (size_t)frames,
+                            logs_on_host));
   if (c->nitems > 0)
     AFP_CUDA(c, cudaMemcpyAsync(c->d_item_stats.p, st.data(), sizeof(ItemStats) * st.size(), cudaMemcpyHostToDevice,
                                 c->stream));
@@ -462,9 +443,7 @@ int afp_fingerprint_from_logs(afp_ctx* c, const void* logs, int logs_on_host, in
   if ((rc = afp_write_hashes(c))) return rc;
   c->batch_valid = true;
   c->total_hashes = 0;
-  if (nfiles > 0)
-    AFP_CUDA(c, cudaMemcpyAsync(&c->total_hashes, c->d_file_off.as<int64_t>() + nfiles, sizeof(int64_t),
-                                cudaMemcpyDeviceToHost, c->stream));
+  if (nfiles > 0) AFP_CUDA(c, afp_read_async(c, &c->total_hashes, c->d_file_off.as<int64_t>() + nfiles, 1));
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));   // `st` and host logs must outlive their copies
   if (total_hashes) *total_hashes = c->total_hashes;
   return AFP_OK;
@@ -501,19 +480,15 @@ int afp_fingerprint_from_peaks(afp_ctx* c, const int32_t* peak_rows, int rows_on
                                 c->stream));
   const int32_t* drows = peak_rows;
   std::vector<int32_t> last((size_t)nfiles, -1);
+  int rc;
   if (staged) {
-    AFP_CUDA(c, c->d_pk_in.reserve(sizeof(int32_t) * 2 * (size_t)nrows));
-    AFP_CUDA(c, cudaMemcpyAsync(c->d_pk_in.p, peak_rows + 2 * row0, sizeof(int32_t) * 2 * (size_t)nrows,
-                                cudaMemcpyHostToDevice, c->stream));
-    drows = c->d_pk_in.as<int32_t>();
+    if ((rc = afp_stage(c, c->d_pk_in, peak_rows + 2 * row0, 2 * (size_t)nrows, 1, &drows))) return rc;
     for (int f = 0; f < nfiles; ++f)
       if (off[f + 1] > off[f]) last[(size_t)f] = peak_rows[2 * (off[f + 1] - 1)];
   } else if (nrows > 0) {
-    int rc = afp_launch_peak_last_cols(c, drows, c->d_pk_inoff.as<int64_t>(), nfiles, c->d_pk_status.as<int32_t>());
-    if (rc) return rc;
-    AFP_CUDA(c, cudaMemcpyAsync(last.data(), c->d_pk_status.p, sizeof(int32_t) * (size_t)nfiles,
-                                cudaMemcpyDeviceToHost, c->stream));
-    AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+    if ((rc = afp_launch_peak_last_cols(c, drows, c->d_pk_inoff.as<int64_t>(), nfiles, c->d_pk_status.as<int32_t>())) ||
+        (rc = afp_read_back(c, last.data(), c->d_pk_status.as<int32_t>(), (size_t)nfiles)))
+      return rc;
   }
   // one item of T_f = last column + 1 columns per file (:321); shift items 1..S-1 are empty.  A last
   // column outside [0, 2^28] gives T_f = 0, so that every row of the file fails the scatter's bounds.
@@ -568,19 +543,15 @@ int afp_fingerprint_from_peaks(afp_ctx* c, const int32_t* peak_rows, int rows_on
   AFP_CUDA(c, cudaMemsetAsync(c->d_pk_status.p, 0, sizeof(int32_t) * (size_t)(nfiles + 1), c->stream));
   if (nfiles == 0) AFP_CUDA(c, cudaMemsetAsync(c->d_file_off.p, 0, sizeof(int64_t), c->stream));
   // the scatter never writes pk_cnt above maxpks, so K3 runs safely before the status is read: one sync
-  int rc = afp_launch_scatter_peaks(c, drows, c->d_pk_inoff.as<int64_t>(), nrows, nfiles, S,
-                                    c->d_pk_status.as<int32_t>());
+  rc = afp_launch_scatter_peaks(c, drows, c->d_pk_inoff.as<int64_t>(), nrows, nfiles, S, c->d_pk_status.as<int32_t>());
   if (!rc) rc = afp_launch_file_hashes(c, 0, nfiles);
   if (!rc) rc = afp_launch_hashes(c);
   if (rc) return rc;
   std::vector<int32_t> st((size_t)nfiles + 1, 0);
   int64_t total = 0;
-  if (nfiles > 0) {
-    AFP_CUDA(c, cudaMemcpyAsync(st.data(), c->d_pk_status.p, sizeof(int32_t) * (size_t)nfiles, cudaMemcpyDeviceToHost,
-                                c->stream));
-    AFP_CUDA(c, cudaMemcpyAsync(&total, c->d_file_off.as<int64_t>() + nfiles, sizeof(int64_t), cudaMemcpyDeviceToHost,
-                                c->stream));
-  }
+  if (nfiles > 0)
+    AFP_CUDA(c, afp_read_async(c, st.data(), c->d_pk_status.as<int32_t>(), (size_t)nfiles, &total,
+                               c->d_file_off.as<int64_t>() + nfiles, 1));
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));   // also: the host vectors above outlive their copies
   int first = -1;
   for (int f = 0; f < nfiles; ++f) {
@@ -607,17 +578,13 @@ int afp_fetch_hashes(afp_ctx* c, int32_t* rows, int rows_on_host, int64_t* row_o
   if (!c) return AFP_ERR_INVALID;
   if (!c->batch_valid) AFP_FAIL(c, AFP_ERR_STATE, "no fingerprint batch to fetch");
   AFP_CUDA(c, cudaSetDevice(c->device));
-  if (c->total_hashes < 0) {
-    AFP_CUDA(c, cudaMemcpyAsync(&c->total_hashes, c->d_file_off.as<int64_t>() + c->nfiles, sizeof(int64_t),
-                                cudaMemcpyDeviceToHost, c->stream));
-    AFP_CUDA(c, cudaStreamSynchronize(c->stream));
-  }
-  if (row_offsets)
-    AFP_CUDA(c, cudaMemcpyAsync(row_offsets, c->d_file_off.p, sizeof(int64_t) * (size_t)(c->nfiles + 1),
-                                cudaMemcpyDeviceToHost, c->stream));
+  int rc;
+  if (c->total_hashes < 0 &&
+      (rc = afp_read_back(c, &c->total_hashes, c->d_file_off.as<int64_t>() + c->nfiles, 1)))
+    return rc;
+  if (row_offsets) AFP_CUDA(c, afp_copy_out(c, row_offsets, c->d_file_off.as<int64_t>(), (size_t)(c->nfiles + 1), 1));
   if (rows && c->total_hashes > 0)
-    AFP_CUDA(c, cudaMemcpyAsync(rows, c->d_hashes.p, sizeof(int32_t) * 2 * (size_t)c->total_hashes,
-                                rows_on_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, c->stream));
+    AFP_CUDA(c, afp_copy_out(c, rows, c->d_hashes.as<int32_t>(), 2 * (size_t)c->total_hashes, rows_on_host));
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));
   return AFP_OK;
 }
@@ -630,13 +597,10 @@ int afp_fetch_peaks(afp_ctx* c, int32_t shift, int32_t* rows, int rows_on_host, 
   int rc = afp_compact_peaks(c, shift);
   if (rc) return rc;
   std::vector<int64_t> off((size_t)c->nfiles + 1);
-  AFP_CUDA(c, cudaMemcpyAsync(off.data(), c->d_pk_off.p, sizeof(int64_t) * off.size(), cudaMemcpyDeviceToHost,
-                              c->stream));
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+  if ((rc = afp_read_back(c, off.data(), c->d_pk_off.as<int64_t>(), off.size()))) return rc;
   if (row_offsets) memcpy(row_offsets, off.data(), sizeof(int64_t) * off.size());
   if (rows && off[c->nfiles] > 0)
-    AFP_CUDA(c, cudaMemcpyAsync(rows, c->d_pk_rows.p, sizeof(int32_t) * 2 * (size_t)off[c->nfiles],
-                                rows_on_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, c->stream));
+    AFP_CUDA(c, afp_copy_out(c, rows, c->d_pk_rows.as<int32_t>(), 2 * (size_t)off[c->nfiles], rows_on_host));
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));
   return AFP_OK;
 }
@@ -654,8 +618,7 @@ int afp_fetch_landmarks(afp_ctx* c, int32_t* rows, int rows_on_host) {
   if (c->nlandmarks < 0) AFP_FAIL(c, AFP_ERR_STATE, "afp_landmarks_from_peaks has not been called");
   AFP_CUDA(c, cudaSetDevice(c->device));
   if (rows && c->nlandmarks > 0)
-    AFP_CUDA(c, cudaMemcpyAsync(rows, c->d_hashes.p, sizeof(int32_t) * 4 * (size_t)c->nlandmarks,
-                                rows_on_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, c->stream));
+    AFP_CUDA(c, afp_copy_out(c, rows, c->d_hashes.as<int32_t>(), 4 * (size_t)c->nlandmarks, rows_on_host));
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));
   return AFP_OK;
 }
@@ -693,8 +656,7 @@ static int single_signal(afp_ctx* c, const void* pcm, int dtype, int on_host, in
     if ((rc = afp_launch_stats(c, 0, c->nitems))) return rc;
     if ((rc = afp_launch_sgram(c, dout))) return rc;
   }
-  if (out_on_host)
-    AFP_CUDA(c, cudaMemcpyAsync(out, dout, sizeof(double) * width * T, cudaMemcpyDeviceToHost, c->stream));
+  if (out_on_host) AFP_CUDA(c, afp_copy_out(c, out, dout, width * T, 1));
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));
   return AFP_OK;
 }

@@ -502,32 +502,22 @@ extern "C" int afp_flac_locate_batch(afp_ctx* c, const uint8_t* bytes, int bytes
   std::vector<FlacResult> r((size_t)nfiles);
   if (nfiles > 0) {
     AFP_CUDA(c, cudaSetDevice(c->device));
-    const uint8_t* dbytes = bytes;
-    if (bytes_on_host && nbytes_total > 0) {
-      AFP_CUDA(c, c->d_fl_in.reserve((size_t)nbytes_total + 16));
-      AFP_CUDA(c, cudaMemcpyAsync(c->d_fl_in.p, bytes, (size_t)nbytes_total, cudaMemcpyHostToDevice, c->stream));
-      dbytes = c->d_fl_in.as<uint8_t>();
-    }
+    const uint8_t* dbytes = nullptr;
+    int rc = afp_stage(c, c->d_fl_in, bytes, (size_t)nbytes_total, bytes_on_host, &dbytes);
+    if (rc) return rc;
     AFP_CUDA(c, c->d_fl_cand.reserve((size_t)cand + 16));
     AFP_CUDA(c, c->d_fl_frame.reserve(sizeof(FlacFrame) * (size_t)frames));
     AFP_CUDA(c, c->d_fl_file.reserve(sizeof(FlacFile) * (size_t)nfiles));
     AFP_CUDA(c, c->d_fl_res.reserve(sizeof(FlacResult) * (size_t)nfiles));
     AFP_CUDA(c, cudaMemcpyAsync(c->d_fl_file.p, d.data(), sizeof(FlacFile) * (size_t)nfiles, cudaMemcpyHostToDevice,
                                 c->stream));
-    if (blocks > 0) {
-      flac_candidate_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(dbytes, c->d_fl_file.as<FlacFile>(), nfiles,
-                                                                     c->d_fl_cand.as<uint8_t>());
-      AFP_CUDA(c, cudaGetLastError());
-      c->launches++;
-    }
-    flac_chain_kernel<<<(unsigned)((nfiles + 63) / 64), 64, 0, c->stream>>>(
-        dbytes, c->d_fl_cand.as<uint8_t>(), c->d_fl_file.as<FlacFile>(), nfiles, c->d_fl_frame.as<FlacFrame>(),
-        c->d_fl_res.as<FlacResult>());
-    AFP_CUDA(c, cudaGetLastError());
-    c->launches++;
-    AFP_CUDA(c, cudaMemcpyAsync(r.data(), c->d_fl_res.p, sizeof(FlacResult) * (size_t)nfiles, cudaMemcpyDeviceToHost,
-                                c->stream));
-    AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+    if ((rc = afp_launch(c, flac_candidate_kernel, (unsigned)blocks, 256, 0, dbytes, c->d_fl_file.as<FlacFile>(), nfiles,
+                         c->d_fl_cand.as<uint8_t>())) ||
+        (rc = afp_launch(c, flac_chain_kernel, (unsigned)((nfiles + 63) / 64), 64, 0, dbytes, c->d_fl_cand.as<uint8_t>(),
+                         c->d_fl_file.as<FlacFile>(), nfiles, c->d_fl_frame.as<FlacFrame>(),
+                         c->d_fl_res.as<FlacResult>())) ||
+        (rc = afp_read_back(c, r.data(), c->d_fl_res.as<FlacResult>(), (size_t)nfiles)))
+      return rc;
     c->fl.bytes = dbytes;
   }
   c->fl.nfiles = nfiles;
@@ -581,15 +571,14 @@ extern "C" int afp_flac_decode_batch(afp_ctx* c, int16_t* out, int64_t out_capac
     AFP_CUDA(c, cudaMemcpyAsync(c->d_fl_file.p, d.data(), sizeof(FlacFile) * (size_t)nfiles, cudaMemcpyHostToDevice,
                                 c->stream));
     AFP_CUDA(c, cudaMemsetAsync(c->d_fl_res.p, 0x7F, sizeof(int32_t) * (size_t)nfiles, c->stream));  // "no failure"
-    flac_decode_kernel<<<(unsigned)((gframes + DECODE_THREADS - 1) / DECODE_THREADS), DECODE_THREADS, 0, c->stream>>>(
-        c->fl.bytes, c->d_fl_file.as<FlacFile>(), nfiles, c->d_fl_frame.as<FlacFrame>(), gframes,
-        c->d_fl_scratch.as<int32_t>(), out, c->d_fl_res.as<int32_t>());
-    AFP_CUDA(c, cudaGetLastError());
-    c->launches++;
     std::vector<int32_t> dst((size_t)nfiles);
-    AFP_CUDA(c, cudaMemcpyAsync(dst.data(), c->d_fl_res.p, sizeof(int32_t) * (size_t)nfiles, cudaMemcpyDeviceToHost,
-                                c->stream));
-    AFP_CUDA(c, cudaStreamSynchronize(c->stream));       // `d` is pageable, and the codes go back now
+    int rc;
+    if ((rc = afp_launch(c, flac_decode_kernel, (unsigned)((gframes + DECODE_THREADS - 1) / DECODE_THREADS),
+                         DECODE_THREADS, 0, c->fl.bytes, c->d_fl_file.as<FlacFile>(), nfiles,
+                         c->d_fl_frame.as<FlacFrame>(), gframes, c->d_fl_scratch.as<int32_t>(), out,
+                         c->d_fl_res.as<int32_t>())) ||
+        (rc = afp_read_back(c, dst.data(), c->d_fl_res.as<int32_t>(), (size_t)nfiles)))   // `d` is pageable, too
+      return rc;
     for (int f = 0; f < nfiles; ++f)
       if (!st[f] && dst[f] != 0x7F7F7F7F) st[f] = dst[f];
   }

@@ -372,40 +372,26 @@ int afp_peak_status_code(int32_t bits) {
 }
 
 int afp_launch_peak_last_cols(afp_ctx* c, const int32_t* rows, const int64_t* off, int32_t nfiles, int32_t* out) {
-  if (nfiles <= 0) return AFP_OK;
-  afp_peak_last_col_kernel<<<(nfiles + 255) / 256, 256, 0, c->stream>>>(rows, off, nfiles, out);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
-  return AFP_OK;
+  return afp_launch(c, afp_peak_last_col_kernel, (nfiles + 255) / 256, 256, 0, rows, off, nfiles, out);
 }
 
 int afp_launch_scatter_peaks(afp_ctx* c, const int32_t* rows, const int64_t* off, int64_t nrows, int32_t nfiles,
                              int item_stride, int32_t* status) {
-  if (nrows <= 0) return AFP_OK;
-  afp_scatter_peaks_kernel<<<(unsigned)((nrows + 255) / 256), 256, 0, c->stream>>>(
-      rows, off, nfiles, c->d_items.as<ItemDesc>(), item_stride, c->ap.maxpksperframe, c->d_pk_bin.as<uint8_t>(),
-      c->d_pk_cnt.as<uint8_t>(), status);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
-  return AFP_OK;
+  return afp_launch(c, afp_scatter_peaks_kernel, (unsigned)((nrows + 255) / 256), 256, 0, rows, off, nfiles,
+                    c->d_items.as<ItemDesc>(), item_stride, c->ap.maxpksperframe, c->d_pk_bin.as<uint8_t>(),
+                    c->d_pk_cnt.as<uint8_t>(), status);
 }
 
 int afp_landmarks_from_peaks_impl(afp_ctx* c, const int32_t* rows_in, int64_t n, int on_host, int64_t* nlm) {
   c->batch_valid = false;
   c->nlandmarks = -1;
   if (n == 0) { c->nlandmarks = 0; if (nlm) *nlm = 0; return AFP_OK; }
-  const int32_t* drows = rows_in;
+  const int32_t* drows = nullptr;
   int32_t last[2];
-  if (on_host) {
-    AFP_CUDA(c, c->d_pk_in.reserve(sizeof(int32_t) * 2 * (size_t)n));
-    AFP_CUDA(c, cudaMemcpyAsync(c->d_pk_in.p, rows_in, sizeof(int32_t) * 2 * (size_t)n, cudaMemcpyHostToDevice,
-                                c->stream));
-    drows = c->d_pk_in.as<int32_t>();
-    last[0] = rows_in[2 * (n - 1)];
-  } else {
-    AFP_CUDA(c, cudaMemcpyAsync(last, rows_in + 2 * (n - 1), sizeof(last), cudaMemcpyDeviceToHost, c->stream));
-    AFP_CUDA(c, cudaStreamSynchronize(c->stream));
-  }
+  int rc = afp_stage(c, c->d_pk_in, rows_in, 2 * (size_t)n, on_host, &drows);
+  if (rc) return rc;
+  if (on_host) last[0] = rows_in[2 * (n - 1)];
+  else if ((rc = afp_read_back(c, last, rows_in + 2 * (n - 1), 2))) return rc;
   if (last[0] < 0 || last[0] > (1 << 28)) AFP_FAIL(c, AFP_ERR_INVALID, "bad peak column");
   const int T = last[0] + 1;   // scols = last peak column + 1 (:321)
   const size_t P = (size_t)c->ap.maxpksperframe, F = (size_t)c->ap.maxpairsperpeak, fr = (size_t)T + 1;
@@ -431,42 +417,33 @@ int afp_landmarks_from_peaks_impl(afp_ctx* c, const int32_t* rows_in, int64_t n,
   AFP_CUDA(c, cudaMemcpyAsync(c->d_item_scols.p, &T, sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
   AFP_CUDA(c, cudaMemsetAsync(c->d_pk_cnt.p, 0, fr, c->stream));
   AFP_CUDA(c, cudaMemsetAsync(c->d_pk_status.p, 0, sizeof(int32_t), c->stream));
-  int rc = afp_launch_scatter_peaks(c, drows, c->d_pk_inoff.as<int64_t>(), n, 1, 1, c->d_pk_status.as<int32_t>());
+  rc = afp_launch_scatter_peaks(c, drows, c->d_pk_inoff.as<int64_t>(), n, 1, 1, c->d_pk_status.as<int32_t>());
   if (rc) return rc;
   c->nfiles = 1; c->nitems = 1; c->total_frames = T; c->total_cols = T;
   HashArgs a = make_args(c);
   AFP_CUDA(c, cudaMemsetAsync(c->d_lm.p, 0xFF, sizeof(uint32_t) * P * F * fr, c->stream));
-  afp_landmark_kernel<<<1, K3_THREADS, 0, c->stream>>>(a);
-  AFP_CUDA(c, cudaGetLastError());
-  afp_lm_rows_kernel<false><<<(T + 127) / 128, 128, 0, c->stream>>>(a.lm, T, (int)(P * F), a.col_cnt, nullptr);
-  AFP_CUDA(c, cudaGetLastError());
-  afp_file_scan_kernel<<<1, 256, 0, c->stream>>>(a);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches += 3;
   int32_t total = 0, err = 0;
-  AFP_CUDA(c, cudaMemcpyAsync(&total, c->d_file_tot.p, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-  AFP_CUDA(c, cudaMemcpyAsync(&err, c->d_pk_status.p, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+  if ((rc = afp_launch(c, afp_landmark_kernel, 1, K3_THREADS, 0, a)) ||
+      (rc = afp_launch(c, afp_lm_rows_kernel<false>, (T + 127) / 128, 128, 0, a.lm, T, (int)(P * F), a.col_cnt,
+                       nullptr)) ||
+      (rc = afp_launch(c, afp_file_scan_kernel, 1, 256, 0, a)) ||
+      (rc = afp_read_back(c, &total, c->d_file_tot.as<int32_t>(), 1, &err, c->d_pk_status.as<int32_t>(), 1)))
+    return rc;
   if (afp_peak_status_code(err) == AFP_ERR_INVALID)
     AFP_FAIL(c, AFP_ERR_INVALID, "peak rows must be (col, bin) in [0,T)x[0,256), column-major, bins ascending");
   if (err) AFP_FAIL(c, AFP_ERR_UNSUPPORTED, "more peaks in one column than maxpksperframe");
   AFP_CUDA(c, c->d_hashes.reserve(sizeof(int32_t) * 4 * (size_t)(total + 1)));
-  if (total > 0) {
-    afp_lm_rows_kernel<true><<<(T + 127) / 128, 128, 0, c->stream>>>(a.lm, T, (int)(P * F), a.col_cnt,
-                                                                    c->d_hashes.as<int32_t>());
-    AFP_CUDA(c, cudaGetLastError());
-    c->launches++;
-  }
+  if (total > 0 &&
+      (rc = afp_launch(c, afp_lm_rows_kernel<true>, (T + 127) / 128, 128, 0, a.lm, T, (int)(P * F), a.col_cnt,
+                       c->d_hashes.as<int32_t>())))
+    return rc;
   c->nlandmarks = total;
   if (nlm) *nlm = total;
   return AFP_OK;
 }
 
 int afp_launch_scan_i32_to_i64(afp_ctx* c, const int32_t* in, int64_t* out, int64_t n) {
-  afp_scan_kernel<<<1, 1024, 0, c->stream>>>(in, out, n);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
-  return AFP_OK;
+  return afp_launch(c, afp_scan_kernel, 1, 1024, 0, in, out, n);
 }
 
 int afp_launch_file_hashes(afp_ctx* c, int file0, int nfiles) {
@@ -476,12 +453,7 @@ int afp_launch_file_hashes(afp_ctx* c, int file0, int nfiles) {
   const size_t smem = sizeof(uint32_t) * a.shifts * a.maxpks * (a.win + a.targetdt);
   AFP_CUDA(c, cudaFuncSetAttribute(afp_file_hash_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
                                    cudaSharedmemCarveoutMaxShared));
-  if (smem > 48 * 1024)
-    AFP_CUDA(c, cudaFuncSetAttribute(afp_file_hash_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  afp_file_hash_kernel<<<nfiles, K3_THREADS, smem, c->stream>>>(a);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
-  return AFP_OK;
+  return afp_launch(c, afp_file_hash_kernel, nfiles, K3_THREADS, smem, a);
 }
 
 int afp_launch_hashes(afp_ctx* c) {
@@ -490,9 +462,6 @@ int afp_launch_hashes(afp_ctx* c) {
 }
 
 int afp_write_hashes(afp_ctx* c) {
-  if (c->nfiles == 0 || c->total_cols == 0) return AFP_OK;
-  afp_gather_rows_kernel<<<c->nfiles, 256, 0, c->stream>>>(make_args(c));
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
-  return AFP_OK;
+  if (c->total_cols == 0) return AFP_OK;
+  return afp_launch(c, afp_gather_rows_kernel, c->nfiles, 256, 0, make_args(c));
 }

@@ -3,7 +3,9 @@
 
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <algorithm>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "afp.h"
@@ -13,10 +15,22 @@
 #define AFP_GAUSS_PAD (AFP_GAUSS_N + AFP_GAUSS_N / 8 + 2)   // padded smem layout, see afp_peaks.cu
 #define AFP_NO_HASH 0xFFFFFFFFu
 
-// A device buffer that only ever grows (workspace arena member).
+// A device buffer that only ever grows (workspace arena member); it owns its allocation.
 struct DevBuf {
   void* p = nullptr;
   size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  DevBuf(DevBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  DevBuf& operator=(DevBuf&& o) noexcept {
+    std::swap(p, o.p);
+    std::swap(cap, o.cap);
+    return *this;
+  }
+  ~DevBuf() {
+    if (p) cudaFree(p);
+  }
   cudaError_t reserve(size_t bytes) {
     if (bytes <= cap) return cudaSuccess;
     if (p) cudaFree(p);
@@ -26,11 +40,6 @@ struct DevBuf {
     cudaError_t e = cudaMalloc(&p, want);
     if (e == cudaSuccess) cap = want;
     return e;
-  }
-  void release() {
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
   }
   template <class T> T* as() const { return reinterpret_cast<T*>(p); }
 };
@@ -142,6 +151,7 @@ struct afp_ctx {
   DevBuf d_pk_inoff;       // int64 [nfiles+1] their per-file offsets
   DevBuf d_pk_status;      // int32 [nfiles]   per-file PK_* flags of the peak scatter (afp_hash.cu)
   DevBuf d_tmp;            // misc
+  DevBuf d_cub;            // CUB's temporary storage (cub_call)
 
   // table + matching
   TableDev tab;
@@ -152,7 +162,7 @@ struct afp_ctx {
   DevBuf d_st_obkt, d_st_opos, d_st_oval, d_st_slot, d_st_last;
   int64_t store_novf = 0;
   // device-side HashTable.remove / retrieve for a list of ids (afp_table_edit.cu)
-  DevBuf d_ed_ids, d_ed_bits, d_ed_slot, d_ed_cnt, d_ed_off, d_ed_key, d_ed_key2, d_ed_val, d_ed_val2, d_ed_cub;
+  DevBuf d_ed_ids, d_ed_bits, d_ed_slot, d_ed_cnt, d_ed_off, d_ed_key, d_ed_key2, d_ed_val, d_ed_val2;
   DevBuf d_ed_uoff, d_ed_req, d_ed_rows;
   int64_t rt_total = -1;              // rows of the last afp_table_retrieve_ids; -1 = none
   int rt_src = 0;                     // where they are: 0 d_ed_val, 1 d_ed_val2, 2 d_ed_rows
@@ -171,14 +181,14 @@ struct afp_ctx {
   int64_t match_total_rows = -1;
   int32_t match_row_cap = 0;
   uint64_t match_layout = 0;   // carve-up of d_mscratch whose counters/histograms are known to be zero
-  // long-query path (afp_match_long.cu): sort keys, CUB temp, per-id counters and slots, ranking
+  // long-query path (afp_match_long.cu): sort keys, per-id counters and slots, ranking
   // keys, candidate segments and rows, candidates' hits, per-CTA dtime histograms
-  DevBuf d_lg_key, d_lg_cub, d_lg_id, d_lg_w, d_lg_cand, d_lg_dts, d_lg_hist;
+  DevBuf d_lg_key, d_lg_id, d_lg_w, d_lg_cand, d_lg_dts, d_lg_hist;
   int lg_ctas = 0;                  // CTAs of the mode pass (one histogram pair each)
   std::vector<int> match_long;      // queries of the last batch the long-query path finished
   // exact_count / find_time_range finish (afp_match_options.cu): per-slot segments and lookup,
-  // routed hits, approximate-row flags, mode supports, packed keys, qtimes, CUB temp, finished rows
-  DevBuf d_op_slot, d_op_hit, d_op_mode, d_op_sup, d_op_key, d_op_tq, d_op_cub, d_op_rows;
+  // routed hits, approximate-row flags, mode supports, packed keys, qtimes, finished rows
+  DevBuf d_op_slot, d_op_hit, d_op_mode, d_op_sup, d_op_key, d_op_tq, d_op_rows;
   // the same finish on one shard of an id-range sharded table, in two calls around the caller's
   // all-reduce of the per-query largest qtime: what the ranking call leaves for the finish call,
   // and the smallest local rank per query whose quantile read failed (0x7f7f7f7f: none)
@@ -220,6 +230,109 @@ struct afp_ctx {
     (ctx)->err = (msg);          \
     return (code);               \
   } while (0)
+
+// ---- launches, copies and scratch: every entry point goes through these -----------------------
+
+// Launch `kernel` on c->stream as it is now (run_chunked switches it per chunk) and count one launch
+// in afp_launch_count.  An empty grid is no launch.  Above 48 KB of dynamic shared memory the kernel's
+// limit is raised first.
+template <class... P, class... A>
+int afp_launch(afp_ctx* c, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, A&&... args) {
+  if ((size_t)grid.x * grid.y * grid.z == 0) return AFP_OK;
+  if (smem > 48 * 1024)
+    AFP_CUDA(c, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kernel<<<grid, block, smem, c->stream>>>(std::forward<A>(args)...);
+  AFP_CUDA(c, cudaGetLastError());
+  c->launches++;
+  return AFP_OK;
+}
+
+// A two-phase CUB call f(temp, bytes): the size query, then the call with the context's temporary
+// buffer.  Counts one launch, whatever CUB runs.
+template <class F>
+int cub_call(afp_ctx* c, F f) {
+  size_t bytes = 0;
+  AFP_CUDA(c, f(nullptr, bytes));
+  AFP_CUDA(c, c->d_cub.reserve(bytes + 16));
+  AFP_CUDA(c, f(c->d_cub.p, bytes));
+  c->launches++;
+  return AFP_OK;
+}
+
+// n values of the device array src to dst, which is host memory or device memory as dst_on_host says;
+// queued on c->stream.
+template <class T>
+cudaError_t afp_copy_out(afp_ctx* c, T* dst, const T* src, size_t n, int dst_on_host) {
+  return cudaMemcpyAsync(dst, src, sizeof(T) * n, dst_on_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice,
+                         c->stream);
+}
+
+// n values of the caller's array src, host memory or device memory as src_on_host says, to the device
+// array dst; queued on c->stream.
+template <class T>
+cudaError_t afp_copy_in(afp_ctx* c, T* dst, const T* src, size_t n, int src_on_host) {
+  return cudaMemcpyAsync(dst, src, sizeof(T) * n, src_on_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice,
+                         c->stream);
+}
+
+// The caller's n values of T on the device: *dev = src itself when it is device memory, else its copy in
+// `stage` (queued on c->stream).
+template <class T>
+int afp_stage(afp_ctx* c, DevBuf& stage, const T* src, size_t n, int on_host, const T** dev) {
+  *dev = src;
+  if (!on_host || n == 0) return AFP_OK;
+  AFP_CUDA(c, stage.reserve(sizeof(T) * n + 16));
+  AFP_CUDA(c, afp_copy_in(c, stage.as<T>(), src, n, 1));
+  *dev = stage.as<T>();
+  return AFP_OK;
+}
+
+inline cudaError_t afp_read_async(afp_ctx*) { return cudaSuccess; }
+template <class T, class... R>
+cudaError_t afp_read_async(afp_ctx* c, T* h, const T* d, size_t n, R... rest) {
+  const cudaError_t e = cudaMemcpyAsync(h, d, sizeof(T) * n, cudaMemcpyDeviceToHost, c->stream);
+  return e != cudaSuccess ? e : afp_read_async(c, rest...);
+}
+
+// Host copies of device values behind everything queued on c->stream, and one synchronise for all of
+// them: afp_read_back(c, &x, d_x, 1, v.data(), d_v, n, ...).
+template <class... A>
+int afp_read_back(afp_ctx* c, A... a) {
+  AFP_CUDA(c, afp_read_async(c, a...));
+  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+  return AFP_OK;
+}
+
+// Consecutive 16-byte-aligned arrays of one DevBuf.  afp_carve runs the same take<T>(n) sequence twice:
+// a Carver without a base only adds up the bytes to reserve, then one on the buffer hands out the arrays.
+struct Carver {
+  char* base = nullptr;
+  size_t bytes = 0;   // offset of the next array
+  template <class T> T* take(int64_t n) {
+    T* r = base ? reinterpret_cast<T*>(base + bytes) : nullptr;
+    bytes += ((size_t)std::max<int64_t>(n, 1) * sizeof(T) + 15) & ~(size_t)15;
+    return r;
+  }
+};
+
+template <class F>
+int afp_carve(afp_ctx* c, DevBuf& buf, F layout) {
+  Carver size;
+  layout(size);
+  AFP_CUDA(c, buf.reserve(size.bytes));
+  Carver arrays{buf.as<char>()};
+  layout(arrays);
+  return AFP_OK;
+}
+
+// What a workspace buffer may grow to: half of the free device memory plus what `held` holds already,
+// and at least 1 GiB.
+inline cudaError_t afp_memory_budget(const DevBuf& held, size_t* budget) {
+  size_t free_b = 0, total_b = 0;
+  const cudaError_t e = cudaMemGetInfo(&free_b, &total_b);
+  *budget = std::max<size_t>((free_b + held.cap) / 2, (size_t)1 << 30);
+  return e;
+}
 
 // ---- kernel launchers (defined in the .cu files) -------------------------------
 int afp_launch_tile_table(afp_ctx* c);

@@ -532,27 +532,20 @@ int afp_finish_match_rows(afp_ctx* c, int nqueries, int row_cap, int64_t* total_
   int* d_over = c->d_mrow_cnt.as<int>() + nqueries + 1;
   AFP_CUDA(c, cudaMemsetAsync(d_over, 0, sizeof(int), c->stream));
   AFP_CUDA(c, c->d_tmp.reserve(sizeof(int32_t) * (size_t)(nqueries + 8)));
-  afp_clamp_kernel<<<(nqueries + 255) / 256, 256, 0, c->stream>>>(c->d_mrow_cnt.as<int32_t>(), nqueries, row_cap,
-                                                                  c->d_tmp.as<int32_t>(), d_over);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
-  int rc;
-  if ((rc = afp_launch_scan_i32_to_i64(c, c->d_tmp.as<int32_t>(), c->d_mrow_off.as<int64_t>(), nqueries))) return rc;
   int64_t total = 0;
   int over = 0;
-  AFP_CUDA(c, cudaMemcpyAsync(&total, c->d_mrow_off.as<int64_t>() + nqueries, sizeof(int64_t),
-                              cudaMemcpyDeviceToHost, c->stream));
-  AFP_CUDA(c, cudaMemcpyAsync(&over, d_over, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+  int rc;
+  if ((rc = afp_launch(c, afp_clamp_kernel, (nqueries + 255) / 256, 256, 0, c->d_mrow_cnt.as<int32_t>(), nqueries,
+                       row_cap, c->d_tmp.as<int32_t>(), d_over)) ||
+      (rc = afp_launch_scan_i32_to_i64(c, c->d_tmp.as<int32_t>(), c->d_mrow_off.as<int64_t>(), nqueries)) ||
+      (rc = afp_read_back(c, &total, c->d_mrow_off.as<int64_t>() + nqueries, 1, &over, d_over, 1)))
+    return rc;
   if (over) AFP_FAIL(c, AFP_ERR_UNSUPPORTED, "row capacity exceeded: a query produced more rows than afp_matcher_params.row_capacity");
   AFP_CUDA(c, c->d_mrows_packed.reserve(sizeof(int32_t) * 7 * (size_t)(total + 1)));
-  if (total > 0) {
-    afp_pack_rows_kernel<<<nqueries, 64, 0, c->stream>>>(c->d_mrows.as<int32_t>(), c->d_mrow_cnt.as<int32_t>(),
-                                                         c->d_mrow_off.as<int64_t>(), row_cap,
-                                                         c->d_mrows_packed.as<int32_t>());
-    AFP_CUDA(c, cudaGetLastError());
-    c->launches++;
-  }
+  if (total > 0 &&
+      (rc = afp_launch(c, afp_pack_rows_kernel, nqueries, 64, 0, c->d_mrows.as<int32_t>(), c->d_mrow_cnt.as<int32_t>(),
+                       c->d_mrow_off.as<int64_t>(), row_cap, c->d_mrows_packed.as<int32_t>())))
+    return rc;
   c->match_total_rows = total;
   *total_out = total;
   return AFP_OK;
@@ -567,16 +560,13 @@ int afp_table_upload(afp_ctx* c, const uint32_t* table, const int32_t* counts, i
     AFP_FAIL(c, AFP_ERR_INVALID, "bad table geometry");
   AFP_CUDA(c, cudaSetDevice(c->device));
   const size_t nb = (size_t)1 << hashbits;
-  const cudaMemcpyKind kind = on_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
   c->tab.loaded = false;
   AFP_CUDA(c, c->tab.table.reserve(nb * (size_t)depth * sizeof(uint32_t)));
   AFP_CUDA(c, c->tab.counts.reserve(nb * sizeof(int32_t)));
   AFP_CUDA(c, c->tab.hashesperid.reserve(((size_t)nids + 1) * sizeof(uint32_t)));
-  AFP_CUDA(c, cudaMemcpyAsync(c->tab.table.p, table, nb * (size_t)depth * sizeof(uint32_t), kind, c->stream));
-  AFP_CUDA(c, cudaMemcpyAsync(c->tab.counts.p, counts, nb * sizeof(int32_t), kind, c->stream));
-  if (nids > 0)
-    AFP_CUDA(c, cudaMemcpyAsync(c->tab.hashesperid.p, hashesperid, (size_t)nids * sizeof(uint32_t), kind,
-                                c->stream));
+  AFP_CUDA(c, afp_copy_in(c, c->tab.table.as<uint32_t>(), table, nb * (size_t)depth, on_host));
+  AFP_CUDA(c, afp_copy_in(c, c->tab.counts.as<int32_t>(), counts, nb, on_host));
+  if (nids > 0) AFP_CUDA(c, afp_copy_in(c, c->tab.hashesperid.as<uint32_t>(), hashesperid, (size_t)nids, on_host));
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));
   c->tab.hashbits = hashbits;
   c->tab.depth = depth;
@@ -594,21 +584,18 @@ int afp_table_stats(afp_ctx* c) {
   unsigned* d = c->d_tmp.as<unsigned>();
   const unsigned init[3] = {0xffffffffu, 0u, 0u};
   AFP_CUDA(c, cudaMemcpyAsync(d, init, sizeof(init), cudaMemcpyHostToDevice, c->stream));
-  afp_hpi_stats_kernel<<<296, 256, 0, c->stream>>>(c->tab.hashesperid.as<uint32_t>(), c->tab.nids, d);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
   unsigned h[3];
-  AFP_CUDA(c, cudaMemcpyAsync(h, d, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+  int rc;
+  if ((rc = afp_launch(c, afp_hpi_stats_kernel, 296, 256, 0, c->tab.hashesperid.as<uint32_t>(), c->tab.nids, d)) ||
+      (rc = afp_read_back(c, h, d, 3)))
+    return rc;
   if (h[1] != 0u) {          // zero entries exist: harmless as long as no table entry names them
     const int64_t nb = (int64_t)1 << c->tab.hashbits;
-    afp_refzero_kernel<<<(unsigned)((nb + 7) / 8), 256, 0, c->stream>>>(
-        c->tab.table.as<uint32_t>(), c->tab.counts.as<int32_t>(), nb, c->tab.depth, c->tab.maxtimebits,
-        c->tab.hashesperid.as<uint32_t>(), c->tab.nids, d + 2);
-    AFP_CUDA(c, cudaGetLastError());
-    c->launches++;
-    AFP_CUDA(c, cudaMemcpyAsync(h, d, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
-    AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+    if ((rc = afp_launch(c, afp_refzero_kernel, (unsigned)((nb + 7) / 8), 256, 0, c->tab.table.as<uint32_t>(),
+                         c->tab.counts.as<int32_t>(), nb, c->tab.depth, c->tab.maxtimebits,
+                         c->tab.hashesperid.as<uint32_t>(), c->tab.nids, d + 2)) ||
+        (rc = afp_read_back(c, h, d, 3)))
+      return rc;
   }
   c->tab.hmin = (h[0] != 0xffffffffu && h[2] == 0u) ? h[0] : 0u;
   return AFP_OK;
@@ -627,23 +614,9 @@ int afp_table_restrict_ids(afp_ctx* c, int64_t id_lo, int64_t id_hi) {
   if (id_lo < 0 || id_hi < id_lo) AFP_FAIL(c, AFP_ERR_INVALID, "bad id range");
   AFP_CUDA(c, cudaSetDevice(c->device));
   const int64_t nb = (int64_t)1 << c->tab.hashbits;
-  afp_restrict_ids_kernel<<<(unsigned)((nb + 255) / 256), 256, 0, c->stream>>>(
-      c->tab.table.as<uint32_t>(), c->tab.counts.as<int32_t>(), nb, c->tab.depth, c->tab.maxtimebits,
-      (uint32_t)id_lo, (uint32_t)id_hi);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
-  return AFP_OK;
-}
-
-static int stage_queries(afp_ctx* c, const int32_t* q, int64_t nrows, int on_host, const int32_t** dq) {
-  *dq = q;
-  if (on_host && nrows > 0) {
-    AFP_CUDA(c, c->d_q.reserve(sizeof(int32_t) * 2 * (size_t)nrows));
-    AFP_CUDA(c, cudaMemcpyAsync(c->d_q.p, q, sizeof(int32_t) * 2 * (size_t)nrows, cudaMemcpyHostToDevice,
-                                c->stream));
-    *dq = c->d_q.as<int32_t>();
-  }
-  return AFP_OK;
+  return afp_launch(c, afp_restrict_ids_kernel, (unsigned)((nb + 255) / 256), 256, 0, c->tab.table.as<uint32_t>(),
+                    c->tab.counts.as<int32_t>(), nb, c->tab.depth, c->tab.maxtimebits, (uint32_t)id_lo,
+                    (uint32_t)id_hi);
 }
 
 int afp_get_hits(afp_ctx* c, const int32_t* q_rows, int64_t nq, int q_on_host, int64_t* nhits) {
@@ -652,29 +625,22 @@ int afp_get_hits(afp_ctx* c, const int32_t* q_rows, int64_t nq, int q_on_host, i
   AFP_CUDA(c, cudaSetDevice(c->device));
   c->nhits = -1;
   const int32_t* dq = nullptr;
-  int rc = stage_queries(c, q_rows, nq, q_on_host, &dq);
+  int rc = afp_stage(c, c->d_q, q_rows, 2 * (size_t)nq, q_on_host, &dq);
   if (rc) return rc;
   AFP_CUDA(c, c->d_tmp.reserve(sizeof(int32_t) * (size_t)(nq + 1)));
   AFP_CUDA(c, c->d_hit_off.reserve(sizeof(int64_t) * (size_t)(nq + 1)));
-  if (nq > 0) {
-    afp_hit_count_kernel<<<(unsigned)((nq + 255) / 256), 256, 0, c->stream>>>(
-        dq, nq, c->tab.counts.as<int32_t>(), c->tab.hashbits, c->tab.depth, c->d_tmp.as<int32_t>());
-    AFP_CUDA(c, cudaGetLastError());
-    c->launches++;
-  }
-  if ((rc = afp_launch_scan_i32_to_i64(c, c->d_tmp.as<int32_t>(), c->d_hit_off.as<int64_t>(), nq))) return rc;
   int64_t total = 0;
-  AFP_CUDA(c, cudaMemcpyAsync(&total, c->d_hit_off.as<int64_t>() + nq, sizeof(int64_t), cudaMemcpyDeviceToHost,
-                              c->stream));
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+  if ((rc = afp_launch(c, afp_hit_count_kernel, (unsigned)((nq + 255) / 256), 256, 0, dq, nq,
+                       c->tab.counts.as<int32_t>(), c->tab.hashbits, c->tab.depth, c->d_tmp.as<int32_t>())) ||
+      (rc = afp_launch_scan_i32_to_i64(c, c->d_tmp.as<int32_t>(), c->d_hit_off.as<int64_t>(), nq)) ||
+      (rc = afp_read_back(c, &total, c->d_hit_off.as<int64_t>() + nq, 1)))
+    return rc;
   AFP_CUDA(c, c->d_hits.reserve(sizeof(int32_t) * 4 * (size_t)(total + 1)));
-  if (total > 0) {
-    afp_hit_write_kernel<<<(unsigned)((nq + 7) / 8), 256, 0, c->stream>>>(
-        dq, nq, c->tab.table.as<uint32_t>(), c->tab.counts.as<int32_t>(), c->tab.hashbits, c->tab.depth,
-        c->tab.maxtimebits, c->d_hit_off.as<int64_t>(), c->d_hits.as<int32_t>());
-    AFP_CUDA(c, cudaGetLastError());
-    c->launches++;
-  }
+  if (total > 0 &&
+      (rc = afp_launch(c, afp_hit_write_kernel, (unsigned)((nq + 7) / 8), 256, 0, dq, nq, c->tab.table.as<uint32_t>(),
+                       c->tab.counts.as<int32_t>(), c->tab.hashbits, c->tab.depth, c->tab.maxtimebits,
+                       c->d_hit_off.as<int64_t>(), c->d_hits.as<int32_t>())))
+    return rc;
   c->nhits = total;
   c->hits_nq = nq;
   if (nhits) *nhits = total;
@@ -685,9 +651,7 @@ int afp_fetch_hits(afp_ctx* c, int32_t* hits, int hits_on_host) {
   if (!c) return AFP_ERR_INVALID;
   if (c->nhits < 0) AFP_FAIL(c, AFP_ERR_STATE, "afp_get_hits has not been called");
   AFP_CUDA(c, cudaSetDevice(c->device));
-  if (hits && c->nhits > 0)
-    AFP_CUDA(c, cudaMemcpyAsync(hits, c->d_hits.p, sizeof(int32_t) * 4 * (size_t)c->nhits,
-                                hits_on_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, c->stream));
+  if (hits && c->nhits > 0) AFP_CUDA(c, afp_copy_out(c, hits, c->d_hits.as<int32_t>(), 4 * (size_t)c->nhits, hits_on_host));
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));
   return AFP_OK;
 }
@@ -723,7 +687,7 @@ int afp_match_batch(afp_ctx* c, const int32_t* q_rows, int q_on_host, int32_t nq
   if (nqueries && q_offsets[0] != 0) AFP_FAIL(c, AFP_ERR_INVALID, "q_offsets[0] must be 0");
   if (nrows_in > 0 && !q_rows) return AFP_ERR_INVALID;
   const int32_t* dq = nullptr;
-  int rc = stage_queries(c, q_rows, nrows_in, q_on_host, &dq);
+  int rc = afp_stage(c, c->d_q, q_rows, 2 * (size_t)nrows_in, q_on_host, &dq);
   if (rc) return rc;
   AFP_CUDA(c, c->d_qoff.reserve(sizeof(int64_t) * (size_t)(nqueries + 1)));
   AFP_CUDA(c, c->d_mrow_cnt.reserve(sizeof(int32_t) * (size_t)(nqueries + 2)));
@@ -742,22 +706,16 @@ int afp_match_batch(afp_ctx* c, const int32_t* q_rows, int q_on_host, int32_t nq
   int* d_mm = c->d_tmp.as<int>();
   AFP_CUDA(c, cudaMemsetAsync(d_mm, 0, 4 * sizeof(int), c->stream));
   auto qmax = [&](int64_t r0, int64_t r1, int* out) {
-    if (r1 <= r0) return cudaSuccess;
-    afp_qmax_kernel<<<296, 256, 0, c->stream>>>(dq + 2 * r0, r1 - r0, out, out + 1);
-    c->launches++;
-    return cudaGetLastError();
+    return r1 <= r0 ? AFP_OK : afp_launch(c, afp_qmax_kernel, 296, 256, 0, dq + 2 * r0, r1 - r0, out, out + 1);
   };
   {
     int64_t r0 = 0;
     for (int li : longq) {
-      AFP_CUDA(c, qmax(r0, q_offsets[li], d_mm));
-      AFP_CUDA(c, qmax(q_offsets[li], q_offsets[li + 1], d_mm + 2));
+      if ((rc = qmax(r0, q_offsets[li], d_mm)) || (rc = qmax(q_offsets[li], q_offsets[li + 1], d_mm + 2))) return rc;
       r0 = q_offsets[li + 1];
     }
-    AFP_CUDA(c, qmax(r0, nrows_in, d_mm));
+    if ((rc = qmax(r0, nrows_in, d_mm)) || (rc = afp_read_back(c, h_mm, d_mm, 4))) return rc;
   }
-  AFP_CUDA(c, cudaMemcpyAsync(h_mm, d_mm, sizeof(h_mm), cudaMemcpyDeviceToHost, c->stream));
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
   if (h_mm[1] < 0 || h_mm[3] < 0) AFP_FAIL(c, AFP_ERR_INVALID, "negative query time");
 
   // persistent grid; a fixed CTA count keeps the scratch layout (and its zeroed state) reusable
@@ -788,38 +746,34 @@ int afp_match_batch(afp_ctx* c, const int32_t* q_rows, int q_on_host, int32_t nq
   // The scratch is per CTA and sized for the longest query the fast / general kernels run (whole
   // shows, searching_for_ads.md, take the long-query path): when it would not fit the memory
   // budget the grid shrinks instead of the call failing.
-  {
-    size_t free_b = 0, total_b = 0;
-    AFP_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
-    const size_t budget = std::max<size_t>((free_b + c->d_mscratch.cap) / 2, (size_t)1 << 30);
-    if (per_cta * (size_t)nctas > budget) nctas = (int)std::max<size_t>(1, budget / per_cta);
-    if (per_cta > budget) AFP_FAIL(c, AFP_ERR_NOMEM, "match scratch of one query exceeds the device memory budget");
-  }
+  size_t budget = 0;
+  AFP_CUDA(c, afp_memory_budget(c->d_mscratch, &budget));
+  if (per_cta * (size_t)nctas > budget) nctas = (int)std::max<size_t>(1, budget / per_cta);
+  if (per_cta > budget) AFP_FAIL(c, AFP_ERR_NOMEM, "match scratch of one query exceeds the device memory budget");
   const size_t before = c->d_mscratch.cap;
-  AFP_CUDA(c, c->d_mscratch.reserve(per_cta * (size_t)nctas + 1024));
   AFP_CUDA(c, c->d_mrows.reserve(sizeof(int32_t) * 7 * (size_t)a.row_cap * (size_t)nqueries));
-  // carve the scratch; the histograms must start (and are left) zeroed
-  char* base = c->d_mscratch.as<char>();
-  auto carve = [&](size_t bytes) {
-    char* p0 = base;
-    base += (bytes + 15) & ~(size_t)15;
-    return p0;
-  };
-  a.hits = (uint2*)carve(sizeof(uint2) * a.hits_cap * nctas);
-  a.wtd = (double*)carve(sizeof(double) * a.hits_cap * nctas);
-  a.dlist = (uint32_t*)carve(sizeof(uint32_t) * a.hits_cap * nctas);
-  a.dts = (uint32_t*)carve(sizeof(uint32_t) * a.hits_cap * nctas);
-  a.recs = (uint32_t*)carve(sizeof(uint32_t) * a.hits_cap * nctas);
-  a.rawl = (uint32_t*)carve(sizeof(uint32_t) * a.hits_cap * nctas);
-  char* zero0 = base;
-  a.hist = (int32_t*)carve(sizeof(int32_t) * (size_t)a.hist_len * nctas);
-  a.filt = (int32_t*)carve(sizeof(int32_t) * (size_t)a.hist_len * nctas);
+  // carve the scratch; the histograms at its end must start (and are left) zeroed
+  const int64_t per_hit = a.hits_cap * nctas, per_bin = (int64_t)a.hist_len * nctas;
+  size_t zero0 = 0, zero1 = 0;
+  if ((rc = afp_carve(c, c->d_mscratch, [&](Carver& k) {
+         a.hits = k.take<uint2>(per_hit);
+         a.wtd = k.take<double>(per_hit);
+         a.dlist = k.take<uint32_t>(per_hit);
+         a.dts = k.take<uint32_t>(per_hit);
+         a.recs = k.take<uint32_t>(per_hit);
+         a.rawl = k.take<uint32_t>(per_hit);
+         zero0 = k.bytes;
+         a.hist = k.take<int32_t>(per_bin);
+         a.filt = k.take<int32_t>(per_bin);
+         zero1 = k.bytes;
+       })))
+    return rc;
   // the histograms are left zeroed by the kernel itself: clear them only when the
   // carve-up changed (or the buffer moved)
   const uint64_t layout = (uint64_t)a.hits_cap * 1000003ull ^ (uint64_t)a.nids * 7919ull ^ (uint64_t)a.hist_len * 31ull ^
                           (uint64_t)(uintptr_t)c->d_mscratch.p ^ (uint64_t)before ^ (uint64_t)nctas * 2654435761ull;
   if (layout != c->match_layout) {
-    AFP_CUDA(c, cudaMemsetAsync(zero0, 0, (size_t)(base - zero0), c->stream));
+    AFP_CUDA(c, cudaMemsetAsync(c->d_mscratch.as<char>() + zero0, 0, zero1 - zero0, c->stream));
     c->match_layout = layout;
   }
   a.rows = c->d_mrows.as<int32_t>();
@@ -884,19 +838,11 @@ int afp_match_batch(afp_ctx* c, const int32_t* q_rows, int q_on_host, int32_t nq
     AFP_CUDA(c, c->d_mfast.reserve(sizeof(uint2) * (size_t)a.mh_cap * (size_t)nctas));
     a.mhits = c->d_mfast.as<uint2>();
     AFP_CUDA(c, cudaMemsetAsync(a.nlist, 0, sizeof(int), c->stream));
-    AFP_CUDA(c, afp_launch_match_fast(a, nctas, c->stream));
-    c->launches++;
+    if ((rc = afp_launch_match_fast(c, a, nctas))) return rc;
     c->match_fast_ran = true;
   }
-  if (nshort) {
-    AFP_CUDA(c, cudaFuncSetAttribute(afp_match_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)(QCAP * sizeof(unsigned long long))));
-    afp_match_kernel<<<nctas, MT, QCAP * sizeof(unsigned long long), c->stream>>>(a);
-    AFP_CUDA(c, cudaGetLastError());
-    c->launches++;
-  }
-  if (c->match_fast_ran)
-    AFP_CUDA(c, cudaMemcpyAsync(&c->match_general_h, a.nlist, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  if (nshort && (rc = afp_launch(c, afp_match_kernel, nctas, MT, QCAP * sizeof(unsigned long long), a))) return rc;
+  if (c->match_fast_ran) AFP_CUDA(c, afp_read_async(c, &c->match_general_h, a.nlist, 1));
   if (nlong) {
     // ---- long queries (afp_match_long.cu): one histogram pair per CTA of the mode pass, sized
     // over the long queries' times, zeroed here and left zeroed by the mode search
@@ -904,9 +850,7 @@ int afp_match_batch(afp_ctx* c, const int32_t* q_rows, int q_on_host, int32_t nq
     al.bias = h_mm[2] + p->window + 2;
     al.hist_len = (1 << c->tab.maxtimebits) + al.bias + p->window + 4;
     const size_t per = (size_t)al.hist_len * 2 * sizeof(int32_t);
-    size_t free_b = 0, total_b = 0;
-    AFP_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
-    const size_t budget = std::max<size_t>((free_b + c->d_lg_hist.cap) / 2, (size_t)1 << 30);
+    AFP_CUDA(c, afp_memory_budget(c->d_lg_hist, &budget));
     c->lg_ctas = (int)std::max<size_t>(1, std::min<size_t>((size_t)c->num_sms, budget / per));
     AFP_CUDA(c, c->d_lg_hist.reserve(per * (size_t)c->lg_ctas));
     al.hist = c->d_lg_hist.as<int32_t>();
@@ -937,10 +881,8 @@ int afp_fetch_match_status(afp_ctx* c, int32_t* status) {
   if (!c->match_fast_ran) {
     for (int i = 0; i < 8 * c->match_nq; ++i) status[i] = -1;
   } else {
-    if (c->match_nq > 0)
-      AFP_CUDA(c, cudaMemcpyAsync(status, c->d_mqlist.as<int32_t>() + 4 + c->match_nq,
-                                  sizeof(int32_t) * 8 * (size_t)c->match_nq, cudaMemcpyDeviceToHost, c->stream));
-    AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+    const int rc = afp_read_back(c, status, c->d_mqlist.as<int32_t>() + 4 + c->match_nq, 8 * (size_t)c->match_nq);
+    if (rc) return rc;
   }
   for (int qi : c->match_long) {          // finished by the long-query path
     status[8 * (size_t)qi] = 6;
@@ -954,12 +896,11 @@ int afp_fetch_match_candidates(afp_ctx* c, double* cand, int32_t* counts, int on
   if (c->match_total_rows < 0 || !c->match_published)
     AFP_FAIL(c, AFP_ERR_STATE, "afp_match_batch with publish_candidates has not been called");
   AFP_CUDA(c, cudaSetDevice(c->device));
-  const cudaMemcpyKind kind = on_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
   if (cand && c->match_nq > 0 && c->match_sdepth > 0)
-    AFP_CUDA(c, cudaMemcpyAsync(cand, c->d_mcand.p, sizeof(double) * 3 * (size_t)c->match_sdepth * (size_t)c->match_nq,
-                                kind, c->stream));
+    AFP_CUDA(c, afp_copy_out(c, cand, c->d_mcand.as<double>(), 3 * (size_t)c->match_sdepth * (size_t)c->match_nq,
+                             on_host));
   if (counts && c->match_nq > 0)
-    AFP_CUDA(c, cudaMemcpyAsync(counts, c->d_mcand_cnt.p, sizeof(int32_t) * 2 * (size_t)c->match_nq, kind, c->stream));
+    AFP_CUDA(c, afp_copy_out(c, counts, c->d_mcand_cnt.as<int32_t>(), 2 * (size_t)c->match_nq, on_host));
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));
   return AFP_OK;
 }
@@ -970,13 +911,10 @@ int afp_fetch_match_rows(afp_ctx* c, int32_t* rows, int rows_on_host, int64_t* r
   AFP_CUDA(c, cudaSetDevice(c->device));
   if (row_offsets) {
     if (c->match_nq == 0) row_offsets[0] = 0;
-    else
-      AFP_CUDA(c, cudaMemcpyAsync(row_offsets, c->d_mrow_off.p, sizeof(int64_t) * (size_t)(c->match_nq + 1),
-                                  cudaMemcpyDeviceToHost, c->stream));
+    else AFP_CUDA(c, afp_copy_out(c, row_offsets, c->d_mrow_off.as<int64_t>(), (size_t)(c->match_nq + 1), 1));
   }
   if (rows && c->match_total_rows > 0)
-    AFP_CUDA(c, cudaMemcpyAsync(rows, c->d_mrows_packed.p, sizeof(int32_t) * 7 * (size_t)c->match_total_rows,
-                                rows_on_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, c->stream));
+    AFP_CUDA(c, afp_copy_out(c, rows, c->d_mrows_packed.as<int32_t>(), 7 * (size_t)c->match_total_rows, rows_on_host));
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));
   return AFP_OK;
 }

@@ -47,7 +47,7 @@ struct MatchArgs {
 };
 
 // The fast kernel over every query (afp_match_fast.cu); it appends the ones it hands over to a.qlist.
-cudaError_t afp_launch_match_fast(const MatchArgs& a, int nctas, cudaStream_t stream);
+int afp_launch_match_fast(afp_ctx* c, const MatchArgs& a, int nctas);
 // Query qi (rows q0 .. q0+nq of a.q) on the long-query path (afp_match_long.cu): writes its rows,
 // row count and, in publish mode, its candidate list.  a.hist / a.filt / a.hist_len / a.bias are
 // the mode pass's per-CTA histograms (zeroed; left zeroed), c->lg_ctas CTAs of them.

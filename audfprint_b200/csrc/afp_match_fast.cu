@@ -567,9 +567,6 @@ __global__ void __launch_bounds__(MT) afp_match_fast_kernel(MatchArgs a) {
 
 }  // namespace
 
-cudaError_t afp_launch_match_fast(const MatchArgs& a, int nctas, cudaStream_t stream) {
-  cudaError_t e = cudaFuncSetAttribute(afp_match_fast_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FAST_SMEM);
-  if (e != cudaSuccess) return e;
-  afp_match_fast_kernel<<<nctas, MT, FAST_SMEM, stream>>>(a);
-  return cudaGetLastError();
+int afp_launch_match_fast(afp_ctx* c, const MatchArgs& a, int nctas) {
+  return afp_launch(c, afp_match_fast_kernel, nctas, MT, FAST_SMEM, a);
 }

@@ -172,83 +172,84 @@ int afp_match_long(afp_ctx* c, const MatchArgs& a0, int qi, int64_t q0, int64_t 
   MatchArgs a = a0;
   cudaStream_t st = c->stream;
   const int64_t nids = a.nids;
+  int rc;
   // ---- 1. rows sorted by (bucket, time)
-  AFP_CUDA(c, c->d_lg_key.reserve(sizeof(unsigned long long) * 2 * (size_t)nq));
-  unsigned long long* k1 = c->d_lg_key.as<unsigned long long>();
-  unsigned long long* k2 = k1 + nq;
-  long_keys_kernel<<<(unsigned)std::min<int64_t>((nq + 255) / 256, 4096), 256, 0, st>>>(
-      a.q + 2 * q0, nq, (1u << a.hashbits) - 1u, k1);
-  AFP_CUDA(c, cudaGetLastError());
-  size_t tmp1 = 0, tmp2 = 0;
-  AFP_CUDA(c, cub::DeviceRadixSort::SortKeys(nullptr, tmp1, k1, k2, (int)nq, 0, 32 + a.hashbits, st));
-  AFP_CUDA(c, cub::DeviceRadixSort::SortPairsDescending(nullptr, tmp2, (unsigned long long*)nullptr,
-                                                        (unsigned long long*)nullptr, (uint32_t*)nullptr,
-                                                        (uint32_t*)nullptr, (int)nids, 0, 64, st));
-  AFP_CUDA(c, c->d_lg_cub.reserve(std::max(tmp1, tmp2)));
-  AFP_CUDA(c, cub::DeviceRadixSort::SortKeys(c->d_lg_cub.p, tmp1, k1, k2, (int)nq, 0, 32 + a.hashbits, st));
+  unsigned long long *k1 = nullptr, *k2 = nullptr;
+  if ((rc = afp_carve(c, c->d_lg_key, [&](Carver& k) {
+         k1 = k.take<unsigned long long>(nq);
+         k2 = k.take<unsigned long long>(nq);
+       })) ||
+      (rc = afp_launch(c, long_keys_kernel, (unsigned)std::min<int64_t>((nq + 255) / 256, 4096), 256, 0, a.q + 2 * q0,
+                       nq, (1u << a.hashbits) - 1u, k1)) ||
+      (rc = cub_call(c, [&](void* t, size_t& b) {
+         return cub::DeviceRadixSort::SortKeys(t, b, k1, k2, (int)nq, 0, 32 + a.hashbits, st);
+       })))
+    return rc;
   // ---- 2. raw counts
-  AFP_CUDA(c, c->d_lg_id.reserve((sizeof(unsigned) + sizeof(int32_t)) * (size_t)nids + 64));
-  unsigned* cnt = c->d_lg_id.as<unsigned>();
-  int32_t* slot = reinterpret_cast<int32_t*>(cnt + nids);
+  unsigned* cnt = nullptr;
+  int32_t* slot = nullptr;
+  if ((rc = afp_carve(c, c->d_lg_id, [&](Carver& k) {
+         cnt = k.take<unsigned>(nids);
+         slot = k.take<int32_t>(nids);
+       })))
+    return rc;
   unsigned* nd_na = c->d_tmp.as<unsigned>();          // (afp_match_batch reserved nqueries + 8 ints)
   AFP_CUDA(c, cudaMemsetAsync(cnt, 0, sizeof(unsigned) * (size_t)nids, st));
   AFP_CUDA(c, cudaMemsetAsync(slot, 0xff, sizeof(int32_t) * (size_t)nids, st));
   AFP_CUDA(c, cudaMemsetAsync(nd_na, 0, 2 * sizeof(unsigned), st));
   const unsigned pgrid = (unsigned)std::min<int64_t>((nq + LT / 32 - 1) / (LT / 32), (int64_t)c->num_sms * 16);
-  long_probe_kernel<0><<<pgrid, LT, 0, st>>>(a, k2, nq, cnt, nullptr, nullptr, nullptr, nullptr);
-  AFP_CUDA(c, cudaGetLastError());
+  if ((rc = afp_launch(c, long_probe_kernel<0>, pgrid, LT, 0, a, k2, nq, cnt, nullptr, nullptr, nullptr, nullptr)))
+    return rc;
   // ---- 3. ranking: (weight desc, id desc)
-  AFP_CUDA(c, c->d_lg_w.reserve((2 * sizeof(unsigned long long) + 2 * sizeof(uint32_t)) * (size_t)nids));
-  unsigned long long* w1 = c->d_lg_w.as<unsigned long long>();
-  unsigned long long* w2 = w1 + nids;
-  uint32_t* i1 = reinterpret_cast<uint32_t*>(w2 + nids);
-  uint32_t* i2 = i1 + nids;
-  long_weights_kernel<<<(unsigned)std::min<int64_t>((nids + 255) / 256, 2048), 256, 0, st>>>(a, cnt, w1, i1, nd_na);
-  AFP_CUDA(c, cudaGetLastError());
-  AFP_CUDA(c, cub::DeviceRadixSort::SortPairsDescending(c->d_lg_cub.p, tmp2, w1, w2, i1, i2, (int)nids, 0, 64, st));
+  unsigned long long *w1 = nullptr, *w2 = nullptr;
+  uint32_t *i1 = nullptr, *i2 = nullptr;
   unsigned h[2];
-  AFP_CUDA(c, cudaMemcpyAsync(h, nd_na, sizeof(h), cudaMemcpyDeviceToHost, st));
-  AFP_CUDA(c, cudaStreamSynchronize(st));
+  if ((rc = afp_carve(c, c->d_lg_w, [&](Carver& k) {
+         w1 = k.take<unsigned long long>(nids);
+         w2 = k.take<unsigned long long>(nids);
+         i1 = k.take<uint32_t>(nids);
+         i2 = k.take<uint32_t>(nids);
+       })) ||
+      (rc = afp_launch(c, long_weights_kernel, (unsigned)std::min<int64_t>((nids + 255) / 256, 2048), 256, 0, a, cnt,
+                       w1, i1, nd_na)) ||
+      (rc = cub_call(c, [&](void* t, size_t& b) {
+         return cub::DeviceRadixSort::SortPairsDescending(t, b, w1, w2, i1, i2, (int)nids, 0, 64, st);
+       })) ||
+      (rc = afp_read_back(c, h, nd_na, 2)))
+    return rc;
   const int ndist = (int)h[0], nabove = (int)h[1];
   const int ncand = a.publish ? std::min(ndist, a.sdepth) : std::min(nabove, a.sdepth);
-  c->launches += 5;
   // ---- 4. candidate segments and their hits
   const int slot_cap = std::max(1, std::min(a.maxalign + 1, a.row_cap));
-  AFP_CUDA(c, c->d_lg_cand.reserve(sizeof(int64_t) * (size_t)(ncand + 1) +
-                                   sizeof(int32_t) * (size_t)(3 * ncand + 4) +
-                                   sizeof(int32_t) * 7 * (size_t)ncand * slot_cap));
-  int64_t* seg = c->d_lg_cand.as<int64_t>();
-  int32_t* seglen = reinterpret_cast<int32_t*>(seg + ncand + 1);
-  unsigned* cur = reinterpret_cast<unsigned*>(seglen + ncand + 1);
-  int32_t* ccnt = reinterpret_cast<int32_t*>(cur + ncand + 1);
-  int32_t* crows = ccnt + ncand + 1;
+  int64_t* seg = nullptr;
+  int32_t *seglen = nullptr, *ccnt = nullptr, *crows = nullptr;
+  unsigned* cur = nullptr;
+  if ((rc = afp_carve(c, c->d_lg_cand, [&](Carver& k) {
+         seg = k.take<int64_t>(ncand + 1);
+         seglen = k.take<int32_t>(ncand + 1);
+         cur = k.take<unsigned>(ncand + 1);
+         ccnt = k.take<int32_t>(ncand + 1);
+         crows = k.take<int32_t>(7 * (int64_t)ncand * slot_cap);
+       })))
+    return rc;
   if (ncand > 0) {
-    long_cands_kernel<<<(ncand + 255) / 256, 256, 0, st>>>(a, qi, ncand, w2, i2, cnt, slot, seglen);
-    AFP_CUDA(c, cudaGetLastError());
-    int rc;
-    if ((rc = afp_launch_scan_i32_to_i64(c, seglen, seg, ncand))) return rc;
     int64_t nseg = 0;
-    AFP_CUDA(c, cudaMemcpyAsync(&nseg, seg + ncand, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    AFP_CUDA(c, cudaStreamSynchronize(st));
+    if ((rc = afp_launch(c, long_cands_kernel, (ncand + 255) / 256, 256, 0, a, qi, ncand, w2, i2, cnt, slot, seglen)) ||
+        (rc = afp_launch_scan_i32_to_i64(c, seglen, seg, ncand)) || (rc = afp_read_back(c, &nseg, seg + ncand, 1)))
+      return rc;
     AFP_CUDA(c, c->d_lg_dts.reserve(sizeof(uint32_t) * (size_t)(nseg + 1)));
     uint32_t* dts = c->d_lg_dts.as<uint32_t>();
     AFP_CUDA(c, cudaMemsetAsync(cur, 0, sizeof(unsigned) * (size_t)ncand, st));
-    if (nseg > 0) {
-      long_probe_kernel<1><<<pgrid, LT, 0, st>>>(a, k2, nq, nullptr, slot, seg, cur, dts);
-      AFP_CUDA(c, cudaGetLastError());
-    }
+    if (nseg > 0 && (rc = afp_launch(c, long_probe_kernel<1>, pgrid, LT, 0, a, k2, nq, nullptr, slot, seg, cur, dts)))
+      return rc;
     // ---- 5. modes, one CTA per candidate; each rank's rows go to a slot of its own
     MatchArgs am = a;
     am.rows = crows;
     am.row_cap = slot_cap;
-    const int grid = std::min(ncand, c->lg_ctas);
-    long_modes_kernel<<<grid, MT, 0, st>>>(am, ncand, i2, seglen, seg, dts, ccnt);
-    AFP_CUDA(c, cudaGetLastError());
-    c->launches += 4;
+    if ((rc = afp_launch(c, long_modes_kernel, std::min(ncand, c->lg_ctas), MT, 0, am, ncand, i2, seglen, seg, dts,
+                         ccnt)))
+      return rc;
   }
   // ---- 6. rows in rank order, end-of-query counts
-  long_rows_kernel<<<1, MT, 0, st>>>(a, qi, ncand, slot_cap, crows, ccnt, nabove);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
-  return AFP_OK;
+  return afp_launch(c, long_rows_kernel, 1, MT, 0, a, qi, ncand, slot_cap, crows, ccnt, nabove);
 }

@@ -280,35 +280,6 @@ unsigned grid_for(int64_t n, int threads) {
   return (unsigned)std::max<int64_t>(1, std::min<int64_t>((n + threads - 1) / threads, 132 * 32));
 }
 
-// carve consecutive 16-byte-aligned arrays out of one buffer
-struct Carver {
-  char* p;
-  template <class T> T* take(int64_t n) {
-    T* r = reinterpret_cast<T*>(p);
-    p += ((size_t)std::max<int64_t>(n, 1) * sizeof(T) + 15) & ~(size_t)15;
-    return r;
-  }
-};
-template <class T> size_t carve_bytes(int64_t n) { return ((size_t)std::max<int64_t>(n, 1) * sizeof(T) + 15) & ~(size_t)15; }
-
-// two-phase CUB call with the options workspace's temp buffer
-template <class F>
-int cub_call(afp_ctx* c, F f) {
-  size_t bytes = 0;
-  AFP_CUDA(c, f(nullptr, bytes));
-  AFP_CUDA(c, c->d_op_cub.reserve(bytes + 16));
-  AFP_CUDA(c, f(c->d_op_cub.p, bytes));
-  c->launches++;
-  return AFP_OK;
-}
-
-template <class T>
-int read_back(afp_ctx* c, const T* d, T* h, size_t n = 1) {
-  AFP_CUDA(c, cudaMemcpyAsync(h, d, sizeof(T) * n, cudaMemcpyDeviceToHost, c->stream));
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
-  return AFP_OK;
-}
-
 // The finish on the ranking afp_match_batch left in the context (publish mode).  On a shard
 // (qmax_shard != nullptr): every published candidate is finished, the key width comes from the
 // caller's per-query largest qtime over ALL shards, and quantile failures go to qfail.
@@ -324,27 +295,32 @@ int finish_options(afp_ctx* c, const int32_t* dq, int nq, int64_t nrows, int64_t
   const int32_t* cnt = c->d_mcand_cnt.as<int32_t>();
   int rc;
   // ---- 1. slots, segments, sorted lookup ids
-  AFP_CUDA(c, c->d_op_slot.reserve(2 * carve_bytes<int64_t>(nslot + 1) + 4 * carve_bytes<uint32_t>(nslot) +
-                                   carve_bytes<int32_t>(nq + 1) + carve_bytes<unsigned>(nslot) +
-                                   carve_bytes<int>(nq) + carve_bytes<int>(4) + carve_bytes<unsigned long long>(nq + 1)));
-  Carver cs{c->d_op_slot.as<char>()};
-  int64_t* seglen = cs.take<int64_t>(nslot + 1);
-  int64_t* segoff = cs.take<int64_t>(nslot + 1);
-  uint32_t* lkey = cs.take<uint32_t>(nslot);
-  uint32_t* lkey2 = cs.take<uint32_t>(nslot);
-  int32_t* lval = cs.take<int32_t>(nslot);
-  int32_t* lval2 = cs.take<int32_t>(nslot);
-  int32_t* loff = cs.take<int32_t>(nq + 1);
-  unsigned* cur = cs.take<unsigned>(nslot);
-  int* qmax = cs.take<int>(nq);
-  int* err = cs.take<int>(4);
-  unsigned long long* qcnt = cs.take<unsigned long long>(nq + 1);
+  int64_t *seglen, *segoff;
+  uint32_t *lkey, *lkey2;
+  int32_t *lval, *lval2, *loff;
+  unsigned* cur;
+  int *qmax, *err;
+  unsigned long long* qcnt;
+  if ((rc = afp_carve(c, c->d_op_slot, [&](Carver& k) {
+         seglen = k.take<int64_t>(nslot + 1);
+         segoff = k.take<int64_t>(nslot + 1);
+         lkey = k.take<uint32_t>(nslot);
+         lkey2 = k.take<uint32_t>(nslot);
+         lval = k.take<int32_t>(nslot);
+         lval2 = k.take<int32_t>(nslot);
+         loff = k.take<int32_t>(nq + 1);
+         cur = k.take<unsigned>(nslot);
+         qmax = k.take<int>(nq);
+         err = k.take<int>(4);
+         qcnt = k.take<unsigned long long>(nq + 1);
+       })))
+    return rc;
   AFP_CUDA(c, cudaMemsetAsync(cur, 0, sizeof(unsigned) * (size_t)std::max<int64_t>(nslot, 1), st));
   AFP_CUDA(c, cudaMemsetAsync(err, 0, sizeof(int) * 4, st));
   AFP_CUDA(c, cudaMemsetAsync(qcnt, 0, sizeof(unsigned long long) * (size_t)(nq + 1), st));
-  opt_slots_kernel<<<grid_for(nslot + 1, OT), OT, 0, st>>>(cand, cnt, nq, sd, thresh, shard, seglen, lkey, lval, loff, qmax);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
+  if ((rc = afp_launch(c, opt_slots_kernel, grid_for(nslot + 1, OT), OT, 0, cand, cnt, nq, sd, thresh, shard, seglen,
+                       lkey, lval, loff, qmax)))
+    return rc;
   if ((rc = cub_call(c, [&](void* t, size_t& b) {
          return cub::DeviceScan::ExclusiveSum(t, b, seglen, segoff, (int)(nslot + 1), st);
        })))
@@ -355,32 +331,29 @@ int finish_options(afp_ctx* c, const int32_t* dq, int nq, int64_t nrows, int64_t
        })))
     return rc;
   int64_t nh = 0;
-  if ((rc = read_back(c, segoff + nslot, &nh))) return rc;
+  if ((rc = afp_read_back(c, &nh, segoff + nslot, 1))) return rc;
   if (nh >= ((int64_t)1 << 31)) AFP_FAIL(c, AFP_ERR_UNSUPPORTED, "the candidates' hits of one call reach 2^31");
   // ---- 2. probe: the routed candidates' hits into their segments
-  AFP_CUDA(c, c->d_op_hit.reserve(2 * carve_bytes<int32_t>(nh) + 2 * carve_bytes<unsigned long long>(nh) +
-                                  carve_bytes<int32_t>(nh) + 2 * carve_bytes<int32_t>(nh + 1)));
-  Carver ch{c->d_op_hit.as<char>()};
-  int32_t* dt = ch.take<int32_t>(nh);
-  int32_t* dt2 = ch.take<int32_t>(nh);
-  unsigned long long* pay = ch.take<unsigned long long>(nh);
-  unsigned long long* pay2 = ch.take<unsigned long long>(nh);
-  int32_t* hseg = ch.take<int32_t>(nh);
-  int32_t* flag = ch.take<int32_t>(nh + 1);
-  int32_t* pos = ch.take<int32_t>(nh + 1);
-  if (nrows > 0) {
-    opt_probe_kernel<<<grid_for(nrows, OT / 32), OT, 0, st>>>(
-        dq, nrows, c->d_qoff.as<int64_t>(), nq, c->tab.table.as<uint32_t>(), c->tab.counts.as<int32_t>(),
-        c->tab.hashbits, c->tab.depth, c->tab.maxtimebits, std::max<int64_t>(c->tab.nids, 1), sd, lkey2, lval2, segoff,
-        cur, dt, pay, hseg, qmax, err);
-    AFP_CUDA(c, cudaGetLastError());
-    c->launches++;
-  }
-  if (nslot > 0) {
-    opt_fill_check_kernel<<<grid_for(nslot, OT), OT, 0, st>>>(seglen, cur, nslot, err);
-    AFP_CUDA(c, cudaGetLastError());
-    c->launches++;
-  }
+  int32_t *dt, *dt2, *hseg, *flag, *pos;
+  unsigned long long *pay, *pay2;
+  if ((rc = afp_carve(c, c->d_op_hit, [&](Carver& k) {
+         dt = k.take<int32_t>(nh);
+         dt2 = k.take<int32_t>(nh);
+         pay = k.take<unsigned long long>(nh);
+         pay2 = k.take<unsigned long long>(nh);
+         hseg = k.take<int32_t>(nh);
+         flag = k.take<int32_t>(nh + 1);
+         pos = k.take<int32_t>(nh + 1);
+       })))
+    return rc;
+  if (nrows > 0 &&
+      (rc = afp_launch(c, opt_probe_kernel, grid_for(nrows, OT / 32), OT, 0, dq, nrows, c->d_qoff.as<int64_t>(), nq,
+                       c->tab.table.as<uint32_t>(), c->tab.counts.as<int32_t>(), c->tab.hashbits, c->tab.depth,
+                       c->tab.maxtimebits, std::max<int64_t>(c->tab.nids, 1), sd, lkey2, lval2, segoff, cur, dt, pay,
+                       hseg, qmax, err)))
+    return rc;
+  if (nslot > 0 && (rc = afp_launch(c, opt_fill_check_kernel, grid_for(nslot, OT), OT, 0, seglen, cur, nslot, err)))
+    return rc;
   // ---- 3. every segment by dtime
   if (nh > 0 && (rc = cub_call(c, [&](void* t, size_t& b) {
                    return cub::DeviceSegmentedSort::SortPairs(t, b, dt, dt2, pay, pay2, (int)nh, (int)nslot, segoff,
@@ -392,66 +365,68 @@ int finish_options(afp_ctx* c, const int32_t* dq, int nq, int64_t nrows, int64_t
   const int64_t* roff = c->d_mrow_off.as<int64_t>();
   const int64_t nsrc = exact ? nh : napprox;
   if (!exact) {
-    AFP_CUDA(c, c->d_op_mode.reserve(2 * carve_bytes<int32_t>(nsrc + 1)));
-    flag = c->d_op_mode.as<int32_t>();
-    pos = flag + ((carve_bytes<int32_t>(nsrc + 1)) / sizeof(int32_t));
-    opt_rowflags_kernel<<<grid_for(nsrc + 1, OT), OT, 0, st>>>(approx, nsrc, roff, nq, cnt, sd, shard, flag);
+    if ((rc = afp_carve(c, c->d_op_mode, [&](Carver& k) {
+           flag = k.take<int32_t>(nsrc + 1);
+           pos = k.take<int32_t>(nsrc + 1);
+         })))
+      return rc;
+    rc = afp_launch(c, opt_rowflags_kernel, grid_for(nsrc + 1, OT), OT, 0, approx, nsrc, roff, nq, cnt, sd, shard, flag);
   } else {
-    opt_modes_kernel<<<grid_for(nsrc + 1, OT), OT, 0, st>>>(dt2, hseg, segoff, nsrc, thresh, flag);
+    rc = afp_launch(c, opt_modes_kernel, grid_for(nsrc + 1, OT), OT, 0, dt2, hseg, segoff, nsrc, thresh, flag);
   }
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
+  if (rc) return rc;
   if ((rc = cub_call(c, [&](void* t, size_t& b) {
          return cub::DeviceScan::ExclusiveSum(t, b, flag, pos, (int)(nsrc + 1), st);
        })))
     return rc;
   int h_m[2] = {0, 0};
-  AFP_CUDA(c, cudaMemcpyAsync(&h_m[0], pos + nsrc, sizeof(int), cudaMemcpyDeviceToHost, st));
-  if ((rc = read_back(c, err, &h_m[1]))) return rc;
+  if ((rc = afp_read_back(c, &h_m[0], pos + nsrc, 1, &h_m[1], err, 1))) return rc;
   if (h_m[1]) AFP_FAIL(c, AFP_ERR_STATE, "a candidate's hits differ from its raw count (table changed during the call?)");
   const int nm = h_m[0];
   // ---- 5. supports
-  AFP_CUDA(c, c->d_op_sup.reserve(carve_bytes<int32_t>(nm) * 8 + 2 * carve_bytes<int64_t>(nm + 1) +
-                                  carve_bytes<int32_t>(nm + 1) * 2 + carve_bytes<int64_t>(nm)));
-  Carver cm{c->d_op_sup.as<char>()};
-  int32_t* midx = cm.take<int32_t>(nm);
-  int32_t* mslot = cm.take<int32_t>(nm);
-  int32_t* mdt = cm.take<int32_t>(nm);
-  int32_t* mcnt = cm.take<int32_t>(nm);
-  int32_t* mtlo = cm.take<int32_t>(nm);
-  int32_t* mthi = cm.take<int32_t>(nm);
-  int32_t* keep = cm.take<int32_t>(nm + 1);
-  int32_t* kpos = cm.take<int32_t>(nm + 1);
-  int64_t* mlo = cm.take<int64_t>(nm);
-  int64_t* slen = cm.take<int64_t>(nm + 1);
-  int64_t* soff = cm.take<int64_t>(nm + 1);
-  if (nsrc > 0) {
-    opt_scatter_kernel<<<grid_for(nsrc, OT), OT, 0, st>>>(flag, pos, nsrc, midx);
-    AFP_CUDA(c, cudaGetLastError());
-    c->launches++;
-  }
-  opt_support_kernel<<<grid_for(nm + 1, OT), OT, 0, st>>>(midx, nm, exact, dt2, hseg, segoff, approx, roff, nq, sd,
-                                                          window, mslot, mdt, mlo, slen);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
+  int32_t *midx, *mslot, *mdt, *mcnt, *mtlo, *mthi, *keep, *kpos;
+  int64_t *mlo, *slen, *soff;
+  if ((rc = afp_carve(c, c->d_op_sup, [&](Carver& k) {
+         midx = k.take<int32_t>(nm);
+         mslot = k.take<int32_t>(nm);
+         mdt = k.take<int32_t>(nm);
+         mcnt = k.take<int32_t>(nm);
+         mtlo = k.take<int32_t>(nm);
+         mthi = k.take<int32_t>(nm);
+         keep = k.take<int32_t>(nm + 1);
+         kpos = k.take<int32_t>(nm + 1);
+         mlo = k.take<int64_t>(nm);
+         slen = k.take<int64_t>(nm + 1);
+         soff = k.take<int64_t>(nm + 1);
+       })))
+    return rc;
+  if (nsrc > 0 && (rc = afp_launch(c, opt_scatter_kernel, grid_for(nsrc, OT), OT, 0, flag, pos, nsrc, midx))) return rc;
+  if ((rc = afp_launch(c, opt_support_kernel, grid_for(nm + 1, OT), OT, 0, midx, nm, exact, dt2, hseg, segoff, approx,
+                       roff, nq, sd, window, mslot, mdt, mlo, slen)))
+    return rc;
   if ((rc = cub_call(c, [&](void* t, size_t& b) {
          return cub::DeviceScan::ExclusiveSum(t, b, slen, soff, nm + 1, st);
        })))
     return rc;
   int64_t ns = 0;
-  if ((rc = read_back(c, soff + nm, &ns))) return rc;
+  if ((rc = afp_read_back(c, &ns, soff + nm, 1))) return rc;
   if (ns >= ((int64_t)1 << 31)) AFP_FAIL(c, AFP_ERR_UNSUPPORTED, "the mode supports of one call reach 2^31 entries");
-  AFP_CUDA(c, c->d_op_key.reserve(exact ? 2 * carve_bytes<unsigned long long>(ns) : 1));
-  AFP_CUDA(c, c->d_op_tq.reserve(trange ? 2 * carve_bytes<int32_t>(ns) : 1));
-  unsigned long long* pk = exact ? c->d_op_key.as<unsigned long long>() : nullptr;
-  unsigned long long* pk2 = exact ? pk + carve_bytes<unsigned long long>(ns) / sizeof(unsigned long long) : nullptr;
-  int32_t* tq = trange ? c->d_op_tq.as<int32_t>() : nullptr;
-  int32_t* tq2 = trange ? tq + carve_bytes<int32_t>(ns) / sizeof(int32_t) : nullptr;
+  unsigned long long *pk = nullptr, *pk2 = nullptr;
+  int32_t *tq = nullptr, *tq2 = nullptr;
+  if (exact && (rc = afp_carve(c, c->d_op_key, [&](Carver& k) {
+                  pk = k.take<unsigned long long>(ns);
+                  pk2 = k.take<unsigned long long>(ns);
+                })))
+    return rc;
+  if (trange && (rc = afp_carve(c, c->d_op_tq, [&](Carver& k) {
+                   tq = k.take<int32_t>(ns);
+                   tq2 = k.take<int32_t>(ns);
+                 })))
+    return rc;
   if (ns > 0) {
-    opt_gather_kernel<<<grid_for(ns, OT), OT, 0, st>>>(soff, nm, mlo, mslot, sd, pay2, shard ? qmax_shard : qmax,
-                                                        br, pk, tq);
-    AFP_CUDA(c, cudaGetLastError());
-    c->launches++;
+    if ((rc = afp_launch(c, opt_gather_kernel, grid_for(ns, OT), OT, 0, soff, nm, mlo, mslot, sd, pay2,
+                         shard ? qmax_shard : qmax, br, pk, tq)))
+      return rc;
     if (exact && (rc = cub_call(c, [&](void* t, size_t& b) {
                     return cub::DeviceSegmentedSort::SortKeys(t, b, pk, pk2, (int)ns, nm, soff, soff + 1, st);
                   })))
@@ -462,26 +437,22 @@ int finish_options(afp_ctx* c, const int32_t* dq, int nq, int64_t nrows, int64_t
       return rc;
   }
   // ---- 6. counts, quantiles, rows
-  opt_stats_kernel<<<grid_for(nm + 1, OT / 32), OT, 0, st>>>(soff, nm, pk2, tq2, thresh, quant, mslot, sd, mcnt, mtlo,
-                                                             mthi, keep, err + 1, qfail);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
+  if ((rc = afp_launch(c, opt_stats_kernel, grid_for(nm + 1, OT / 32), OT, 0, soff, nm, pk2, tq2, thresh, quant, mslot,
+                       sd, mcnt, mtlo, mthi, keep, err + 1, qfail)))
+    return rc;
   if ((rc = cub_call(c, [&](void* t, size_t& b) {
          return cub::DeviceScan::ExclusiveSum(t, b, keep, kpos, nm + 1, st);
        })))
     return rc;
   int h_r[2] = {0, 0};
-  AFP_CUDA(c, cudaMemcpyAsync(&h_r[0], kpos + nm, sizeof(int), cudaMemcpyDeviceToHost, st));
-  if ((rc = read_back(c, err + 1, &h_r[1]))) return rc;
+  if ((rc = afp_read_back(c, &h_r[0], kpos + nm, 1, &h_r[1], err + 1, 1))) return rc;
   if (h_r[1]) AFP_FAIL(c, AFP_ERR_INDEX, "time_quantile index outside a support (IndexError)");
   const int nr = h_r[0];
   AFP_CUDA(c, c->d_op_rows.reserve(sizeof(int32_t) * 7 * (size_t)(nr + 1)));
-  if (nm > 0) {
-    opt_rows_kernel<<<grid_for(nm, OT), OT, 0, st>>>(nm, keep, kpos, midx, mslot, mdt, mcnt, mtlo, mthi, exact, trange,
-                                                     cand, sd, approx, c->d_op_rows.as<int32_t>(), qcnt);
-    AFP_CUDA(c, cudaGetLastError());
-    c->launches++;
-  }
+  if (nm > 0 &&
+      (rc = afp_launch(c, opt_rows_kernel, grid_for(nm, OT), OT, 0, nm, keep, kpos, midx, mslot, mdt, mcnt, mtlo, mthi,
+                       exact, trange, cand, sd, approx, c->d_op_rows.as<int32_t>(), qcnt)))
+    return rc;
   static_assert(sizeof(unsigned long long) == sizeof(int64_t), "row counts scan in place of int64 offsets");
   if ((rc = cub_call(c, [&](void* t, size_t& b) {
          return cub::DeviceScan::ExclusiveSum(t, b, reinterpret_cast<int64_t*>(qcnt), c->d_mrow_off.as<int64_t>(),
@@ -581,13 +552,10 @@ extern "C" int afp_match_options_shard_rank(afp_ctx* c, const int32_t* q_rows, i
   const int64_t nrows = nqueries ? q_offsets[nqueries] : 0;
   if (nqueries > 0) {
     AFP_CUDA(c, cudaMemsetAsync(qmax_dev, 0, sizeof(int32_t) * (size_t)nqueries, c->stream));
-    if (nrows > 0) {
-      opt_shard_qmax_kernel<<<grid_for(nrows, OT), OT, 0, c->stream>>>(
-          dq, nrows, c->d_qoff.as<int64_t>(), nqueries, c->tab.counts.as<int32_t>(), c->tab.hashbits, c->tab.depth,
-          qmax_dev);
-      AFP_CUDA(c, cudaGetLastError());
-      c->launches++;
-    }
+    if (nrows > 0 &&
+        (rc = afp_launch(c, opt_shard_qmax_kernel, grid_for(nrows, OT), OT, 0, dq, nrows, c->d_qoff.as<int64_t>(),
+                         nqueries, c->tab.counts.as<int32_t>(), c->tab.hashbits, c->tab.depth, qmax_dev)))
+      return rc;
   }
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));       // qmax is the caller's to all-reduce now
   c->match_total_rows = -1;                             // nothing to fetch or pack before the finish

@@ -101,29 +101,21 @@ extern "C" int afp_pcm_frontend(afp_ctx* c, const int16_t* pcm, int pcm_on_host,
   const int64_t n_out = (nframes * up + down - 1) / down;                // ceil, as resample_poly
   if (nout) *nout = n_out;
   if (n_out == 0) return AFP_OK;
-  const int16_t* dpcm = pcm;
-  if (pcm_on_host) {
-    AFP_CUDA(c, c->d_pcm_stage.reserve(sizeof(int16_t) * (size_t)nframes * channels + 16));
-    AFP_CUDA(c, cudaMemcpyAsync(c->d_pcm_stage.p, pcm, sizeof(int16_t) * (size_t)nframes * channels,
-                                cudaMemcpyHostToDevice, c->stream));
-    dpcm = c->d_pcm_stage.as<int16_t>();
-  }
-  const double* dtaps = nullptr;
-  if (resample) {
-    AFP_CUDA(c, c->d_tmp.reserve(sizeof(double) * (size_t)ntaps + sizeof(float) * (size_t)(out_on_host ? n_out : 0) + 64));
-    AFP_CUDA(c, cudaMemcpyAsync(c->d_tmp.p, taps, sizeof(double) * (size_t)ntaps, cudaMemcpyHostToDevice, c->stream));
-    dtaps = c->d_tmp.as<double>();
-  } else {
-    AFP_CUDA(c, c->d_tmp.reserve(sizeof(float) * (size_t)(out_on_host ? n_out : 0) + 64));
-  }
+  const int16_t* dpcm = nullptr;
+  double* dtaps = nullptr;
   float* dout = out;
-  if (out_on_host) dout = reinterpret_cast<float*>(c->d_tmp.as<char>() + (resample ? ((sizeof(double) * (size_t)ntaps + 15) & ~(size_t)15) : 0));
-  afp_pcm_frontend_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, c->stream>>>(dpcm, nframes, channels, up, down,
-                                                                                 dtaps, (ntaps - 1) / 2, dout, n_out);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
-  if (out_on_host)
-    AFP_CUDA(c, cudaMemcpyAsync(out, dout, sizeof(float) * (size_t)n_out, cudaMemcpyDeviceToHost, c->stream));
+  int rc;
+  if ((rc = afp_stage(c, c->d_pcm_stage, pcm, (size_t)nframes * channels, pcm_on_host, &dpcm)) ||
+      (rc = afp_carve(c, c->d_tmp, [&](Carver& k) {
+         dtaps = resample ? k.take<double>(ntaps) : nullptr;
+         if (out_on_host) dout = k.take<float>(n_out);
+       })))
+    return rc;
+  if (resample) AFP_CUDA(c, afp_copy_in(c, dtaps, taps, (size_t)ntaps, 1));
+  if ((rc = afp_launch(c, afp_pcm_frontend_kernel, (unsigned)((n_out + 255) / 256), 256, 0, dpcm, nframes, channels,
+                       up, down, dtaps, (ntaps - 1) / 2, dout, n_out)))
+    return rc;
+  if (out_on_host) AFP_CUDA(c, afp_copy_out(c, out, dout, (size_t)n_out, 1));
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));
   c->batch_valid = false;     // the PCM staging buffer of the last batch may have been reused
   return AFP_OK;
@@ -189,27 +181,27 @@ extern "C" int afp_pcm_frontend_batch(afp_ctx* c, const int16_t* pcm, int pcm_on
     for (int f = 0; f < nfiles; ++f) out_lengths[f] = d[f].nout;
   if (!out || blocks == 0) return AFP_OK;                                 // sizing call, or nothing to compute
   AFP_CUDA(c, cudaSetDevice(c->device));
-  const int16_t* dpcm = pcm;
-  if (pcm_on_host) {
-    AFP_CUDA(c, c->d_pcm_stage.reserve(sizeof(int16_t) * (size_t)pcm_len + 16));
-    AFP_CUDA(c, cudaMemcpyAsync(c->d_pcm_stage.p, pcm, sizeof(int16_t) * (size_t)pcm_len, cudaMemcpyHostToDevice,
-                                c->stream));
-    dpcm = c->d_pcm_stage.as<int16_t>();
-    c->batch_valid = false;   // the PCM staging buffer of the last fingerprint batch is overwritten
-  }
+  const int16_t* dpcm = nullptr;
+  int rc = afp_stage(c, c->d_pcm_stage, pcm, (size_t)pcm_len, pcm_on_host, &dpcm);
+  if (rc) return rc;
+  if (pcm_on_host) c->batch_valid = false;   // the PCM staging buffer of the last fingerprint batch is overwritten
   // descriptors and every distinct design's taps in one upload
-  const size_t desc_bytes = ((sizeof(PcmFileDesc) * (size_t)nfiles + 15) & ~(size_t)15);
-  const size_t tap_bytes = npairs > 0 ? sizeof(double) * (size_t)tap_offsets[npairs] : 0;
-  std::vector<char> h(desc_bytes + tap_bytes);
+  const int64_t ntaps = npairs > 0 ? tap_offsets[npairs] : 0;
+  PcmFileDesc* dd = nullptr;
+  double* dtaps = nullptr;
+  size_t desc_bytes = 0;
+  if ((rc = afp_carve(c, c->d_tmp, [&](Carver& k) {
+         dd = k.take<PcmFileDesc>(nfiles);
+         desc_bytes = k.bytes;
+         dtaps = k.take<double>(ntaps);
+       })))
+    return rc;
+  std::vector<char> h(desc_bytes + sizeof(double) * (size_t)ntaps);
   memcpy(h.data(), d.data(), sizeof(PcmFileDesc) * (size_t)nfiles);
-  if (tap_bytes) memcpy(h.data() + desc_bytes, taps, tap_bytes);
-  AFP_CUDA(c, c->d_tmp.reserve(h.size() + 64));
-  AFP_CUDA(c, cudaMemcpyAsync(c->d_tmp.p, h.data(), h.size(), cudaMemcpyHostToDevice, c->stream));
-  const PcmFileDesc* dd = c->d_tmp.as<PcmFileDesc>();
-  const double* dtaps = reinterpret_cast<const double*>(c->d_tmp.as<char>() + desc_bytes);
-  afp_pcm_frontend_batch_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(dpcm, dd, nfiles, dtaps, out);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
+  if (ntaps) memcpy(h.data() + desc_bytes, taps, sizeof(double) * (size_t)ntaps);
+  AFP_CUDA(c, afp_copy_in(c, reinterpret_cast<char*>(dd), h.data(), h.size(), 1));
+  if ((rc = afp_launch(c, afp_pcm_frontend_batch_kernel, (unsigned)blocks, 256, 0, dpcm, dd, nfiles, dtaps, out)))
+    return rc;
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));       // one synchronise for the whole list (`h` is pageable)
   return AFP_OK;
 }

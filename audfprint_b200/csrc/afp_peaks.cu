@@ -446,19 +446,13 @@ int afp_spread_peaks_impl(afp_ctx* c, const double* vector, int32_t n, const dou
   AFP_CUDA(c, cudaMemcpyAsync(d_vec, vector, sizeof(double) * nn, cudaMemcpyHostToDevice, c->stream));
   AFP_CUDA(c, cudaMemcpyAsync(d_tab, tab.data(), sizeof(double) * tab.size(), cudaMemcpyHostToDevice, c->stream));
   if (base) AFP_CUDA(c, cudaMemcpyAsync(d_base, base, sizeof(double) * nn, cudaMemcpyHostToDevice, c->stream));
-  const size_t smem = sizeof(int) * nn;
-  if (smem > 48 * 1024)
-    AFP_CUDA(c, cudaFuncSetAttribute(afp_spread_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  afp_spread_kernel<<<1, 256, smem, c->stream>>>(d_vec, n, d_tab, base ? d_base : nullptr, d_out);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
-  AFP_CUDA(c, cudaMemcpyAsync(out, d_out, sizeof(double) * nn, cudaMemcpyDeviceToHost, c->stream));
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));   // `tab` must outlive the copy
-  return AFP_OK;
+  const int rc = afp_launch(c, afp_spread_kernel, 1, 256, sizeof(int) * nn, d_vec, n, d_tab, base ? d_base : nullptr,
+                            d_out);
+  if (rc) return rc;
+  return afp_read_back(c, out, d_out, nn);   // also: `tab` outlives its copy
 }
 
 int afp_launch_peaks(afp_ctx* c, int item0, int nitems) {
-  if (nitems <= 0) return AFP_OK;
   PeakArgs a;
   a.items = c->d_items.as<ItemDesc>();
   a.stats = c->d_item_stats.as<ItemStats>();
@@ -483,34 +477,24 @@ int afp_launch_peaks(afp_ctx* c, int item0, int nitems) {
                                      cudaSharedmemCarveoutMaxShared));
     c->peaks_carveout_set = true;
   }
-  if (c->ap.spectrogram_fp32) afp_peaks_kernel<float><<<nitems, 32, 0, c->stream>>>(a);
-  else afp_peaks_kernel<double><<<nitems, 32, 0, c->stream>>>(a);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
-  return AFP_OK;
+  return c->ap.spectrogram_fp32 ? afp_launch(c, afp_peaks_kernel<float>, nitems, 32, 0, a)
+                                : afp_launch(c, afp_peaks_kernel<double>, nitems, 32, 0, a);
 }
 
 int afp_compact_peaks(afp_ctx* c, int shift) {
   // per-file counts of this shift -> offsets -> rows
   AFP_CUDA(c, c->d_tmp.reserve(sizeof(int32_t) * (size_t)(c->nfiles + 1)));
   AFP_CUDA(c, c->d_pk_off.reserve(sizeof(int64_t) * (size_t)(c->nfiles + 1)));
-  afp_gather_npeaks_kernel<<<(c->nfiles + 255) / 256, 256, 0, c->stream>>>(
-      c->d_item_npeaks.as<int32_t>(), c->nfiles, c->ap.shifts, shift, c->d_tmp.as<int32_t>());
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
-  int rc = afp_launch_scan_i32_to_i64(c, c->d_tmp.as<int32_t>(), c->d_pk_off.as<int64_t>(), c->nfiles);
-  if (rc) return rc;
   int64_t total = 0;
-  AFP_CUDA(c, cudaMemcpyAsync(&total, c->d_pk_off.as<int64_t>() + c->nfiles, sizeof(int64_t),
-                              cudaMemcpyDeviceToHost, c->stream));
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+  int rc;
+  if ((rc = afp_launch(c, afp_gather_npeaks_kernel, (c->nfiles + 255) / 256, 256, 0, c->d_item_npeaks.as<int32_t>(),
+                       c->nfiles, c->ap.shifts, shift, c->d_tmp.as<int32_t>())) ||
+      (rc = afp_launch_scan_i32_to_i64(c, c->d_tmp.as<int32_t>(), c->d_pk_off.as<int64_t>(), c->nfiles)) ||
+      (rc = afp_read_back(c, &total, c->d_pk_off.as<int64_t>() + c->nfiles, 1)))
+    return rc;
   AFP_CUDA(c, c->d_pk_rows.reserve(sizeof(int32_t) * 2 * (size_t)(total + 1)));
-  if (total > 0) {
-    afp_peaks_compact_kernel<<<c->nfiles, 256, 0, c->stream>>>(
-        c->d_items.as<ItemDesc>(), c->ap.shifts, shift, c->ap.maxpksperframe, c->d_pk_bin.as<uint8_t>(),
-        c->d_pk_cnt.as<uint8_t>(), c->d_pk_off.as<int64_t>(), c->d_pk_rows.as<int32_t>());
-    AFP_CUDA(c, cudaGetLastError());
-    c->launches++;
-  }
-  return AFP_OK;
+  if (total == 0) return AFP_OK;
+  return afp_launch(c, afp_peaks_compact_kernel, c->nfiles, 256, 0, c->d_items.as<ItemDesc>(), c->ap.shifts, shift,
+                    c->ap.maxpksperframe, c->d_pk_bin.as<uint8_t>(), c->d_pk_cnt.as<uint8_t>(),
+                    c->d_pk_off.as<int64_t>(), c->d_pk_rows.as<int32_t>());
 }

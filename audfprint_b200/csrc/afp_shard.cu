@@ -195,16 +195,16 @@ int afp_shard_pack(afp_ctx* c, int32_t row_cap, void* records_dev) {
   int* d_over = c->d_tmp.as<int>();
   AFP_CUDA(c, cudaMemsetAsync(d_over, 0, sizeof(int), c->stream));
   const bool fin = c->sopt.finished;             // an options finish: its packed rows and status
-  afp_shard_pack_kernel<<<c->match_nq, 64, 0, c->stream>>>(
-      c->d_mcand.as<double>(), c->d_mcand_cnt.as<int32_t>(), c->match_sdepth,
-      fin ? c->d_mrows_packed.as<int32_t>() : c->d_mrows.as<int32_t>(), c->d_mrow_cnt.as<int32_t>(),
-      c->match_row_cap, fin ? c->d_mrow_off.as<int64_t>() : nullptr, fin ? c->d_op_qfail.as<int32_t>() : nullptr,
-      row_cap, static_cast<unsigned char*>(records_dev), d_over);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
   int over = 0;
-  AFP_CUDA(c, cudaMemcpyAsync(&over, d_over, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+  int rc;
+  if ((rc = afp_launch(c, afp_shard_pack_kernel, c->match_nq, 64, 0, c->d_mcand.as<double>(),
+                       c->d_mcand_cnt.as<int32_t>(), c->match_sdepth,
+                       fin ? c->d_mrows_packed.as<int32_t>() : c->d_mrows.as<int32_t>(), c->d_mrow_cnt.as<int32_t>(),
+                       c->match_row_cap, fin ? c->d_mrow_off.as<int64_t>() : nullptr,
+                       fin ? c->d_op_qfail.as<int32_t>() : nullptr, row_cap, static_cast<unsigned char*>(records_dev),
+                       d_over)) ||
+      (rc = afp_read_back(c, &over, d_over, 1)))
+    return rc;
   if (over) AFP_FAIL(c, AFP_ERR_UNSUPPORTED, "row capacity exceeded: a shard produced more rows for one query than the record holds");
   return AFP_OK;
 }
@@ -232,16 +232,14 @@ int afp_shard_merge(afp_ctx* c, const void* gathered_dev, int32_t nshards, int32
   AFP_CUDA(c, c->d_tmp.reserve(sizeof(int32_t) * (size_t)(nqueries + 16)));
   int* d_err = c->d_tmp.as<int>() + nqueries + 8;
   AFP_CUDA(c, cudaMemsetAsync(d_err, 0, sizeof(int) * 3, c->stream));
-  afp_shard_merge_kernel<<<nqueries, MERGE_T, 0, c->stream>>>(static_cast<const unsigned char*>(gathered_dev), nshards,
-                                                             nqueries, search_depth, row_cap, c->d_mrows.as<int32_t>(),
-                                                             ocap, c->d_mrow_cnt.as<int32_t>(), d_err);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
   int64_t total = 0;
-  int rc = afp_finish_match_rows(c, nqueries, ocap, &total);
-  if (rc) return rc;
   int err[3] = {0, 0, 0};
-  AFP_CUDA(c, cudaMemcpy(err, d_err, sizeof(err), cudaMemcpyDeviceToHost));
+  int rc;
+  if ((rc = afp_launch(c, afp_shard_merge_kernel, nqueries, MERGE_T, 0, static_cast<const unsigned char*>(gathered_dev),
+                       nshards, nqueries, search_depth, row_cap, c->d_mrows.as<int32_t>(), ocap,
+                       c->d_mrow_cnt.as<int32_t>(), d_err)) ||
+      (rc = afp_finish_match_rows(c, nqueries, ocap, &total)) || (rc = afp_read_back(c, err, d_err, 3)))
+    return rc;
   if (err[0]) AFP_FAIL(c, AFP_ERR_INVALID, "shard records are inconsistent (a row's rank is outside its candidate list)");
   if (err[1]) AFP_FAIL(c, AFP_ERR_INDEX, "time_quantile index outside a support (IndexError)");
   if (err[2]) {

@@ -564,9 +564,9 @@ __global__ void afp_sgram_kernel(const ItemDesc* items, const ItemStats* stats, 
 
 int afp_launch_tile_table(afp_ctx* c) {
   if (c->nitems == 0 || c->tile_tag.is(c->d_tile_item)) return AFP_OK;   // already built for these items
-  afp_tile_table_kernel<<<c->nitems, 128, 0, c->stream>>>(c->d_items.as<ItemDesc>(), c->d_tile_item.as<int32_t>());
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
+  const int rc = afp_launch(c, afp_tile_table_kernel, c->nitems, 128, 0, c->d_items.as<ItemDesc>(),
+                            c->d_tile_item.as<int32_t>());
+  if (rc) return rc;
   c->tile_tag.set(c->d_tile_item);
   return AFP_OK;
 }
@@ -575,18 +575,14 @@ namespace {
 
 // One K1 instantiation: num_sms x its CTAs per SM, at most one CTA per tile.
 template <typename R, typename PcmT, bool WRITE_MAG>
-cudaError_t launch_k1(const StftArgs<R>& a, int num_sms, int64_t ntiles, cudaStream_t stream) {
-  constexpr size_t smem = k1_smem_bytes<R, PcmT>();
-  const int nctas = (int)std::min<int64_t>(ntiles, (int64_t)num_sms * K1Traits<R>::MIN_CTAS);
-  const cudaError_t e =
-      cudaFuncSetAttribute(afp_stft_kernel<R, PcmT, WRITE_MAG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e == cudaSuccess) afp_stft_kernel<R, PcmT, WRITE_MAG><<<nctas, K1_THREADS, smem, stream>>>(a);
-  return e;
+int launch_k1(afp_ctx* c, const StftArgs<R>& a, int64_t ntiles) {
+  const int nctas = (int)std::min<int64_t>(ntiles, (int64_t)c->num_sms * K1Traits<R>::MIN_CTAS);
+  return afp_launch(c, afp_stft_kernel<R, PcmT, WRITE_MAG>, nctas, K1_THREADS, k1_smem_bytes<R, PcmT>(), a);
 }
 
 // window: 2 x 512 (the second pre-scaled by 2^-15 for int16 PCM); twid: tw256, then W512
 template <typename R>
-cudaError_t launch_stft(afp_ctx* c, const DevBuf& window, const DevBuf& twid, const void* pcm, int dtype,
+int launch_stft(afp_ctx* c, const DevBuf& window, const DevBuf& twid, const void* pcm, int dtype,
                         double* mag_out, int64_t tile0, int64_t ntiles) {
   using R2 = typename K1Traits<R>::R2;
   StftArgs<R> a;
@@ -604,57 +600,38 @@ cudaError_t launch_stft(afp_ctx* c, const DevBuf& window, const DevBuf& twid, co
   a.nyq = c->d_nyq.as<double>();
   a.tile_stats = c->d_tile_stats.as<double>();
   a.mag = mag_out;
-  const int n = c->num_sms;
   if (dtype == AFP_PCM_I16)
-    return mag_out ? launch_k1<R, int16_t, true>(a, n, ntiles, c->stream)
-                   : launch_k1<R, int16_t, false>(a, n, ntiles, c->stream);
-  return mag_out ? launch_k1<R, float, true>(a, n, ntiles, c->stream)
-                 : launch_k1<R, float, false>(a, n, ntiles, c->stream);
+    return mag_out ? launch_k1<R, int16_t, true>(c, a, ntiles) : launch_k1<R, int16_t, false>(c, a, ntiles);
+  return mag_out ? launch_k1<R, float, true>(c, a, ntiles) : launch_k1<R, float, false>(c, a, ntiles);
 }
 
 }  // namespace
 
 int afp_launch_stft(afp_ctx* c, const void* pcm, int dtype, double* mag_out, int64_t tile0, int64_t ntiles) {
-  if (ntiles <= 0) return AFP_OK;
-  const cudaError_t e =
-      c->ap.spectrogram_fp32
-          ? launch_stft<float>(c, c->d_window_f, c->d_twid_f, pcm, dtype, mag_out, tile0, ntiles)
-          : launch_stft<double>(c, c->d_window, c->d_twid, pcm, dtype, mag_out, tile0, ntiles);
-  AFP_CUDA(c, e);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
-  return AFP_OK;
+  return c->ap.spectrogram_fp32 ? launch_stft<float>(c, c->d_window_f, c->d_twid_f, pcm, dtype, mag_out, tile0, ntiles)
+                                : launch_stft<double>(c, c->d_window, c->d_twid, pcm, dtype, mag_out, tile0, ntiles);
 }
 
 int afp_launch_stats(afp_ctx* c, int item0, int nitems) {
-  if (nitems <= 0) return AFP_OK;
   const ItemDesc* items = c->d_items.as<ItemDesc>();
   ItemStats* st = c->d_item_stats.as<ItemStats>();
   double* ts = c->d_tile_stats.as<double>();
   int* ticket = c->d_stats_ticket.as<int>();
-  afp_stats_kernel<<<(nitems + 7) / 8, 256, 0, c->stream>>>(items, item0, nitems, ts, st, ticket);
-  AFP_CUDA(c, cudaGetLastError());
+  int rc = afp_launch(c, afp_stats_kernel, (nitems + 7) / 8, 256, 0, items, item0, nitems, ts, st, ticket);
+  if (rc) return rc;
   const dim3 grid((unsigned)nitems, FS_SPLIT);
   if (c->ap.spectrogram_fp32)
-    afp_floorsum_kernel<float><<<grid, AFP_NBINS, 0, c->stream>>>(items, item0, st, c->d_logs.as<float>(),
-                                                                  c->d_nyq.as<double>(), ts, ticket);
-  else
-    afp_floorsum_kernel<double><<<grid, AFP_NBINS, 0, c->stream>>>(items, item0, st, c->d_logs.as<double>(),
-                                                                   c->d_nyq.as<double>(), ts, ticket);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches += 2;
-  return AFP_OK;
+    return afp_launch(c, afp_floorsum_kernel<float>, grid, AFP_NBINS, 0, items, item0, st, c->d_logs.as<float>(),
+                      c->d_nyq.as<double>(), ts, ticket);
+  return afp_launch(c, afp_floorsum_kernel<double>, grid, AFP_NBINS, 0, items, item0, st, c->d_logs.as<double>(),
+                    c->d_nyq.as<double>(), ts, ticket);
 }
 
 int afp_launch_sgram(afp_ctx* c, double* sgram_out) {
-  if (c->nitems == 0 || c->total_frames == 0) return AFP_OK;
+  if (c->total_frames == 0) return AFP_OK;
   if (c->ap.spectrogram_fp32)
-    afp_sgram_kernel<float><<<c->nitems, AFP_NBINS, 0, c->stream>>>(
-        c->d_items.as<ItemDesc>(), c->d_item_stats.as<ItemStats>(), c->d_logs.as<float>(), c->ap.hpf_pole, sgram_out);
-  else
-    afp_sgram_kernel<double><<<c->nitems, AFP_NBINS, 0, c->stream>>>(
-        c->d_items.as<ItemDesc>(), c->d_item_stats.as<ItemStats>(), c->d_logs.as<double>(), c->ap.hpf_pole, sgram_out);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
-  return AFP_OK;
+    return afp_launch(c, afp_sgram_kernel<float>, c->nitems, AFP_NBINS, 0, c->d_items.as<ItemDesc>(),
+                      c->d_item_stats.as<ItemStats>(), c->d_logs.as<float>(), c->ap.hpf_pole, sgram_out);
+  return afp_launch(c, afp_sgram_kernel<double>, c->nitems, AFP_NBINS, 0, c->d_items.as<ItemDesc>(),
+                    c->d_item_stats.as<ItemStats>(), c->d_logs.as<double>(), c->ap.hpf_pole, sgram_out);
 }

@@ -255,11 +255,10 @@ int afp_table_store_batch(afp_ctx* c, const int32_t* rows, int rows_on_host, con
   if (!rows) {                               // the hashes of the last fingerprint batch, in place
     if (!c->batch_valid) AFP_FAIL(c, AFP_ERR_STATE, "no fingerprint batch in the workspace");
     if (nfiles != c->nfiles) AFP_FAIL(c, AFP_ERR_INVALID, "nfiles differs from the fingerprint batch");
-    if (c->total_hashes < 0) {
-      AFP_CUDA(c, cudaMemcpyAsync(&c->total_hashes, c->d_file_off.as<int64_t>() + c->nfiles, sizeof(int64_t),
-                                  cudaMemcpyDeviceToHost, c->stream));
-      AFP_CUDA(c, cudaStreamSynchronize(c->stream));
-    }
+    int rc;
+    if (c->total_hashes < 0 &&
+        (rc = afp_read_back(c, &c->total_hashes, c->d_file_off.as<int64_t>() + c->nfiles, 1)))
+      return rc;
     M = c->total_hashes;
     drows = c->d_hashes.as<int32_t>();
     droff = c->d_file_off.as<int64_t>();
@@ -272,12 +271,8 @@ int afp_table_store_batch(afp_ctx* c, const int32_t* rows, int rows_on_host, con
     AFP_CUDA(c, cudaMemcpyAsync(c->d_st_off.p, row_offsets, sizeof(int64_t) * (size_t)(nfiles + 1),
                                 cudaMemcpyHostToDevice, c->stream));
     droff = c->d_st_off.as<int64_t>();
-    drows = rows;
-    if (rows_on_host && M > 0) {
-      AFP_CUDA(c, c->d_q.reserve(sizeof(int32_t) * 2 * (size_t)M));
-      AFP_CUDA(c, cudaMemcpyAsync(c->d_q.p, rows, sizeof(int32_t) * 2 * (size_t)M, cudaMemcpyHostToDevice, c->stream));
-      drows = c->d_q.as<int32_t>();
-    }
+    const int rc = afp_stage(c, c->d_q, rows, 2 * (size_t)M, rows_on_host, &drows);
+    if (rc) return rc;
   }
   if (M >= ((int64_t)1 << 31)) AFP_FAIL(c, AFP_ERR_UNSUPPORTED, "more than 2^31 entries in one store batch");
   for (int f = 0; f < nfiles; ++f)
@@ -304,35 +299,27 @@ int afp_table_store_batch(afp_ctx* c, const int32_t* rows, int rows_on_host, con
   a.eval = c->d_st_eval.as<uint32_t>(); a.cnt_new = cnt_new; a.seg_off = c->d_st_seg.as<int64_t>();
   a.seq = c->d_st_seq.as<int32_t>(); a.ovf_pos = c->d_st_ovf.as<int32_t>();
   a.heavy = c->d_st_heavy.as<int32_t>(); a.nheavy = nheavy;
-  afp_store_count_kernel<<<nfiles, 256, 0, c->stream>>>(a);
-  AFP_CUDA(c, cudaGetLastError());
-  int rc = afp_scan_large(c, reinterpret_cast<const int32_t*>(cnt_new), c->d_st_seg.as<int64_t>(), nb);
-  if (rc) return rc;
-  afp_store_scatter_kernel<<<(unsigned)((M + 255) / 256), 256, 0, c->stream>>>(a, M, cursor);
-  AFP_CUDA(c, cudaGetLastError());
-  afp_store_place_kernel<<<(unsigned)((nb + 255) / 256), 256, 0, c->stream>>>(a, nb);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches += 3;
   int h_heavy = 0;
-  AFP_CUDA(c, cudaMemcpyAsync(&h_heavy, nheavy, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
-  if (h_heavy > 0) {
-    AFP_CUDA(c, cudaFuncSetAttribute(afp_store_heavy_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 4));
-    afp_store_heavy_kernel<<<h_heavy, 256, 8192 * 4, c->stream>>>(a);
-    AFP_CUDA(c, cudaGetLastError());
-    c->launches++;
-  }
+  int rc;
+  if ((rc = afp_launch(c, afp_store_count_kernel, nfiles, 256, 0, a)) ||
+      (rc = afp_scan_large(c, reinterpret_cast<const int32_t*>(cnt_new), c->d_st_seg.as<int64_t>(), nb)) ||
+      (rc = afp_launch(c, afp_store_scatter_kernel, (unsigned)((M + 255) / 256), 256, 0, a, M, cursor)) ||
+      (rc = afp_launch(c, afp_store_place_kernel, (unsigned)((nb + 255) / 256), 256, 0, a, nb)) ||
+      (rc = afp_read_back(c, &h_heavy, nheavy, 1)) ||
+      (rc = afp_launch(c, afp_store_heavy_kernel, std::max(h_heavy, 0), 256, 8192 * 4, a)))
+    return rc;
   // ---- overflow entries, in sequence order -------------------------------------------------
   const int64_t nblk = (M + SB - 1) / SB;
-  AFP_CUDA(c, c->d_st_part.reserve(sizeof(int32_t) * (size_t)(nblk + 1) + sizeof(int64_t) * (size_t)(nblk + 2)));
-  int32_t* part = c->d_st_part.as<int32_t>();
-  int64_t* part_off = reinterpret_cast<int64_t*>(c->d_st_part.as<char>() + ((sizeof(int32_t) * (size_t)(nblk + 1) + 7) & ~(size_t)7));
-  afp_flag_blocksum_kernel<<<(unsigned)nblk, SB, 0, c->stream>>>(a.ovf_pos, M, part);
-  AFP_CUDA(c, cudaGetLastError());
-  if ((rc = afp_scan_large(c, part, part_off, nblk))) return rc;
+  int32_t* part = nullptr;
+  int64_t* part_off = nullptr;
   int64_t novf = 0;
-  AFP_CUDA(c, cudaMemcpyAsync(&novf, part_off + nblk, sizeof(int64_t), cudaMemcpyDeviceToHost, c->stream));
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+  if ((rc = afp_carve(c, c->d_st_part, [&](Carver& k) {
+         part = k.take<int32_t>(nblk + 1);
+         part_off = k.take<int64_t>(nblk + 2);
+       })) ||
+      (rc = afp_launch(c, afp_flag_blocksum_kernel, (unsigned)nblk, SB, 0, a.ovf_pos, M, part)) ||
+      (rc = afp_scan_large(c, part, part_off, nblk)) || (rc = afp_read_back(c, &novf, part_off + nblk, 1)))
+    return rc;
   if (novf > 0) {
     // sized for the whole batch at once: the overflow grows from step to step as the table fills, and
     // every regrowth would be a cudaFree + cudaMalloc in the middle of an ingest
@@ -340,12 +327,10 @@ int afp_table_store_batch(afp_ctx* c, const int32_t* rows, int rows_on_host, con
     AFP_CUDA(c, c->d_st_opos.reserve(sizeof(int32_t) * (size_t)M));
     AFP_CUDA(c, c->d_st_oval.reserve(sizeof(uint32_t) * (size_t)M));
     AFP_CUDA(c, c->d_st_slot.reserve(sizeof(int32_t) * (size_t)M));
-    afp_ovf_compact_kernel<<<(unsigned)nblk, SB, 0, c->stream>>>(a, M, part_off, c->d_st_obkt.as<uint32_t>(),
-                                                                c->d_st_opos.as<int32_t>(), c->d_st_oval.as<uint32_t>());
-    AFP_CUDA(c, cudaGetLastError());
-    c->launches++;
+    if ((rc = afp_launch(c, afp_ovf_compact_kernel, (unsigned)nblk, SB, 0, a, M, part_off, c->d_st_obkt.as<uint32_t>(),
+                         c->d_st_opos.as<int32_t>(), c->d_st_oval.as<uint32_t>())))
+      return rc;
   }
-  c->launches++;
   c->store_novf = novf;
   if (noverflow) *noverflow = novf;
   return AFP_OK;
@@ -355,26 +340,19 @@ int afp_table_fetch_overflow(afp_ctx* c, uint32_t* bucket, int32_t* count_before
   if (!c) return AFP_ERR_INVALID;
   AFP_CUDA(c, cudaSetDevice(c->device));
   const size_t n = (size_t)c->store_novf;
-  if (n) {
-    if (!bucket || !count_before || !value) return AFP_ERR_INVALID;
-    AFP_CUDA(c, cudaMemcpyAsync(bucket, c->d_st_obkt.p, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost, c->stream));
-    AFP_CUDA(c, cudaMemcpyAsync(count_before, c->d_st_opos.p, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, c->stream));
-    AFP_CUDA(c, cudaMemcpyAsync(value, c->d_st_oval.p, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost, c->stream));
-  }
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
-  return AFP_OK;
+  if (!n) return afp_read_back(c);
+  if (!bucket || !count_before || !value) return AFP_ERR_INVALID;
+  return afp_read_back(c, bucket, c->d_st_obkt.as<uint32_t>(), n, count_before, c->d_st_opos.as<int32_t>(), n, value,
+                       c->d_st_oval.as<uint32_t>(), n);
 }
 
 int afp_table_fetch_overflow_counts(afp_ctx* c, int32_t* count_before) {
   if (!c) return AFP_ERR_INVALID;
   AFP_CUDA(c, cudaSetDevice(c->device));
   const size_t n = (size_t)c->store_novf;
-  if (n) {
-    if (!count_before) return AFP_ERR_INVALID;
-    AFP_CUDA(c, cudaMemcpyAsync(count_before, c->d_st_opos.p, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, c->stream));
-  }
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
-  return AFP_OK;
+  if (!n) return afp_read_back(c);
+  if (!count_before) return AFP_ERR_INVALID;
+  return afp_read_back(c, count_before, c->d_st_opos.as<int32_t>(), n);
 }
 
 int afp_table_apply_slots(afp_ctx* c, const int32_t* slot, int64_t n) {
@@ -392,14 +370,13 @@ int afp_table_apply_slots(afp_ctx* c, const int32_t* slot, int64_t n) {
   AFP_CUDA(c, c->d_st_slot.reserve(sizeof(int32_t) * (size_t)n));
   AFP_CUDA(c, cudaMemcpyAsync(c->d_st_slot.p, slot, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, c->stream));
   const unsigned grid = (unsigned)((n + 255) / 256);
-  afp_slots_mark_kernel<<<grid, 256, 0, c->stream>>>(c->d_st_obkt.as<uint32_t>(), c->d_st_slot.as<int32_t>(), n,
-                                                     c->tab.depth, c->d_st_last.as<uint32_t>());
-  AFP_CUDA(c, cudaGetLastError());
-  afp_slots_write_kernel<<<grid, 256, 0, c->stream>>>(c->d_st_obkt.as<uint32_t>(), c->d_st_slot.as<int32_t>(),
-                                                      c->d_st_oval.as<uint32_t>(), n, c->tab.depth,
-                                                      c->d_st_last.as<uint32_t>(), c->tab.table.as<uint32_t>());
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches += 2;
+  int rc;
+  if ((rc = afp_launch(c, afp_slots_mark_kernel, grid, 256, 0, c->d_st_obkt.as<uint32_t>(), c->d_st_slot.as<int32_t>(),
+                       n, c->tab.depth, c->d_st_last.as<uint32_t>())) ||
+      (rc = afp_launch(c, afp_slots_write_kernel, grid, 256, 0, c->d_st_obkt.as<uint32_t>(),
+                       c->d_st_slot.as<int32_t>(), c->d_st_oval.as<uint32_t>(), n, c->tab.depth,
+                       c->d_st_last.as<uint32_t>(), c->tab.table.as<uint32_t>())))
+    return rc;
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));     // `slot` is the caller's
   c->store_novf = 0;
   return AFP_OK;
@@ -419,11 +396,10 @@ int afp_table_apply_patches(afp_ctx* c, const uint32_t* bucket, const int32_t* s
   AFP_CUDA(c, cudaMemcpyAsync(c->d_st_obkt.p, bucket, sizeof(uint32_t) * (size_t)n, cudaMemcpyHostToDevice, c->stream));
   AFP_CUDA(c, cudaMemcpyAsync(c->d_st_opos.p, slot, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, c->stream));
   AFP_CUDA(c, cudaMemcpyAsync(c->d_st_oval.p, value, sizeof(uint32_t) * (size_t)n, cudaMemcpyHostToDevice, c->stream));
-  afp_patch_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c->stream>>>(
-      c->tab.table.as<uint32_t>(), c->tab.depth, c->d_st_obkt.as<uint32_t>(), c->d_st_opos.as<int32_t>(),
-      c->d_st_oval.as<uint32_t>(), n);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
+  const int rc = afp_launch(c, afp_patch_kernel, (unsigned)((n + 255) / 256), 256, 0, c->tab.table.as<uint32_t>(),
+                            c->tab.depth, c->d_st_obkt.as<uint32_t>(), c->d_st_opos.as<int32_t>(),
+                            c->d_st_oval.as<uint32_t>(), n);
+  if (rc) return rc;
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));
   return AFP_OK;
 }
@@ -433,10 +409,8 @@ int afp_table_download(afp_ctx* c, uint32_t* table, int32_t* counts) {
   if (!c->tab.loaded) AFP_FAIL(c, AFP_ERR_STATE, "no table on the device");
   AFP_CUDA(c, cudaSetDevice(c->device));
   const size_t nb = (size_t)1 << c->tab.hashbits;
-  AFP_CUDA(c, cudaMemcpyAsync(table, c->tab.table.p, nb * (size_t)c->tab.depth * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
-  AFP_CUDA(c, cudaMemcpyAsync(counts, c->tab.counts.p, nb * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
-  return AFP_OK;
+  return afp_read_back(c, table, c->tab.table.as<uint32_t>(), nb * (size_t)c->tab.depth, counts,
+                       c->tab.counts.as<int32_t>(), nb);
 }
 
 // ---- CPython's random.randint(0, count) replayed in C (host bookkeeping, not the hot path) ----
@@ -562,12 +536,9 @@ int afp_scan_large(afp_ctx* c, const int32_t* in, int64_t* out, int64_t n) {
   const int64_t nblk = (n + SB - 1) / SB;
   AFP_CUDA(c, c->d_st_scan.reserve(sizeof(int64_t) * (size_t)(nblk + 2)));
   int64_t* part = c->d_st_scan.as<int64_t>();
-  afp_blocksum_kernel<<<(unsigned)nblk, SB, 0, c->stream>>>(in, n, part);
-  AFP_CUDA(c, cudaGetLastError());
-  afp_partscan_kernel<<<1, SB, 0, c->stream>>>(part, nblk);
-  AFP_CUDA(c, cudaGetLastError());
-  afp_blockscan_kernel<<<(unsigned)nblk, SB, 0, c->stream>>>(in, n, part, out);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches += 3;
-  return AFP_OK;
+  int rc;
+  if ((rc = afp_launch(c, afp_blocksum_kernel, (unsigned)nblk, SB, 0, in, n, part)) ||
+      (rc = afp_launch(c, afp_partscan_kernel, 1, SB, 0, part, nblk)))
+    return rc;
+  return afp_launch(c, afp_blockscan_kernel, (unsigned)nblk, SB, 0, in, n, part, out);
 }

@@ -157,12 +157,9 @@ int stage_id_set(afp_ctx* c, const int64_t* ids, int64_t n, bool zero_hpi, uint3
   AFP_CUDA(c, c->d_ed_slot.reserve(sizeof(int32_t) * ((size_t)mx + 1)));
   AFP_CUDA(c, cudaMemcpyAsync(c->d_ed_ids.p, ids, sizeof(int64_t) * (size_t)n, cudaMemcpyHostToDevice, c->stream));
   AFP_CUDA(c, cudaMemsetAsync(c->d_ed_bits.p, 0, sizeof(uint32_t) * words, c->stream));
-  afp_edit_idset_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c->stream>>>(
-      c->d_ed_ids.as<int64_t>(), n, c->d_ed_bits.as<uint32_t>(), c->d_ed_slot.as<int32_t>(),
-      zero_hpi ? c->tab.hashesperid.as<uint32_t>() : nullptr);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
-  return AFP_OK;
+  return afp_launch(c, afp_edit_idset_kernel, (unsigned)((n + 255) / 256), 256, 0, c->d_ed_ids.as<int64_t>(), n,
+                    c->d_ed_bits.as<uint32_t>(), c->d_ed_slot.as<int32_t>(),
+                    zero_hpi ? c->tab.hashesperid.as<uint32_t>() : nullptr);
 }
 
 }  // namespace
@@ -185,13 +182,11 @@ int afp_table_remove_ids(afp_ctx* c, const int64_t* ids, int64_t n, int64_t* rem
   AFP_CUDA(c, c->d_ed_cnt.reserve(sizeof(unsigned long long) * (size_t)n));
   AFP_CUDA(c, cudaMemsetAsync(c->d_ed_cnt.p, 0, sizeof(unsigned long long) * (size_t)n, c->stream));
   const int64_t nb = (int64_t)1 << c->tab.hashbits;
-  afp_remove_kernel<<<(unsigned)((nb + WARPS - 1) / WARPS), 256, 0, c->stream>>>(
-      c->tab.table.as<uint32_t>(), c->tab.counts.as<int32_t>(), nb, c->tab.depth, c->tab.maxtimebits,
-      c->d_ed_bits.as<uint32_t>(), nbits, c->d_ed_slot.as<int32_t>(), c->d_ed_cnt.as<unsigned long long>());
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
-  if (removed)
-    AFP_CUDA(c, cudaMemcpyAsync(removed, c->d_ed_cnt.p, sizeof(int64_t) * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
+  if ((rc = afp_launch(c, afp_remove_kernel, (unsigned)((nb + WARPS - 1) / WARPS), 256, 0, c->tab.table.as<uint32_t>(),
+                       c->tab.counts.as<int32_t>(), nb, c->tab.depth, c->tab.maxtimebits, c->d_ed_bits.as<uint32_t>(),
+                       nbits, c->d_ed_slot.as<int32_t>(), c->d_ed_cnt.as<unsigned long long>())))
+    return rc;
+  if (removed) AFP_CUDA(c, afp_read_async(c, removed, c->d_ed_cnt.as<int64_t>(), (size_t)n));
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));
   // hashesperid lost zeros-to-be and the table lost entries: the matcher's pruning bound and its
   // check for live entries of zero-length tracks are recomputed
@@ -228,52 +223,50 @@ int afp_table_retrieve_ids(afp_ctx* c, const int64_t* ids, int64_t n, int64_t* t
   const int mtb = c->tab.maxtimebits, depth = c->tab.depth;
   AFP_CUDA(c, c->d_ed_cnt.reserve(sizeof(int32_t) * (size_t)nb));
   AFP_CUDA(c, c->d_ed_off.reserve(sizeof(int64_t) * (size_t)(nb + 1)));
-  AFP_CUDA(c, c->d_ed_uoff.reserve(sizeof(int32_t) * (size_t)nu + sizeof(int64_t) * (size_t)(nu + 1)));
   int32_t* bcnt = c->d_ed_cnt.as<int32_t>();
   int64_t* boff = c->d_ed_off.as<int64_t>();
-  int64_t* uoff = c->d_ed_uoff.as<int64_t>();
-  int32_t* ucnt = reinterpret_cast<int32_t*>(uoff + nu + 1);
+  int64_t* uoff = nullptr;
+  int32_t* ucnt = nullptr;
+  if ((rc = afp_carve(c, c->d_ed_uoff, [&](Carver& k) {
+         uoff = k.take<int64_t>(nu + 1);
+         ucnt = k.take<int32_t>(nu);
+       })))
+    return rc;
   const unsigned grid = (unsigned)((nb + WARPS - 1) / WARPS);
-  afp_retrieve_count_kernel<<<grid, 256, 0, c->stream>>>(c->tab.table.as<uint32_t>(), c->tab.counts.as<int32_t>(), nb,
-                                                         depth, mtb, c->d_ed_bits.as<uint32_t>(), nbits, bcnt);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
-  if ((rc = afp_scan_large(c, bcnt, boff, nb))) return rc;
   int64_t M = 0;
-  AFP_CUDA(c, cudaMemcpyAsync(&M, boff + nb, sizeof(int64_t), cudaMemcpyDeviceToHost, c->stream));
   AFP_CUDA(c, cudaMemsetAsync(ucnt, 0, sizeof(int32_t) * (size_t)nu, c->stream));
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+  if ((rc = afp_launch(c, afp_retrieve_count_kernel, grid, 256, 0, c->tab.table.as<uint32_t>(),
+                       c->tab.counts.as<int32_t>(), nb, depth, mtb, c->d_ed_bits.as<uint32_t>(), nbits, bcnt)) ||
+      (rc = afp_scan_large(c, bcnt, boff, nb)) || (rc = afp_read_back(c, &M, boff + nb, 1)))
+    return rc;
   if (M >= ((int64_t)1 << 31)) AFP_FAIL(c, AFP_ERR_UNSUPPORTED, "more than 2^31 rows in one retrieve");
   c->rt_src = 0;
   if (M > 0) {
     AFP_CUDA(c, c->d_ed_key.reserve(sizeof(uint32_t) * (size_t)M));
     AFP_CUDA(c, c->d_ed_val.reserve(sizeof(unsigned long long) * (size_t)M));
-    afp_retrieve_scatter_kernel<<<grid, 256, 0, c->stream>>>(
-        c->tab.table.as<uint32_t>(), c->tab.counts.as<int32_t>(), nb, depth, mtb, c->d_ed_bits.as<uint32_t>(), nbits,
-        c->d_ed_slot.as<int32_t>(), bcnt, boff, c->d_ed_key.as<uint32_t>(), c->d_ed_val.as<unsigned long long>(), ucnt);
-    AFP_CUDA(c, cudaGetLastError());
-    c->launches++;
+    if ((rc = afp_launch(c, afp_retrieve_scatter_kernel, grid, 256, 0, c->tab.table.as<uint32_t>(),
+                         c->tab.counts.as<int32_t>(), nb, depth, mtb, c->d_ed_bits.as<uint32_t>(), nbits,
+                         c->d_ed_slot.as<int32_t>(), bcnt, boff, c->d_ed_key.as<uint32_t>(),
+                         c->d_ed_val.as<unsigned long long>(), ucnt)))
+      return rc;
     if (nu > 1) {      // stable: within one id the (hash, slot) order of the scatter is kept
       int end_bit = 1;
       while (((int64_t)1 << end_bit) < nu) ++end_bit;
-      size_t tmp = 0;
       AFP_CUDA(c, c->d_ed_key2.reserve(sizeof(uint32_t) * (size_t)M));
       AFP_CUDA(c, c->d_ed_val2.reserve(sizeof(unsigned long long) * (size_t)M));
-      AFP_CUDA(c, cub::DeviceRadixSort::SortPairs(nullptr, tmp, c->d_ed_key.as<uint32_t>(), c->d_ed_key2.as<uint32_t>(),
-                                                  c->d_ed_val.as<unsigned long long>(),
-                                                  c->d_ed_val2.as<unsigned long long>(), (int)M, 0, end_bit, c->stream));
-      AFP_CUDA(c, c->d_ed_cub.reserve(tmp));
-      AFP_CUDA(c, cub::DeviceRadixSort::SortPairs(c->d_ed_cub.p, tmp, c->d_ed_key.as<uint32_t>(),
-                                                  c->d_ed_key2.as<uint32_t>(), c->d_ed_val.as<unsigned long long>(),
-                                                  c->d_ed_val2.as<unsigned long long>(), (int)M, 0, end_bit, c->stream));
-      c->launches++;
+      if ((rc = cub_call(c, [&](void* t, size_t& b) {
+             return cub::DeviceRadixSort::SortPairs(t, b, c->d_ed_key.as<uint32_t>(), c->d_ed_key2.as<uint32_t>(),
+                                                    c->d_ed_val.as<unsigned long long>(),
+                                                    c->d_ed_val2.as<unsigned long long>(), (int)M, 0, end_bit,
+                                                    c->stream);
+           })))
+        return rc;
       c->rt_src = 1;
     }
   }
   if ((rc = afp_launch_scan_i32_to_i64(c, ucnt, uoff, nu))) return rc;
   std::vector<int64_t> h_uoff((size_t)nu + 1);
-  AFP_CUDA(c, cudaMemcpyAsync(h_uoff.data(), uoff, sizeof(int64_t) * (size_t)(nu + 1), cudaMemcpyDeviceToHost, c->stream));
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+  if ((rc = afp_read_back(c, h_uoff.data(), uoff, h_uoff.size()))) return rc;
   for (int64_t k = 0; k < n; ++k) {
     const int32_t u = req_u[(size_t)k];
     c->h_rt_off[(size_t)k + 1] = c->h_rt_off[(size_t)k] + h_uoff[(size_t)u + 1] - h_uoff[(size_t)u];
@@ -281,17 +274,19 @@ int afp_table_retrieve_ids(afp_ctx* c, const int64_t* ids, int64_t n, int64_t* t
   const int64_t total = c->h_rt_off[(size_t)n];
   if (nu < n && total > 0) {       // a repeated id: copy its rows once per request
     const unsigned long long* src = c->rt_src ? c->d_ed_val2.as<unsigned long long>() : c->d_ed_val.as<unsigned long long>();
-    AFP_CUDA(c, c->d_ed_req.reserve(sizeof(int64_t) * (size_t)(n + 1) + sizeof(int32_t) * (size_t)n));
     AFP_CUDA(c, c->d_ed_rows.reserve(sizeof(unsigned long long) * (size_t)total));
-    int64_t* d_roff = c->d_ed_req.as<int64_t>();
-    int32_t* d_requ = reinterpret_cast<int32_t*>(d_roff + n + 1);
-    AFP_CUDA(c, cudaMemcpyAsync(d_roff, c->h_rt_off.data(), sizeof(int64_t) * (size_t)(n + 1), cudaMemcpyHostToDevice,
-                                c->stream));
-    AFP_CUDA(c, cudaMemcpyAsync(d_requ, req_u.data(), sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, c->stream));
-    afp_retrieve_gather_kernel<<<(unsigned)n, 128, 0, c->stream>>>(src, uoff, d_requ, d_roff,
-                                                                  c->d_ed_rows.as<unsigned long long>());
-    AFP_CUDA(c, cudaGetLastError());
-    c->launches++;
+    int64_t* d_roff = nullptr;
+    int32_t* d_requ = nullptr;
+    if ((rc = afp_carve(c, c->d_ed_req, [&](Carver& k) {
+           d_roff = k.take<int64_t>(n + 1);
+           d_requ = k.take<int32_t>(n);
+         })))
+      return rc;
+    AFP_CUDA(c, afp_copy_in(c, d_roff, c->h_rt_off.data(), (size_t)(n + 1), 1));
+    AFP_CUDA(c, afp_copy_in(c, d_requ, req_u.data(), (size_t)n, 1));
+    if ((rc = afp_launch(c, afp_retrieve_gather_kernel, (unsigned)n, 128, 0, src, uoff, d_requ, d_roff,
+                         c->d_ed_rows.as<unsigned long long>())))
+      return rc;
     AFP_CUDA(c, cudaStreamSynchronize(c->stream));      // req_u and h_rt_off are host memory being read
     c->rt_src = 2;
   }
@@ -307,8 +302,7 @@ int afp_fetch_retrieved(afp_ctx* c, int32_t* rows, int rows_on_host, int64_t* ro
   if (row_offsets) std::copy(c->h_rt_off.begin(), c->h_rt_off.end(), row_offsets);
   if (rows && c->rt_total > 0) {
     const DevBuf& src = c->rt_src == 2 ? c->d_ed_rows : (c->rt_src == 1 ? c->d_ed_val2 : c->d_ed_val);
-    AFP_CUDA(c, cudaMemcpyAsync(rows, src.p, sizeof(int32_t) * 2 * (size_t)c->rt_total,
-                                rows_on_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, c->stream));
+    AFP_CUDA(c, afp_copy_out(c, rows, src.as<int32_t>(), 2 * (size_t)c->rt_total, rows_on_host));
   }
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));
   return AFP_OK;

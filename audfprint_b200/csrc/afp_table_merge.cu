@@ -215,14 +215,11 @@ int apply_overflow(afp_ctx* c, const MergeArgs& a, const std::vector<int32_t>& p
     }
     if (stage_ms) cudaEventRecord(e[1], c->stream);
     const unsigned grid = (unsigned)((m + WARPS - 1) / WARPS);
-    afp_merge_gather_kernel<IdxT><<<grid, 256, 0, c->stream>>>(a, bkt + o0, m, c->d_mg_idx.as<IdxT>(),
-                                                               c->d_mg_row.as<uint32_t>());
-    afp_merge_writeback_kernel<<<grid, 256, 0, c->stream>>>(a, bkt + o0, m, c->d_mg_row.as<uint32_t>());
-    if ((r = cudaGetLastError()) != cudaSuccess) {
-      c->err = std::string("merge apply kernels: ") + cudaGetErrorString(r);
-      return fail(AFP_ERR_CUDA);
-    }
-    c->launches += 2;
+    int rc;
+    if ((rc = afp_launch(c, afp_merge_gather_kernel<IdxT>, grid, 256, 0, a, bkt + o0, m, c->d_mg_idx.as<IdxT>(),
+                         c->d_mg_row.as<uint32_t>())) ||
+        (rc = afp_launch(c, afp_merge_writeback_kernel, grid, 256, 0, a, bkt + o0, m, c->d_mg_row.as<uint32_t>())))
+      return fail(rc);
     if (stage_ms) cudaEventRecord(e[2], c->stream);
   }
   const auto t1 = std::chrono::steady_clock::now();
@@ -276,29 +273,30 @@ int merge_body(afp_ctx* c, const uint32_t* d_in, const int32_t* d_cnt, int32_t d
   a.table = c->tab.table.as<uint32_t>(); a.counts = c->tab.counts.as<int32_t>(); a.depth = c->tab.depth;
   a.in_table = d_in; a.in_counts = d_cnt; a.in_depth = depth; a.in_nb = nm;
   a.shift = (uint32_t)(id_offset << c->tab.maxtimebits);
-  AFP_CUDA(c, c->d_mg_flag.reserve(sizeof(int32_t) * 2 * (size_t)nm));
   AFP_CUDA(c, c->d_mg_off.reserve(sizeof(int64_t) * (size_t)(nm + 1)));
-  int32_t* flag = c->d_mg_flag.as<int32_t>();
-  int32_t* pool_of = flag + nm;
+  int32_t *flag = nullptr, *pool_of = nullptr;
   int64_t* off = c->d_mg_off.as<int64_t>();
-  afp_merge_classify_kernel<<<(unsigned)((nm + WARPS - 1) / WARPS), 256, 0, c->stream>>>(a, flag, pool_of);
-  AFP_CUDA(c, cudaGetLastError());
-  c->launches++;
-  int rc = afp_scan_large(c, flag, off, nm);
-  if (rc) return rc;
   int64_t n = 0;
-  AFP_CUDA(c, cudaMemcpyAsync(&n, off + nm, sizeof(int64_t), cudaMemcpyDeviceToHost, c->stream));
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+  int rc;
+  if ((rc = afp_carve(c, c->d_mg_flag, [&](Carver& k) {
+         flag = k.take<int32_t>(nm);
+         pool_of = k.take<int32_t>(nm);
+       })) ||
+      (rc = afp_launch(c, afp_merge_classify_kernel, (unsigned)((nm + WARPS - 1) / WARPS), 256, 0, a, flag, pool_of)) ||
+      (rc = afp_scan_large(c, flag, off, nm)) || (rc = afp_read_back(c, &n, off + nm, 1)))
+    return rc;
   std::vector<int32_t> psz((size_t)n);
   if (n > 0) {
-    AFP_CUDA(c, c->d_mg_bkt.reserve((sizeof(uint32_t) + sizeof(int32_t)) * (size_t)n));
-    int32_t* d_psz = reinterpret_cast<int32_t*>(c->d_mg_bkt.as<uint32_t>() + n);
-    afp_merge_compact_kernel<<<(unsigned)((nm + 255) / 256), 256, 0, c->stream>>>(flag, pool_of, off, nm,
-                                                                                 c->d_mg_bkt.as<uint32_t>(), d_psz);
-    AFP_CUDA(c, cudaGetLastError());
-    c->launches++;
-    AFP_CUDA(c, cudaMemcpyAsync(psz.data(), d_psz, sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
-    AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+    uint32_t* d_bkt = nullptr;
+    int32_t* d_psz = nullptr;
+    if ((rc = afp_carve(c, c->d_mg_bkt, [&](Carver& k) {
+           d_bkt = k.take<uint32_t>(n);
+           d_psz = k.take<int32_t>(n);
+         })) ||
+        (rc = afp_launch(c, afp_merge_compact_kernel, (unsigned)((nm + 255) / 256), 256, 0, flag, pool_of, off, nm,
+                         d_bkt, d_psz)) ||
+        (rc = afp_read_back(c, psz.data(), d_psz, (size_t)n)))
+      return rc;
   }
   if (stage_ms) stage_ms[1] = ms_since(t0);
   if (n > 0) {
@@ -348,12 +346,15 @@ int afp_table_merge(afp_ctx* c, const uint32_t* table, const int32_t* counts, in
   if (stage_ms) std::fill(stage_ms, stage_ms + 6, 0.0);
   AFP_CUDA(c, cudaSetDevice(c->device));
   const auto t0 = std::chrono::steady_clock::now();
-  const size_t tbytes = (size_t)nm * (size_t)depth * sizeof(uint32_t);
-  AFP_CUDA(c, c->d_mg_in.reserve(tbytes + sizeof(int32_t) * (size_t)nm));
-  uint32_t* d_in = c->d_mg_in.as<uint32_t>();
-  int32_t* d_cnt = reinterpret_cast<int32_t*>(c->d_mg_in.as<char>() + tbytes);
-  AFP_CUDA(c, cudaMemcpyAsync(d_in, table, tbytes, cudaMemcpyHostToDevice, c->stream));
-  AFP_CUDA(c, cudaMemcpyAsync(d_cnt, counts, sizeof(int32_t) * (size_t)nm, cudaMemcpyHostToDevice, c->stream));
+  uint32_t* d_in = nullptr;
+  int32_t* d_cnt = nullptr;
+  if ((rc = afp_carve(c, c->d_mg_in, [&](Carver& k) {
+         d_in = k.take<uint32_t>(nm * depth);
+         d_cnt = k.take<int32_t>(nm);
+       })))
+    return rc;
+  AFP_CUDA(c, afp_copy_in(c, d_in, table, (size_t)nm * depth, 1));
+  AFP_CUDA(c, afp_copy_in(c, d_cnt, counts, (size_t)nm, 1));
   if (stage_ms) {
     AFP_CUDA(c, cudaStreamSynchronize(c->stream));
     stage_ms[0] = ms_since(t0);
@@ -370,11 +371,10 @@ int afp_table_merge_device(afp_ctx* c, const uint32_t* table_dev, const int32_t*
   // the checks read the counts on the host (4 MB at 2^20 buckets); the rows stay where they are
   const auto t0 = std::chrono::steady_clock::now();
   std::vector<int32_t> h_counts((size_t)1 << hashbits);
-  AFP_CUDA(c, cudaMemcpyAsync(h_counts.data(), counts_dev, sizeof(int32_t) * h_counts.size(), cudaMemcpyDeviceToHost,
-                              c->stream));
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));
+  int rc = afp_read_back(c, h_counts.data(), counts_dev, h_counts.size());
+  if (rc) return rc;
   const double download_ms = ms_since(t0);
-  int rc = merge_check(c, h_counts.data(), hashbits, depth, id_offset, np_state625);
+  rc = merge_check(c, h_counts.data(), hashbits, depth, id_offset, np_state625);
   if (rc) return rc;
   if (noverflow) *noverflow = 0;
   if (stage_ms) {
@@ -390,9 +390,8 @@ int afp_table_export(afp_ctx* c, uint32_t* table_dev, int32_t* counts_dev) {
   if (!c->tab.loaded) AFP_FAIL(c, AFP_ERR_STATE, "no table on the device");
   AFP_CUDA(c, cudaSetDevice(c->device));
   const size_t nb = (size_t)1 << c->tab.hashbits;
-  AFP_CUDA(c, cudaMemcpyAsync(table_dev, c->tab.table.p, nb * (size_t)c->tab.depth * sizeof(uint32_t),
-                              cudaMemcpyDeviceToDevice, c->stream));
-  AFP_CUDA(c, cudaMemcpyAsync(counts_dev, c->tab.counts.p, nb * sizeof(int32_t), cudaMemcpyDeviceToDevice, c->stream));
+  AFP_CUDA(c, afp_copy_out(c, table_dev, c->tab.table.as<uint32_t>(), nb * (size_t)c->tab.depth, 0));
+  AFP_CUDA(c, afp_copy_out(c, counts_dev, c->tab.counts.as<int32_t>(), nb, 0));
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));
   return AFP_OK;
 }
