@@ -67,7 +67,8 @@ __device__ int parse_header(const uint8_t* p, int64_t avail, const FlacFile& f, 
   h.variable = p[1] & 1;
   const int bs_code = p[2] >> 4, sr_code = p[2] & 15, ch_code = p[3] >> 4, ss_code = (p[3] >> 1) & 7;
   bool reserved = bs_code == 0 || sr_code == 15 || ch_code > 10 || ss_code == 3 || (p[3] & 1);
-  // the coded number: 1-7 bytes, UTF-8 style (up to 36 bits for a sample number, 31 for a frame number)
+  // the coded number: 1-6 bytes, UTF-8 style, up to 31 bits.  The format allows a 7-byte (36-bit) sample
+  // number, but FFmpeg's header reader refuses the 0xFE lead byte, so such a header is not a header here
   int pos = 4;
   const uint32_t b0 = p[pos++];
   int extra;
@@ -78,9 +79,7 @@ __device__ int parse_header(const uint8_t* p, int64_t avail, const FlacFile& f, 
   else if ((b0 & 0xF8) == 0xF0) { extra = 3; v = b0 & 0x07; }
   else if ((b0 & 0xFC) == 0xF8) { extra = 4; v = b0 & 0x03; }
   else if ((b0 & 0xFE) == 0xFC) { extra = 5; v = b0 & 0x01; }
-  else if (b0 == 0xFE) { extra = 6; v = 0; }
   else return HDR_NONE;
-  if (extra == 6 && !h.variable) return HDR_NONE;
   if (avail < pos + extra + 1) return HDR_NONE;
   for (int k = 0; k < extra; ++k) {
     const uint32_t b = p[pos++];
@@ -311,10 +310,15 @@ __device__ __forceinline__ int read_residual(BitReader& br, int32_t* s, int bs, 
       const int nb = br.getu(5);
       for (; i < end; ++i) s[i] = br.gets(nb);
     } else {
+      // FFmpeg's Rice reader caps the quotient at limit = 2^(32 - k) + 1 (2^31 - 1 for k < 2): a run of
+      // limit zeros is refused, a run of limit - 1 reads one bit b and gives u = b + 1, and u = 2^32 - 1
+      // (residual -2^31) is refused.  Both refusals drop the frame there, so they make the file unreadable.
+      const uint32_t limit = k > 1 ? (INT_MAX >> (k - 1)) + 2u : (uint32_t)INT_MAX;
       for (; i < end; ++i) {
         const uint32_t q = br.unary();
-        if (br.bad) return AFP_FLAC_CORRUPT;
-        const uint32_t u = (q << k) | br.getu(k);
+        if (br.bad || q >= limit) return AFP_FLAC_CORRUPT;
+        const uint32_t u = q == limit - 1 ? br.getu(1) + 1 : (q << k) | br.getu(k);
+        if (u == 0xFFFFFFFFu) return AFP_FLAC_CORRUPT;
         s[i] = (int32_t)((u >> 1) ^ (0u - (u & 1)));
       }
     }

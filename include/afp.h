@@ -173,8 +173,8 @@ int afp_pcm_frontend_batch(afp_ctx* ctx, const int16_t* pcm, int pcm_on_host, in
  *
  * Locate: every byte that starts a frame header (sync code, no reserved value, fields consistent with
  * STREAMINFO, correct CRC-8) is a candidate.  From the first byte of the file, a frame ends at the next
- * candidate whose frame number (fixed block size) or first-sample number (variable block size)
- * follows on and where the CRC-16 over [frame start, candidate) is right; the last frame ends at the
+ * candidate whose frame number (fixed block size) or first-sample number (variable block size; below
+ * 2^31, as FFmpeg reads no 7-byte coded number) follows on and where the CRC-16 over [frame start, candidate) is right; the last frame ends at the
  * end of the file's bytes.  So a sync pattern inside compressed data never splits a frame.  STREAMINFO's
  * total sample count is not used (it may be 0): the count is the sum of the frames' block sizes.
  *
@@ -209,7 +209,11 @@ enum {
   AFP_FLAC_TRUNCATED = 5,   /* the last frame does not end in its CRC-16 (cut short, or damaged: no
                              * later header tells the two apart) */
   AFP_FLAC_CORRUPT = 6      /* subframe data that does not fit its frame (residual past the frame's
-                             * end, a partition order the block size cannot take, a negative LPC shift) */
+                             * end, a partition order the block size cannot take, a negative LPC shift),
+                             * or that FFmpeg's decoder refuses: wasted bits >= the subframe's depth, a
+                             * residual of -2^31, a Rice quotient of 2^(32 - k) + 1 or more (2^31 - 1 for
+                             * k < 2).  A quotient of exactly 2^(32 - k) is read as FFmpeg reads it: one
+                             * more bit b, u = b + 1. */
 };
 
 /*   bytes         packed FLAC frame bytes of all files, HOST or DEVICE, nbytes_total of them.  A DEVICE

@@ -81,27 +81,30 @@ def _width(r):
     return 0 if not np.any(r) else m.bit_length() + 1
 
 
-def residual(w, r, order, bs, po=0, method=0, escape=()):
+def residual(w, r, order, bs, po=0, method=0, escape=(), *, rice=None, esc_width=None):
     """Rice-coded residual r (the block's residual after `order` warm-up samples); partitions listed in
-    `escape` are written raw."""
+    `escape` are written raw.  rice: a Rice parameter per partition (None: chosen from the partition's
+    mean); esc_width: the escape partitions' sample width (None: the narrowest that holds them).  A
+    method above 1 or a partition order that does not divide the block writes only what fits, for
+    streams a decoder must refuse."""
     w.u(method, 2)
     w.u(po, 4)
     kbits, esc = (5, 31) if method else (4, 15)
     psize = bs >> po
     i = 0
     for p in range(1 << po):
-        n = psize - (order if p == 0 else 0)
+        n = max(psize - (order if p == 0 else 0), 0)
         part = np.asarray(r[i:i + n], np.int64)
         i += n
         if p in escape:
-            nb = _width(part)
+            nb = _width(part) if esc_width is None else esc_width
             w.u(esc, kbits)
             w.u(nb, 5)
             for v in part:
                 w.u(int(v), nb)
             continue
-        mean = float(np.mean(np.abs(part))) if n else 0.0
-        k = min(max(int(np.log2(mean + 1.0)), 0), esc - 1)
+        mean = float(np.mean(np.abs(part))) if len(part) else 0.0
+        k = min(max(int(np.log2(mean + 1.0)), 0), esc - 1) if rice is None or rice[p] is None else rice[p]
         w.u(k, kbits)
         for v in part:
             v = int(v)
@@ -111,12 +114,15 @@ def residual(w, r, order, bs, po=0, method=0, escape=()):
 
 
 def subframe(w, x, sbps, kind="fixed", order=2, coefs=None, prec=12, shift=10, wasted=0, po=0, method=0,
-             escape=(), sub_type=None):
+             escape=(), sub_type=None, *, rice=None, esc_width=None, raw=None, pad=0, prec_code=None):
     """One subframe of the int64 samples x at sbps bits.  kind: constant, verbatim, fixed (order 0-4),
-    lpc (coefs quantised ints, precision prec, shift).  sub_type overrides the 6-bit type code."""
+    lpc (coefs quantised ints, precision prec, shift).  sub_type overrides the 6-bit type code.
+    rice / esc_width: see residual(); raw: the residual to write instead of x's (x then gives only the
+    warm-up samples), pad: the subframe header's padding bit, prec_code: the 4-bit precision code
+    instead of prec - 1."""
     x = np.asarray(x, np.int64)
     bs = len(x)
-    w.u(0, 1)
+    w.u(pad, 1)
     code = {"constant": 0, "verbatim": 1, "fixed": 8 + order, "lpc": 32 + (len(coefs or [1]) - 1)}[kind]
     w.u(code if sub_type is None else sub_type, 6)
     if wasted:
@@ -139,26 +145,29 @@ def subframe(w, x, sbps, kind="fixed", order=2, coefs=None, prec=12, shift=10, w
         r = x.copy()
         for _ in range(order):
             r = np.diff(r)
-        residual(w, r, order, bs, po, method, escape)
+        residual(w, r if raw is None else raw, order, bs, po, method, escape, rice=rice, esc_width=esc_width)
     else:
         c = np.asarray(coefs, np.int64)
         p = len(c)
         for v in x[:p]:
             w.u(int(v), sbps)
-        w.u(prec - 1, 4)
+        w.u(prec - 1 if prec_code is None else prec_code, 4)
         w.u(shift, 5)
         for v in c:
             w.u(int(v), prec)
-        pred = np.zeros(bs - p, np.int64)
+        pred = np.zeros(max(bs - p, 0), np.int64)
         for j in range(p):
             pred += c[j] * x[p - 1 - j:bs - 1 - j]
-        residual(w, x[p:] - (pred >> shift), p, bs, po, method, escape)
+        r = x[p:] - (pred >> shift) if raw is None else raw
+        residual(w, r, p, bs, po, method, escape, rice=rice, esc_width=esc_width)
 
 
-def frame(block, number, bps, rate, variable=False, chmode=None, bs_code=None, sr_code=None, specs=None):
+def frame(block, number, bps, rate, variable=False, chmode=None, bs_code=None, sr_code=None, specs=None, *,
+          ss_code=None, reserved=0, tail=b""):
     """One frame of the int64 block (bs, nch): its header, subframes and CRC-16.  chmode 8-10 codes the
     first two channels as left/side, right/side or mid/side.  specs: one dict of subframe() keywords
-    per channel."""
+    per channel.  ss_code: the sample-size code (None: the code of bps, 0 for a depth without one);
+    reserved: the header's reserved bit; tail: bytes after the subframes, before the CRC-16."""
     block = np.asarray(block, np.int64)
     bs, nch = block.shape
     chmode = nch - 1 if chmode is None else chmode
@@ -166,7 +175,9 @@ def frame(block, number, bps, rate, variable=False, chmode=None, bs_code=None, s
         bs_code = _STD_BS.get(bs, 6 if bs <= 256 else 7)
     if sr_code is None:
         sr_code = _STD_SR.get(rate, 0)
-    hdr = bytearray([0xFF, 0xF8 | int(variable), (bs_code << 4) | sr_code, (chmode << 4) | (_SS.get(bps, 0) << 1)])
+    if ss_code is None:
+        ss_code = _SS.get(bps, 0)
+    hdr = bytearray([0xFF, 0xF8 | int(variable), (bs_code << 4) | sr_code, (chmode << 4) | (ss_code << 1) | reserved])
     hdr += utf8_number(number)
     if bs_code == 6:
         hdr += bytes([bs - 1])
@@ -192,7 +203,7 @@ def frame(block, number, bps, rate, variable=False, chmode=None, bs_code=None, s
     specs = specs or [{}] * nch
     for c in range(nch):
         subframe(w, chans[c], bps + side[c], **specs[c])
-    body = bytes(hdr) + w.tobytes()
+    body = bytes(hdr) + w.tobytes() + tail
     out = bytearray(body)
     out += crc16(out).to_bytes(2, "big")
     return bytes(out)
@@ -217,12 +228,15 @@ def block_header(typ, length, last):
     return bytes([(0x80 if last else 0) | typ]) + length.to_bytes(3, "big")
 
 
-def stream(pcm, bps, rate, sizes=None, variable=False, total=None, blocks=b"", id3=0, **frame_kw):
+def stream(pcm, bps, rate, sizes=None, variable=False, total=None, blocks=b"", id3=0, *, first=0, max_bs=None,
+           **frame_kw):
     """A whole FLAC file of the int (n, nch) pcm cut into blocks of `sizes` (default 4096).  blocks:
     metadata blocks after STREAMINFO (header bytes included, the last one flagged); id3: bytes of an
-    ID3v2 tag body put in front.  frame_kw goes to every frame; a callable value is called with the frame
-    index."""
-    pcm = np.asarray(pcm, np.int64).reshape(len(pcm), -1)
+    ID3v2 tag body put in front; first: the first frame's number (fixed block size) or sample number
+    (variable); max_bs: STREAMINFO's largest block size (None: the largest of `sizes`).  frame_kw goes to
+    every frame; a callable value is called with the frame index."""
+    pcm = np.asarray(pcm, np.int64)
+    pcm = pcm if pcm.ndim == 2 else pcm.reshape(len(pcm), -1)
     n = len(pcm)
     if sizes is None:
         sizes = [4096] * (n // 4096) + ([n % 4096] if n % 4096 else [])
@@ -230,9 +244,10 @@ def stream(pcm, bps, rate, sizes=None, variable=False, total=None, blocks=b"", i
     frames, pos = [], 0
     for k, bs in enumerate(sizes):
         kw = {key: (v(k) if callable(v) else v) for key, v in frame_kw.items()}
-        frames.append(frame(pcm[pos:pos + bs], pos if variable else k, bps, rate, variable, **kw))
+        frames.append(frame(pcm[pos:pos + bs], first + (pos if variable else k), bps, rate, variable, **kw))
         pos += bs
-    out = b"fLaC" + streaminfo(min(sizes) if variable else max(sizes), max(sizes), rate, pcm.shape[1], bps,
+    top = max(sizes, default=0) if max_bs is None else max_bs
+    out = b"fLaC" + streaminfo(min(sizes, default=0) if variable else top, top, rate, pcm.shape[1], bps,
                                n if total is None else total, last=not blocks) + blocks
     if id3:
         size = bytes([(id3 >> 21) & 127, (id3 >> 14) & 127, (id3 >> 7) & 127, id3 & 127])
