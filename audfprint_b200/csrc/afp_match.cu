@@ -660,7 +660,7 @@ int afp_match_batch(afp_ctx* c, const int32_t* q_rows, int q_on_host, int32_t nq
                     const afp_matcher_params* p, int64_t* total_rows) {
   if (!c || !p || nqueries < 0 || (nqueries > 0 && !q_offsets)) return AFP_ERR_INVALID;
   if (!c->tab.loaded) AFP_FAIL(c, AFP_ERR_STATE, "no table uploaded");
-  if (p->window < 0 || p->window > 4096 || p->search_depth < 0 || p->max_alignments_per_id < 0)
+  if (p->window < 0 || p->window > 4096 || p->threshcount < 0 || p->search_depth < 0 || p->max_alignments_per_id < 0)
     AFP_FAIL(c, AFP_ERR_INVALID, "bad matcher parameters");
   AFP_CUDA(c, cudaSetDevice(c->device));
   c->match_total_rows = -1;
@@ -717,6 +717,15 @@ int afp_match_batch(afp_ctx* c, const int32_t* q_rows, int q_on_host, int32_t nq
     if ((rc = qmax(r0, nrows_in, d_mm)) || (rc = afp_read_back(c, h_mm, d_mm, 4))) return rc;
   }
   if (h_mm[1] < 0 || h_mm[3] < 0) AFP_FAIL(c, AFP_ERR_INVALID, "negative query time");
+  // dtime histogram: bin dt + bias for dt in [-qmax, 2^maxtimebits), bias = qmax + window + 2,
+  // indexed with int by the kernels.  [0] short queries, [1] long ones.
+  int64_t bias[2], hist_len[2];
+  for (int k = 0; k < 2; ++k) {
+    bias[k] = (int64_t)h_mm[2 * k] + p->window + 2;
+    hist_len[k] = ((int64_t)1 << c->tab.maxtimebits) + bias[k] + p->window + 4;
+    if (hist_len[k] > INT32_MAX)
+      AFP_FAIL(c, AFP_ERR_UNSUPPORTED, "query time too large: 2^maxtimebits + query time + 2 * window + 6 must not exceed 2^31 - 1");
+  }
 
   // persistent grid; a fixed CTA count keeps the scratch layout (and its zeroed state) reusable
   int nctas = c->num_sms;
@@ -736,8 +745,8 @@ int afp_match_batch(afp_ctx* c, const int32_t* q_rows, int q_on_host, int32_t nq
   a.sdepth = p->search_depth;
   a.maxalign = p->max_alignments_per_id;
   a.hits_cap = std::max<int64_t>(maxnq * c->tab.depth, 1);
-  a.bias = h_mm[0] + p->window + 2;
-  a.hist_len = (1 << c->tab.maxtimebits) + a.bias + p->window + 4;
+  a.bias = (int)bias[0];
+  a.hist_len = (int)hist_len[0];
   a.row_cap = p->row_capacity > 0 ? p->row_capacity : 256;
   if (a.hits_cap >= HITS_MAX || a.nids >= ((int64_t)1 << 24))
     AFP_FAIL(c, AFP_ERR_UNSUPPORTED, "query too large (rows * depth >= 2^30) or more than 2^24 track ids");
@@ -847,8 +856,8 @@ int afp_match_batch(afp_ctx* c, const int32_t* q_rows, int q_on_host, int32_t nq
     // ---- long queries (afp_match_long.cu): one histogram pair per CTA of the mode pass, sized
     // over the long queries' times, zeroed here and left zeroed by the mode search
     MatchArgs al = a;
-    al.bias = h_mm[2] + p->window + 2;
-    al.hist_len = (1 << c->tab.maxtimebits) + al.bias + p->window + 4;
+    al.bias = (int)bias[1];
+    al.hist_len = (int)hist_len[1];
     const size_t per = (size_t)al.hist_len * 2 * sizeof(int32_t);
     AFP_CUDA(c, afp_memory_budget(c->d_lg_hist, &budget));
     c->lg_ctas = (int)std::max<size_t>(1, std::min<size_t>((size_t)c->num_sms, budget / per));

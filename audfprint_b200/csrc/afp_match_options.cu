@@ -486,7 +486,7 @@ int rank_options(afp_ctx* c, const int32_t* q_rows, int q_on_host, int32_t nquer
       !(exact_count || find_time_range))
     AFP_FAIL(c, AFP_ERR_INVALID, "exact_count and find_time_range are 0 or 1, and one of them is 1");
   if (!isfinite(time_quantile)) AFP_FAIL(c, AFP_ERR_INVALID, "time_quantile must be finite");
-  if (p->window < 0 || p->window > 4096 || p->search_depth < 0 || p->max_alignments_per_id < 0)
+  if (p->window < 0 || p->window > 4096 || p->threshcount < 0 || p->search_depth < 0 || p->max_alignments_per_id < 0)
     AFP_FAIL(c, AFP_ERR_INVALID, "bad matcher parameters");
   for (int k = 0; k < 32; ++k) {
     br.v[k] = timebits_breaks[k];

@@ -67,6 +67,9 @@ class Matcher(object):
     def _params(self):
         if self.illustrate:
             raise NotImplementedError("illustrate is not implemented (SURVEY.md §8f-4)")
+        if int(self.threshcount) < 0:
+            # the reference's rows are degenerate there (DESIGN.md §8)
+            raise ValueError("threshcount must be >= 0, got %d" % int(self.threshcount))
         return _lib.MatcherParams(int(self.window), int(self.threshcount), int(self.search_depth),
                                   int(self.max_alignments_per_id), 0, 0,
                                   1 if getattr(self, "force_general_kernel", False) else 0)

@@ -80,8 +80,9 @@ typedef struct {
 
 /* Matcher attributes (audfprint_match.py:96-122). */
 typedef struct {
-  int32_t window;                /* Matcher.window                    */
-  int32_t threshcount;           /* Matcher.threshcount               */
+  int32_t window;                /* Matcher.window, 0 .. 4096         */
+  int32_t threshcount;           /* Matcher.threshcount, >= 0 (a negative one is AFP_ERR_INVALID:
+                                  * the reference's rows there are degenerate, DESIGN.md §8)    */
   int32_t search_depth;          /* Matcher.search_depth              */
   int32_t max_alignments_per_id; /* Matcher.max_alignments_per_id     */
   int32_t publish_candidates;    /* table-shard mode (SURVEY.md §8e): 0 = off.  1 = rank and report

@@ -56,7 +56,9 @@ def candidates(h, hpi, thresh, sdepth, publish=False):
 def rows_in_rank_order(h, ids, raws, window, thresh, maxalign=100):
     """orc.offset_histogram_rows: rows [id, count, dtime, raw, rank, 0, 0] of the ranked
     candidates, in rank order (before the final sort by count).  Each id's histogram starts at its
-    own smallest dtime instead of the query's: the bins below are empty and change nothing."""
+    own smallest dtime instead of the query's: the bins below are empty and change nothing as long
+    as threshcount >= 0 (an empty bin is then never a mode).  With threshcount < 0 the reference
+    also reports empty bins below the id's own range; the project refuses such a threshcount."""
     if len(h) == 0:
         return np.zeros((0, 7), np.int32)
     by_id = np.argsort(h[:, 0], kind="stable")

@@ -93,21 +93,22 @@ def singles(ids, sc, hpi=None, width=None, qt=0):
         sc.group(ids[s:s + width], 1, qt, 100 + s // width)
 
 
-def matcher(window, thresh, sdepth, force=False):
+def matcher(window, thresh, sdepth, force=False, maxalign=100):
     m = Matcher()
     m.window, m.threshcount, m.search_depth = window, thresh, sdepth
+    m.max_alignments_per_id = maxalign
     m.force_general_kernel = force
     return m
 
 
 class Ref:
-    def __init__(self, sc, q, thresh, sdepth, window):
+    def __init__(self, sc, q, thresh, sdepth, window, maxalign=100):
         h = k4.hits(sc.table, sc.counts, sc.hashbits, sc.depth, sc.mtb, q)
         self.h = h
         self.ids, self.raw, self.w = k4.candidates(h, sc.hpi, thresh, sdepth)
-        self.rows = k4.rows_in_rank_order(h, self.ids, self.raw, window, thresh)
+        self.rows = k4.rows_in_rank_order(h, self.ids, self.raw, window, thresh, maxalign)
         self.pid, self.praw, self.pw, self.pcnt = k4.candidates(h, sc.hpi, thresh, sdepth, publish=True)
-        self.prows = k4.rows_in_rank_order(h, self.pid, self.praw, window, thresh)
+        self.prows = k4.rows_in_rank_order(h, self.pid, self.praw, window, thresh, maxalign)
         uid, cnt = np.unique(h[:, 0], return_counts=True)
         self.uid, self.ucnt = uid, cnt
 
@@ -121,15 +122,15 @@ def padded(sc, q):
     return np.concatenate([q, pad.astype(np.int32)])
 
 
-def run(sc, thresh, sdepth, status, window=1, paths=("fast", "general", "long"), q=None, ref=None):
+def run(sc, thresh, sdepth, status, window=1, paths=("fast", "general", "long"), q=None, ref=None, maxalign=100):
     """Compare every path with the reference.  status = (plain, publish) expected in column 0 of
     the fast kernel's status.  Returns the reference."""
     ht = sc.ht()
     q = sc.query() if q is None else q
-    ref = ref or Ref(sc, q, thresh, sdepth, window)
+    ref = ref or Ref(sc, q, thresh, sdepth, window, maxalign)
     for path in paths:
         qq = padded(sc, q) if path == "long" else q
-        m = matcher(window, thresh, sdepth, force=(path == "general"))
+        m = matcher(window, thresh, sdepth, force=(path == "general"), maxalign=maxalign)
         qoff = np.array([0, len(qq)], np.int64)
         got = m.match_batch(ht, [qq], sort=False)[0]
         st = Matcher.last_status(ht, 1)[0]
