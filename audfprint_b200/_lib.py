@@ -59,6 +59,10 @@ _SIGS = {
                                    C.c_int, _I64P]),
     "afp_pcm_frontend_batch": (C.c_int, [_P, _P, C.c_int, C.c_int64, C.c_int32, _I64P, _I64P, _P, _P, _P, C.c_int32,
                                          _P, _I64P, _P, _P, C.c_int64, _I64P, _I64P]),
+    "afp_swr_design": (C.c_int, [C.c_int32, C.c_int32, _P, C.c_int64, _P, _P]),
+    "afp_swr_length": (C.c_int, [C.c_int64, C.c_int32, C.c_int32, _I64P]),
+    "afp_swr_frontend_batch": (C.c_int, [_P, _P, C.c_int, C.c_int64, C.c_int32, _I64P, _I64P, _P, _P, C.c_int32, _P,
+                                         C.c_int64, _I64P, _I64P]),
     "afp_flac_locate_batch": (C.c_int, [_P, _P, C.c_int, C.c_int64, C.c_int32, C.POINTER(FlacStream), _I64P, _P]),
     "afp_flac_decode_batch": (C.c_int, [_P, _P, C.c_int64, _I64P, _P]),
     "afp_set_analyzer": (C.c_int, [_P, C.POINTER(AnalyzerParams), _P, _P, C.c_double]),

@@ -67,12 +67,19 @@ def resample_taps(up, down):
     return np.ascontiguousarray(firwin(2 * half + 1, 1.0 / max_rate, window=('kaiser', 5.0)) * up, dtype=np.float64)
 
 
-def pcm_frontend(raw, channels, src_rate, dst_rate=None, device=None, to_host=True):
+def pcm_frontend(raw, channels, src_rate, dst_rate=None, device=None, to_host=True, resampler='poly'):
     """Interleaved int16 PCM -> mono float32 at dst_rate, on the device (afp_pcm_frontend:
     channel mean, 1/32768 scaling, polyphase resampling).  Returns a NumPy array, or with
-    to_host=False a torch CUDA tensor that Analyzer.fingerprint_packed takes as it is."""
+    to_host=False a torch CUDA tensor that Analyzer.fingerprint_packed takes as it is.
+    resampler='ffmpeg' gives instead the bits `ffmpeg -ac 1 -ar dst_rate` gives, v / 32768
+    (afp_swr_frontend_batch; mono or stereo, and rates with out / gcd <= 1024)."""
     from math import gcd
     raw = np.ascontiguousarray(raw, dtype=np.int16).reshape(-1)
+    if _check_resampler(resampler) == 'ffmpeg':
+        out, off, lens = pcm_frontend_batch([raw], [channels], [src_rate], dst_rate if dst_rate is not None else src_rate,
+                                            device=device, resampler='ffmpeg')
+        out = out[:int(lens[0])].clone()
+        return out.cpu().numpy() if to_host else out
     nframes = len(raw) // max(1, int(channels))
     up, down = 1, 1
     if dst_rate is not None and int(dst_rate) != int(src_rate):
@@ -122,21 +129,74 @@ def _audio_read_raw(filename):
     return _wav_read_raw(filename)
 
 
-def _wav_reader(filename, sr=None, channels=None, device=None):
+def _check_resampler(resampler):
+    if resampler not in ('poly', 'ffmpeg'):
+        raise ValueError("resampler must be 'poly' or 'ffmpeg'")
+    return resampler
+
+
+def swr_length(nframes, src_rate, dst_rate):
+    """Samples the 'ffmpeg' front-end (afp_swr_frontend_batch) yields for nframes input frames (host
+    arithmetic, no device).  Raises AfpError for a rate the front-end refuses."""
+    n = C.c_int64(0)
+    rc = _lib.load().afp_swr_length(int(nframes), int(src_rate), int(dst_rate), C.byref(n))
+    if rc == -3:
+        raise _lib.AfpError("the ffmpeg front-end does not take %d Hz -> %d Hz" % (src_rate, dst_rate))
+    if rc:
+        raise ValueError("afp_swr_length: %d frames, %d Hz -> %d Hz" % (nframes, src_rate, dst_rate))
+    return int(n.value)
+
+
+# the channel masks ffmpeg gives a WAV that names none: FC for mono, FL|FR for stereo
+_DEFAULT_WAV_MASKS = {1: 0x4, 2: 0x3}
+
+
+def _wav_channel_mask(filename):
+    """dwChannelMask of a WAVE_FORMAT_EXTENSIBLE file, or None for any other WAV."""
+    with open(filename, 'rb') as f:
+        if f.read(12)[8:12] != b'WAVE':
+            return None
+        while True:
+            head = f.read(8)
+            if len(head) < 8:
+                return None
+            cid, size = head[:4], int.from_bytes(head[4:], 'little')
+            if cid == b'fmt ':
+                fmt = f.read(size)
+                if size >= 24 and int.from_bytes(fmt[:2], 'little') == 0xFFFE:
+                    return int.from_bytes(fmt[20:24], 'little')
+                return None
+            f.seek(size + (size & 1), 1)
+
+
+def _swr_check(filename, raw, nch, fs, sr):
+    """Raise for a file the 'ffmpeg' front-end cannot give ffmpeg's bits for: more than two channels,
+    a WAV whose channel mask is not the default layout, or a rate afp_swr_frontend_batch refuses."""
+    if nch > 2:
+        raise ValueError("%s: the ffmpeg front-end takes mono or stereo, not %d channels" % (filename, nch))
+    if isinstance(raw, np.ndarray) and _wav_channel_mask(filename) not in (None, 0, _DEFAULT_WAV_MASKS[nch]):
+        raise ValueError("%s: the ffmpeg front-end takes only the default channel layout" % filename)
+    swr_length(0, fs, sr)
+
+
+def _wav_reader(filename, sr=None, channels=None, device=None, resampler='poly'):
     """PCM-WAV and FLAC reader standing in for audio_read.audio_read (audio_read.py:56-68; ffmpeg
     decoding of other formats is out of scope, SURVEY §2 #9).  Returns (float32 samples in [-1,1), sr)
     like the reference reader does (audio_read.py:139-145).  A WAV is parsed on the host; a FLAC file's
     frames are decoded on the device (flac.decode) to the int16 samples ffmpeg's decoder gives.  The
     arithmetic the reference hands to ffmpeg - down-mix to mono, resampling to `sr` - runs on the
     device (afp_pcm_frontend, SURVEY.md 8f-2).  No two resamplers agree bit for bit, so parity
-    statements in this repo are made on 11025 Hz PCM."""
+    statements in this repo are made on 11025 Hz PCM.  With resampler='ffmpeg' the down-mix and
+    resampling are ffmpeg's own, bit for bit (afp_swr_frontend_batch)."""
     raw, nch, fs = _audio_read_raw(filename)
+    if _check_resampler(resampler) == 'ffmpeg':
+        _swr_check(filename, raw, nch, fs, fs if sr is None else sr)
     if isinstance(raw, flac.FlacStream):
         raw = flac.decode(raw, device)
     if nch == 1 and (sr is None or fs == sr):
         # nothing to do but the reader's own scaling (exact in float32)
         return raw.astype(np.float32) * np.float32(1.0 / 32768.0), fs
-    data = pcm_frontend(raw, nch, fs, sr, device=device)
+    data = pcm_frontend(raw, nch, fs, sr, device=device, resampler=resampler)
     return data, (fs if sr is None else sr)
 
 
@@ -164,22 +224,23 @@ def taps_table(pairs):
     return np.array(uniq, np.int32).reshape(-1, 2), off, taps
 
 
-def pcm_frontend_batch(raws, channels, src_rates, dst_rate, device=None):
+def pcm_frontend_batch(raws, channels, src_rates, dst_rate, device=None, resampler='poly'):
     """Many files' interleaved int16 PCM -> mono float32 at dst_rate in ONE device buffer
     (afp_pcm_frontend_batch: one upload of the packed PCM, one launch, one synchronise).
     Every file's samples are bit-identical to pcm_frontend on that file alone.
     Returns (out torch CUDA float32, offsets int64 [n+1], lengths int64 [n]): file i is
     out[offsets[i]:offsets[i] + lengths[i]], starting on a 16-byte boundary - the layout
-    Analyzer.fingerprint_packed(out, offsets, sample_lengths=lengths) takes as it is."""
+    Analyzer.fingerprint_packed(out, offsets, sample_lengths=lengths) takes as it is.
+    resampler='ffmpeg': afp_swr_frontend_batch, ffmpeg's down-mix and resampler (pcm_frontend)."""
     raws = [np.ascontiguousarray(r, dtype=np.int16).reshape(-1) for r in raws]
     inoff = np.zeros(len(raws) + 1, np.int64)
     inoff[1:] = np.cumsum([len(r) for r in raws])
     nfr = [len(r) // max(1, int(c)) for r, c in zip(raws, channels)]
     packed = np.concatenate(raws) if raws else np.zeros(0, np.int16)
-    return _frontend_packed(_lib.context(device), packed, inoff, nfr, channels, src_rates, dst_rate)
+    return _frontend_packed(_lib.context(device), packed, inoff, nfr, channels, src_rates, dst_rate, resampler)
 
 
-def _frontend_packed(ctx, pcm, inoff, nfr, channels, src_rates, dst_rate):
+def _frontend_packed(ctx, pcm, inoff, nfr, channels, src_rates, dst_rate, resampler='poly'):
     """afp_pcm_frontend_batch over files packed in `pcm`, a host int16 array or a device int16 tensor:
     file i's nfr[i] frames of channels[i] channels start at pcm[inoff[i]].  -> (out, offsets, lengths)
     as pcm_frontend_batch returns them."""
@@ -189,17 +250,26 @@ def _frontend_packed(ctx, pcm, inoff, nfr, channels, src_rates, dst_rate):
     ch = np.array([int(c) for c in channels], np.int32)
     nfr = np.ascontiguousarray(nfr, dtype=np.int64)
     inoff = np.ascontiguousarray(inoff, dtype=np.int64)
+    P = C.POINTER(C.c_int64)
+    ptr, on_host = _lib.ptr_of(pcm)
+    plen = len(pcm) if isinstance(pcm, np.ndarray) else pcm.numel()
+    off = np.zeros(n + 1, np.int64)
+    lens = np.zeros(n, np.int64)
+    if _check_resampler(resampler) == 'ffmpeg':
+        rates = np.array([int(fs) for fs in src_rates], np.int32)
+        args = [ctx.h, ptr if plen else None, on_host, plen, n, inoff.ctypes.data_as(P), nfr.ctypes.data_as(P),
+                ch.ctypes.data, rates.ctypes.data, int(dst_rate)]
+        ctx.check(ctx.lib.afp_swr_frontend_batch(*args, None, 0, off.ctypes.data_as(P), lens.ctypes.data_as(P)))
+        out = torch.zeros(int(off[-1]) + 4, dtype=torch.float32, device=torch.device("cuda", ctx.device))
+        with ctx.after_torch(out, pcm):
+            ctx.check(ctx.lib.afp_swr_frontend_batch(*args, out.data_ptr(), out.numel(), None, None))
+        return out, off, lens
     up, down = np.ones(n, np.int32), np.ones(n, np.int32)
     for i, fs in enumerate(src_rates):
         if dst_rate is not None and int(dst_rate) != int(fs):
             g = gcd(int(dst_rate), int(fs))
             up[i], down[i] = int(dst_rate) // g, int(fs) // g
     rates, toff, taps = taps_table(zip(up, down))
-    off = np.zeros(n + 1, np.int64)
-    lens = np.zeros(n, np.int64)
-    P = C.POINTER(C.c_int64)
-    ptr, on_host = _lib.ptr_of(pcm)
-    plen = len(pcm) if isinstance(pcm, np.ndarray) else pcm.numel()
     args = [ctx.h, ptr if plen else None, on_host, plen, n, inoff.ctypes.data_as(P),
             nfr.ctypes.data_as(P), ch.ctypes.data, up.ctypes.data, down.ctypes.data, len(rates), rates.ctypes.data,
             toff.ctypes.data_as(P), taps.ctypes.data]
@@ -211,7 +281,7 @@ def _frontend_packed(ctx, pcm, inoff, nfr, channels, src_rates, dst_rate):
     return out, off, lens
 
 
-def _frontend_sources(sources, channels, src_rates, dst_rate, device=None):
+def _frontend_sources(sources, channels, src_rates, dst_rate, device=None, resampler='poly'):
     """pcm_frontend_batch over files given as int16 PCM or as flac.FlacStream.  With FLAC files among
     them, the round's int16 buffer is built on the device: the PCM files go up in one copy, the FLAC
     files are located (one call) and decoded in place after them (one call), and one front-end call
@@ -222,7 +292,7 @@ def _frontend_sources(sources, channels, src_rates, dst_rate, device=None):
     status = np.zeros(n, np.int32)
     fl = [k for k, s in enumerate(sources) if isinstance(s, flac.FlacStream)]
     if not fl:
-        return pcm_frontend_batch(sources, channels, src_rates, dst_rate, device=device) + (status,)
+        return pcm_frontend_batch(sources, channels, src_rates, dst_rate, device=device, resampler=resampler) + (status,)
     ctx = _lib.context(device)
     nsamples, _ = flac.locate(ctx, [sources[k] for k in fl])
     is_flac = set(fl)
@@ -247,7 +317,7 @@ def _frontend_sources(sources, channels, src_rates, dst_rate, device=None):
     for j, k in enumerate(fl):
         if fst[j]:
             status[k], nfr[k] = fst[j], 0
-    return _frontend_packed(ctx, pcm, inoff, nfr, channels, src_rates, dst_rate) + (status,)
+    return _frontend_packed(ctx, pcm, inoff, nfr, channels, src_rates, dst_rate, resampler) + (status,)
 
 
 class _ChunkPlanner(object):
@@ -378,7 +448,7 @@ class Analyzer(object):
                                soundfiledur=0.0, soundfiletotaldur=0.0, soundfilecount=0,
                                fail_on_error=True)
 
-    def __init__(self, density=DENSITY, device=None):
+    def __init__(self, density=DENSITY, device=None, resampler='poly'):
         self.density = density
         for attr, default in self._REFERENCE_DEFAULTS.items():
             setattr(self, attr, default)
@@ -388,6 +458,10 @@ class Analyzer(object):
         self.device = device
         self.precision = 'fp64'
         self.reader = _wav_reader
+        # how the default reader down-mixes and resamples: 'poly' (the channel mean and a
+        # resample_poly FIR) or 'ffmpeg' (ffmpeg's own arithmetic, so files at any supported rate
+        # give the reference's hashes)
+        self.resampler = _check_resampler(resampler)
 
     # objects are pickled into worker processes by the reference CLI
     # (audfprint.py:218-223,249-265): carry only plain attributes
@@ -400,6 +474,7 @@ class Analyzer(object):
     def __setstate__(self, st):
         self.__dict__.update(st)
         self.__dict__.setdefault("precision", "fp64")
+        self.__dict__.setdefault("resampler", "poly")
         if self.reader is None:
             self.reader = _wav_reader
 
@@ -591,7 +666,11 @@ class Analyzer(object):
 
     def _read(self, filename):
         try:
-            d, sr = self.reader(filename, sr=self.target_sr, channels=1)
+            if self.reader is _wav_reader:
+                d, sr = _wav_reader(filename, sr=self.target_sr, channels=1,
+                                    resampler=_check_resampler(self.resampler))
+            else:
+                d, sr = self.reader(filename, sr=self.target_sr, channels=1)
         except Exception as e:
             self._read_failed(filename, e)
             d, sr = [], self.target_sr
@@ -789,10 +868,14 @@ class Analyzer(object):
                     # the per-file reader fails here in the device front-end (down < 1)
                     raise ValueError("%s: sample rate %d" % (fn, fs))
                 nframes = len(raw) // nch if isinstance(raw, np.ndarray) else self._flac_frames(raw)
+                if _check_resampler(self.resampler) == 'ffmpeg':
+                    _swr_check(fn, raw, nch, fs, self.target_sr)
+                    nout = swr_length(nframes, fs, self.target_sr)
+                else:
+                    nout = -(-nframes * self.target_sr // fs)      # ceil(nframes * up / down)
             except Exception as e:
                 self._read_failed(fn, e)
-                raw, nch, fs, nframes = np.zeros(0, np.int16), 1, self.target_sr, 0
-            nout = -(-nframes * self.target_sr // fs)      # ceil(nframes * up / down)
+                raw, nch, fs, nframes, nout = np.zeros(0, np.int16), 1, self.target_sr, 0, 0
             if nout == 0:
                 return 'host', (i, None, 0.0), 0, 0
             nbytes = raw.nbytes if isinstance(raw, np.ndarray) else 2 * nframes * nch     # decoded int16
@@ -823,7 +906,8 @@ class Analyzer(object):
         if self.reader is _wav_reader:
             raws = [it[1] for it in items]
             out, off, lens, status = _frontend_sources([r[0] for r in raws], [r[1] for r in raws],
-                                                       [r[2] for r in raws], self.target_sr, device=self.device)
+                                                       [r[2] for r in raws], self.target_sr, device=self.device,
+                                                       resampler=_check_resampler(self.resampler))
             for i, ln in zip(idx, lens):
                 durs[i] = int(ln) / self.target_sr
             self.fingerprint_packed(out, off, shifts, fetch=False, sample_lengths=lens)

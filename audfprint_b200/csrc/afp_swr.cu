@@ -1,0 +1,288 @@
+// ffmpeg front-end on the device: interleaved int16 mono or stereo PCM -> the mono int16 stream
+// `ffmpeg -i F -f s16le -ac 1 -ar 11025 -` writes for it (audio_read.py:196-203), scaled to float32
+// v / 32768 as the reference's reader does.  libswresample (FFmpeg 8.0, library defaults) does:
+//
+//   equal rates   s16 arithmetic: stereo -> (16384 (l + r) + 16384) >> 15, mono as it is.
+//   other rates   float32 arithmetic on x / 32768: each channel through a polyphase FIR of P phases
+//                 x L taps (afp_swr_design), output n at input position n D / P (D = in / g,
+//                 P = out / g <= 1024), summed as the library's x86 FMA3 kernel sums: eight lanes,
+//                 lane k accumulating taps k, k+8, ... by fused multiply-add, then the lanes folded
+//                 (k, k+4), (k, k+2), (0, 1).  Stereo: 0.5 l + 0.5 r of the two resampled channels.
+//                 Then lrintf(v * 32768), clipped to int16.  Edges: the input is mirrored around its
+//                 last sample for R samples and then around sample 0 (swr_edges).
+//
+// tests/swr_reference.py states the same in NumPy; tests/test_ffmpeg_frontend_cpu.py holds it to the
+// library's own output and tests/test_gpu_ffmpeg_frontend.py holds this kernel to both.  One thread
+// computes one output and reads its taps from global memory through the cache.  A design has P L
+// floats: 1 KB at 22050 Hz, 83 KB at 48000 Hz, up to 166 KB (32000 and 96000 Hz: 441 and 147 phases).
+// tools/ffmpeg_frontend_timing.py measures the kernel against afp_pcm_frontend_batch.
+#include <cmath>
+#include <cstring>
+#include <map>
+#include <mutex>
+#include <numeric>
+
+#include "afp_internal.cuh"
+
+namespace {
+
+// 176400 Hz (528 taps) is held to the library; 192000 Hz (575 taps) is not yet, so longer designs are refused
+constexpr int kFilterSize = 32, kPhaseCount = 1024, kLanes = 8, kMaxTaps = 528;
+constexpr double kCutoff = 0.97, kBeta = 9.0;
+
+struct SwrGeometry {
+  int32_t P, D, L;
+  double factor;
+};
+
+bool swr_geometry(int32_t in_rate, int32_t out_rate, SwrGeometry* g) {
+  if (in_rate < 1 || out_rate < 1) return false;
+  const int32_t d = std::gcd(in_rate, out_rate);
+  g->P = out_rate / d;
+  g->D = in_rate / d;
+  if (g->P > kPhaseCount) return false;               // needs interpolated phases
+  g->factor = std::min(out_rate * kCutoff / in_rate, 1.0);
+  g->L = std::max((int32_t)std::ceil(kFilterSize / g->factor), 1);
+  return g->L <= kMaxTaps;
+}
+
+double bessel_i0(double x) {  // power series, summed until the terms stop changing the sum
+  double s = 1.0, t = 1.0;
+  const double q = x * x / 4.0;
+  for (int k = 1;; ++k) {
+    t *= q / ((double)k * k);
+    if (s + t == s) return s;
+    s += t;
+  }
+}
+
+void swr_design(const SwrGeometry& g, float* bank) {
+  const int P = g.P, L = g.L, center = (L - 1) / 2;
+  std::vector<double> tab((size_t)L);
+  double norm = 0.0;
+  const int nph = (P % 2) ? P : P / 2 + 1;
+  for (int ph = 0; ph < nph; ++ph) {
+    double s = g.factor == 1.0 ? std::sin(M_PI * ph / P) * ((center & 1) ? 1 : -1) : 0.0;
+    for (int i = 0; i < L; ++i) {
+      const double x = M_PI * ((double)(i - center) - (double)ph / P) * g.factor;
+      double y = x == 0 ? 1.0 : (g.factor == 1.0 ? s / x : std::sin(x) / x);
+      const double w = 2.0 * x / (g.factor * L * M_PI);
+      y *= bessel_i0(kBeta * std::sqrt(std::max(1 - w * w, 0.0)));
+      tab[i] = y;
+      s = -s;
+      if (ph == 0) norm += y;
+    }
+    for (int i = 0; i < L; ++i) bank[(size_t)ph * L + i] = (float)(tab[i] / norm);
+    if (P % 2 == 0 && ph > 0)
+      for (int i = 0; i < L; ++i) bank[(size_t)(P - ph) * L + L - 1 - i] = bank[(size_t)ph * L + i];
+  }
+}
+
+// outputs for n input frames, as the library's buffering gives them: the end is mirrored for R samples
+int64_t swr_edges(const SwrGeometry& g, int64_t n) {
+  const int64_t P = g.P, D = g.D, L = g.L, S = (L - 1) / 2 + n;
+  int64_t R;
+  if (n <= L) {
+    R = (n + 1) / 2;
+    if (n + R <= L) return 0;
+  } else {
+    const int64_t made = ((S - L + 1) * P - 1) / D + 1;   // outputs before the end is reflected
+    R = (std::min(S - made * D / P, L) + 1) / 2;
+  }
+  return ((S + R - L + 1) * P - 1) / D + 1;
+}
+
+// designs cached per (in, out) rate pair for the process
+std::mutex g_design_mu;
+std::map<std::pair<int32_t, int32_t>, std::vector<float>> g_designs;
+
+const std::vector<float>& cached_design(int32_t in_rate, int32_t out_rate, const SwrGeometry& g) {
+  std::lock_guard<std::mutex> lk(g_design_mu);
+  auto& v = g_designs[{in_rate, out_rate}];
+  if (v.empty()) {
+    v.resize((size_t)g.P * g.L);
+    swr_design(g, v.data());
+  }
+  return v;
+}
+
+struct SwrFileDesc {
+  int64_t in_off, nframes, out_off, nout, bank_off, block_base;
+  int32_t ch, P, D, L, resample;
+};
+
+// sample c of extended input position e: mirrored around the end, then around 0 (the output count keeps
+// e within the reflected samples)
+__device__ __forceinline__ float swr_in(const int16_t* pcm, int64_t n, int ch, int c, int64_t e) {
+  if (e < 0) e = -e;
+  if (e >= n) e = 2 * n - 1 - e;
+  return (float)pcm[e * ch + c] * (1.0f / 32768.0f);
+}
+
+__device__ __forceinline__ float swr_channel(const int16_t* pcm, const SwrFileDesc& f, const float* taps, int64_t start,
+                                             int c) {
+  float lane[kLanes];
+#pragma unroll
+  for (int k = 0; k < kLanes; ++k) lane[k] = 0.0f;
+  for (int j = 0; j < f.L; j += kLanes) {
+#pragma unroll
+    for (int k = 0; k < kLanes; ++k)
+      if (j + k < f.L) lane[k] = __fmaf_rn(swr_in(pcm, f.nframes, f.ch, c, start + j + k), __ldg(taps + j + k), lane[k]);
+  }
+  float a[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) a[k] = __fadd_rn(lane[k], lane[k + 4]);
+  return __fadd_rn(__fadd_rn(a[0], a[2]), __fadd_rn(a[1], a[3]));
+}
+
+__device__ __forceinline__ float swr_sample(const int16_t* pcm, const SwrFileDesc& f, const float* bank, int64_t n) {
+  if (!f.resample) {
+    if (f.ch == 1) return (float)pcm[n] * (1.0f / 32768.0f);
+    const int v = (16384 * ((int)pcm[2 * n] + (int)pcm[2 * n + 1]) + 16384) >> 15;
+    return (float)v * (1.0f / 32768.0f);
+  }
+  const int64_t k = n * f.D;
+  const int64_t start = k / f.P - (f.L - 1) / 2;
+  const float* taps = bank + (k % f.P) * f.L;
+  float v = swr_channel(pcm, f, taps, start, 0);
+  if (f.ch == 2) v = __fadd_rn(__fmul_rn(v, 0.5f), __fmul_rn(swr_channel(pcm, f, taps, start, 1), 0.5f));
+  const int s = min(max(__float2int_rn(__fmul_rn(v, 32768.0f)), -32768), 32767);
+  return (float)s * (1.0f / 32768.0f);
+}
+
+__global__ void __launch_bounds__(256) afp_swr_frontend_kernel(const int16_t* pcm, const SwrFileDesc* files, int nfiles,
+                                                              const float* banks, float* out) {
+  __shared__ int s_file;
+  const int64_t b = blockIdx.x;
+  if (threadIdx.x == 0) {
+    int lo = 0, hi = nfiles - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (files[mid].block_base <= b) lo = mid; else hi = mid - 1;
+    }
+    s_file = lo;
+  }
+  __syncthreads();
+  const SwrFileDesc f = files[s_file];
+  const int64_t n = (b - f.block_base) * blockDim.x + threadIdx.x;
+  if (n >= f.nout) return;
+  out[f.out_off + n] = swr_sample(pcm + f.in_off, f, banks + f.bank_off, n);
+}
+
+}  // namespace
+
+extern "C" int afp_swr_design(int32_t in_rate, int32_t out_rate, float* bank, int64_t capacity, int32_t* phases,
+                              int32_t* taps) {
+  SwrGeometry g;
+  if (in_rate < 1 || out_rate < 1) return AFP_ERR_INVALID;
+  if (!swr_geometry(in_rate, out_rate, &g)) return AFP_ERR_UNSUPPORTED;
+  if (phases) *phases = g.P;
+  if (taps) *taps = g.L;
+  if (!bank) return AFP_OK;
+  if (capacity < (int64_t)g.P * g.L) return AFP_ERR_INVALID;
+  swr_design(g, bank);
+  return AFP_OK;
+}
+
+extern "C" int afp_swr_length(int64_t nframes, int32_t in_rate, int32_t out_rate, int64_t* nout) {
+  SwrGeometry g;
+  if (nframes < 0 || in_rate < 1 || out_rate < 1 || !nout) return AFP_ERR_INVALID;
+  if (in_rate == out_rate) {
+    *nout = nframes;
+    return AFP_OK;
+  }
+  if (!swr_geometry(in_rate, out_rate, &g)) return AFP_ERR_UNSUPPORTED;
+  if (nframes > (INT64_MAX / 2 - g.L) / g.P) return AFP_ERR_INVALID;
+  *nout = swr_edges(g, nframes);
+  return AFP_OK;
+}
+
+extern "C" int afp_swr_frontend_batch(afp_ctx* c, const int16_t* pcm, int pcm_on_host, int64_t pcm_len, int32_t nfiles,
+                                      const int64_t* pcm_offsets, const int64_t* nframes, const int32_t* channels,
+                                      const int32_t* rates, int32_t out_rate, float* out, int64_t out_capacity,
+                                      int64_t* out_offsets, int64_t* out_lengths) {
+  if (!c) return AFP_ERR_INVALID;
+  if (nfiles < 0 || pcm_len < 0) AFP_FAIL(c, AFP_ERR_INVALID, "negative count");
+  if (out_rate < 1) AFP_FAIL(c, AFP_ERR_INVALID, "output rate must be >= 1");
+  if (nfiles > 0 && (!pcm_offsets || !nframes || !channels || !rates)) AFP_FAIL(c, AFP_ERR_INVALID, "null per-file array");
+  std::vector<SwrFileDesc> d((size_t)nfiles);
+  std::vector<std::pair<int32_t, const std::vector<float>*>> uniq;   // distinct input rates, first use first
+  int64_t o = 0, blocks = 0, nbank = 0;
+  for (int f = 0; f < nfiles; ++f) {
+    SwrFileDesc& x = d[f];
+    const std::string tag = "file " + std::to_string(f) + ": ";
+    x.nframes = nframes[f];
+    x.ch = channels[f];
+    x.in_off = pcm_offsets[f];
+    if (x.nframes < 0) AFP_FAIL(c, AFP_ERR_INVALID, tag + "negative length");
+    if (x.ch < 1) AFP_FAIL(c, AFP_ERR_INVALID, tag + "channels must be >= 1");
+    if (rates[f] < 1) AFP_FAIL(c, AFP_ERR_INVALID, tag + "sample rate must be >= 1");
+    if (x.ch > 2) AFP_FAIL(c, AFP_ERR_UNSUPPORTED, tag + "the ffmpeg front-end takes mono or stereo");
+    if (x.nframes > 0 && (x.in_off < 0 || x.in_off > pcm_len || x.nframes > (pcm_len - x.in_off) / x.ch))
+      AFP_FAIL(c, AFP_ERR_INVALID, tag + "input range outside the PCM buffer");
+    x.resample = rates[f] != out_rate;
+    x.P = x.D = x.L = 1;
+    x.bank_off = 0;
+    x.nout = x.nframes;
+    if (x.resample) {
+      SwrGeometry g;
+      if (!swr_geometry(rates[f], out_rate, &g))
+        AFP_FAIL(c, AFP_ERR_UNSUPPORTED, tag + std::to_string(rates[f]) + " Hz needs interpolated phases or more than 528 taps");
+      if (x.nframes > (INT64_MAX / 2 - g.L) / g.P) AFP_FAIL(c, AFP_ERR_INVALID, tag + "too long");
+      x.P = g.P;
+      x.D = g.D;
+      x.L = g.L;
+      x.nout = swr_edges(g, x.nframes);
+      size_t u = 0;
+      int64_t off = 0;
+      while (u < uniq.size() && uniq[u].first != rates[f]) off += (int64_t)uniq[u++].second->size();
+      if (u == uniq.size()) {
+        uniq.push_back({rates[f], &cached_design(rates[f], out_rate, g)});
+        nbank += (int64_t)g.P * g.L;
+      }
+      x.bank_off = off;
+    }
+    x.out_off = o;
+    x.block_base = blocks;
+    o += (x.nout + 3) & ~(int64_t)3;
+    blocks += (x.nout + 255) / 256;
+  }
+  if (blocks > INT32_MAX) AFP_FAIL(c, AFP_ERR_INVALID, "batch too large for one launch");
+  if (out) {
+    if (o > out_capacity) AFP_FAIL(c, AFP_ERR_INVALID, "output buffer smaller than the batch's " + std::to_string(o) + " samples");
+    if (blocks > 0 && !pcm) AFP_FAIL(c, AFP_ERR_INVALID, "null pcm");
+  }
+  if (out_offsets) {
+    for (int f = 0; f < nfiles; ++f) out_offsets[f] = d[f].out_off;
+    out_offsets[nfiles] = o;
+  }
+  if (out_lengths)
+    for (int f = 0; f < nfiles; ++f) out_lengths[f] = d[f].nout;
+  if (!out || blocks == 0) return AFP_OK;                                 // sizing call, or nothing to compute
+  AFP_CUDA(c, cudaSetDevice(c->device));
+  const int16_t* dpcm = nullptr;
+  int rc = afp_stage(c, c->d_pcm_stage, pcm, (size_t)pcm_len, pcm_on_host, &dpcm);
+  if (rc) return rc;
+  if (pcm_on_host) c->batch_valid = false;   // the PCM staging buffer of the last fingerprint batch is overwritten
+  // descriptors and every distinct rate's design in one upload
+  SwrFileDesc* dd = nullptr;
+  float* dbank = nullptr;
+  size_t desc_bytes = 0;
+  if ((rc = afp_carve(c, c->d_tmp, [&](Carver& k) {
+         dd = k.take<SwrFileDesc>(nfiles);
+         desc_bytes = k.bytes;
+         dbank = k.take<float>(nbank);
+       })))
+    return rc;
+  std::vector<char> h(desc_bytes + sizeof(float) * (size_t)nbank);
+  memcpy(h.data(), d.data(), sizeof(SwrFileDesc) * (size_t)nfiles);
+  size_t pos = desc_bytes;
+  for (auto& u : uniq) {
+    memcpy(h.data() + pos, u.second->data(), sizeof(float) * u.second->size());
+    pos += sizeof(float) * u.second->size();
+  }
+  AFP_CUDA(c, afp_copy_in(c, reinterpret_cast<char*>(dd), h.data(), h.size(), 1));
+  if ((rc = afp_launch(c, afp_swr_frontend_kernel, (unsigned)blocks, 256, 0, dpcm, dd, nfiles, dbank, out))) return rc;
+  AFP_CUDA(c, cudaStreamSynchronize(c->stream));       // one synchronise for the whole list (`h` is pageable)
+  return AFP_OK;
+}

@@ -163,6 +163,34 @@ int afp_pcm_frontend_batch(afp_ctx* ctx, const int16_t* pcm, int pcm_on_host, in
                            const int64_t* tap_offsets, const double* taps, float* out, int64_t out_capacity,
                            int64_t* out_offsets, int64_t* out_lengths);
 
+/* ---- ffmpeg front-end (audfprint_b200/csrc/afp_swr.cu) ----
+ * What `ffmpeg -i F -f s16le -ac 1 -ar <out_rate> -` (the reference's reader, audio_read.py:196-203)
+ * makes of 16-bit mono or stereo PCM, bit for bit, scaled to float32 v / 32768: libswresample's s16
+ * down-mix at equal rates, and at other rates its float32 polyphase resampler (Kaiser, beta 9,
+ * cut-off 0.97, 32 taps per output period, exact-rational phases) summed in the order of its x86 FMA3
+ * kernel, with its edge reflections and output count.  tests/swr_reference.py states it in NumPy.
+ *
+ * afp_swr_design: the float32 bank of in_rate -> out_rate, host only (no device, no context):
+ * *phases = P, *taps = L (either may be NULL) and, when bank is not NULL, P x L floats (row p = phase
+ * p) into bank[0 .. capacity).  AFP_ERR_UNSUPPORTED when out / gcd(in, out) > 1024 (a rate such as
+ * 44099 Hz needs interpolated phases) or a design longer than 528 taps (above 176400 Hz, not yet
+ * matched to the library); AFP_ERR_INVALID for a rate < 1 or a capacity below P L. */
+int afp_swr_design(int32_t in_rate, int32_t out_rate, float* bank, int64_t capacity, int32_t* phases, int32_t* taps);
+/* afp_swr_length: host only, *nout = the samples afp_swr_frontend_batch gives a mono or stereo file of
+ * nframes frames at in_rate (nframes itself at equal rates).  AFP_ERR_UNSUPPORTED for a rate
+ * afp_swr_design refuses; AFP_ERR_INVALID for nframes < 0, a rate < 1, NULL nout or a file too long. */
+int afp_swr_length(int64_t nframes, int32_t in_rate, int32_t out_rate, int64_t* nout);
+/* afp_swr_frontend_batch: the layout and calls of afp_pcm_frontend_batch (a sizing call with out =
+ * NULL, then the compute call; pcm HOST or DEVICE; out DEVICE in afp_fingerprint_batch's packed layout),
+ * with each file's input rate in `rates` HOST int32 [nfiles] instead of up/down and taps: the library
+ * designs each distinct rate once per process and uploads it once per call.  out_lengths are the
+ * library's output counts.  AFP_ERR_UNSUPPORTED for more than 2 channels or a rate afp_swr_design
+ * refuses; AFP_ERR_INVALID as afp_pcm_frontend_batch.  One launch and one synchronise per call. */
+int afp_swr_frontend_batch(afp_ctx* ctx, const int16_t* pcm, int pcm_on_host, int64_t pcm_len, int32_t nfiles,
+                           const int64_t* pcm_offsets, const int64_t* nframes, const int32_t* channels,
+                           const int32_t* rates, int32_t out_rate, float* out, int64_t out_capacity,
+                           int64_t* out_offsets, int64_t* out_lengths);
+
 /* ---- FLAC decoding -----------------------------------------------------------
  * What the reference's `ffmpeg -i F -f s16le` does for a FLAC file, up to the int16 stream the PCM
  * front-end takes: the frames of a list of FLAC streams are decoded on the device into interleaved
