@@ -14,7 +14,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libafp.so")
 HEADER = os.path.join(os.path.dirname(_HERE), "include", "afp.h")
 
-PCM_I16, PCM_F32 = 0, 1
+PCM_I16, PCM_F32, PCM_S24, PCM_S32 = 0, 1, 2, 3
 
 
 class AfpError(RuntimeError):
@@ -59,12 +59,17 @@ _SIGS = {
                                    C.c_int, _I64P]),
     "afp_pcm_frontend_batch": (C.c_int, [_P, _P, C.c_int, C.c_int64, C.c_int32, _I64P, _I64P, _P, _P, _P, C.c_int32,
                                          _P, _I64P, _P, _P, C.c_int64, _I64P, _I64P]),
+    "afp_pcm_frontend_batch_bytes": (C.c_int, [_P, _P, C.c_int, C.c_int64, C.c_int32, _I64P, _P, _I64P, _P, _P, _P,
+                                               C.c_int32, _P, _I64P, _P, _P, C.c_int64, _I64P, _I64P]),
     "afp_swr_design": (C.c_int, [C.c_int32, C.c_int32, _P, C.c_int64, _P, _P]),
     "afp_swr_length": (C.c_int, [C.c_int64, C.c_int32, C.c_int32, _I64P]),
     "afp_swr_frontend_batch": (C.c_int, [_P, _P, C.c_int, C.c_int64, C.c_int32, _I64P, _I64P, _P, _P, C.c_int32, _P,
                                          C.c_int64, _I64P, _I64P]),
+    "afp_swr_frontend_batch_bytes": (C.c_int, [_P, _P, C.c_int, C.c_int64, C.c_int32, _I64P, _P, _I64P, _P, _P,
+                                               C.c_int32, _P, C.c_int64, _I64P, _I64P]),
     "afp_flac_locate_batch": (C.c_int, [_P, _P, C.c_int, C.c_int64, C.c_int32, C.POINTER(FlacStream), _I64P, _P]),
     "afp_flac_decode_batch": (C.c_int, [_P, _P, C.c_int64, _I64P, _P]),
+    "afp_flac_decode_batch_bytes": (C.c_int, [_P, _P, C.c_int64, _I64P, C.c_int32, _P]),
     "afp_set_analyzer": (C.c_int, [_P, C.POINTER(AnalyzerParams), _P, _P, C.c_double]),
     "afp_fingerprint_batch": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int32, _I64P, _I64P, _I64P]),
     "afp_fetch_hashes": (C.c_int, [_P, _P, C.c_int, _I64P]),

@@ -67,13 +67,39 @@ def resample_taps(up, down):
     return np.ascontiguousarray(firwin(2 * half + 1, 1.0 / max_rate, window=('kaiser', 5.0)) * up, dtype=np.float64)
 
 
-def pcm_frontend(raw, channels, src_rate, dst_rate=None, device=None, to_host=True, resampler='poly'):
+# sample formats of the front-ends (afp.h AFP_PCM_*), by name
+SAMPLE_FORMATS = {'s16': _lib.PCM_I16, 's24': _lib.PCM_S24, 's32': _lib.PCM_S32, 'f32': _lib.PCM_F32}
+_WIDTH = {_lib.PCM_I16: 2, _lib.PCM_S24: 3, _lib.PCM_S32: 4, _lib.PCM_F32: 4}
+
+
+def _as_payload(raw, sample_format):
+    """One file's samples -> (payload bytes as uint8, AFP_PCM_* code).  sample_format None: int16 as
+    pcm_frontend has always taken it (values converted to int16).  Otherwise 's16', 's24', 's32' or 'f32':
+    `raw` holds the data chunk's little-endian bytes, in any array type (a 24-bit file as uint8 bytes)."""
+    if sample_format is None:
+        return np.ascontiguousarray(raw, dtype=np.int16).reshape(-1).view(np.uint8), _lib.PCM_I16
+    if sample_format not in SAMPLE_FORMATS:
+        raise ValueError("sample_format must be one of %s" % ", ".join(sorted(SAMPLE_FORMATS)))
+    code = SAMPLE_FORMATS[sample_format]
+    b = np.ascontiguousarray(raw).reshape(-1).view(np.uint8)
+    return b[:len(b) // _WIDTH[code] * _WIDTH[code]], code
+
+
+def pcm_frontend(raw, channels, src_rate, dst_rate=None, device=None, to_host=True, resampler='poly',
+                 sample_format=None):
     """Interleaved int16 PCM -> mono float32 at dst_rate, on the device (afp_pcm_frontend:
     channel mean, 1/32768 scaling, polyphase resampling).  Returns a NumPy array, or with
     to_host=False a torch CUDA tensor that Analyzer.fingerprint_packed takes as it is.
     resampler='ffmpeg' gives instead the bits `ffmpeg -ac 1 -ar dst_rate` gives, v / 32768
-    (afp_swr_frontend_batch; mono or stereo, and rates with out / gcd <= 1024)."""
+    (afp_swr_frontend_batch; mono or stereo, and rates with out / gcd <= 1024).
+    sample_format 's24', 's32' or 'f32' (or 's16') takes `raw` as a WAV data chunk's bytes of that
+    format (_as_payload) and runs the byte form of the same front-end (pcm_frontend_batch)."""
     from math import gcd
+    if sample_format is not None:
+        out, off, lens = pcm_frontend_batch([raw], [channels], [src_rate], dst_rate if dst_rate is not None else src_rate,
+                                            device=device, resampler=resampler, sample_formats=[sample_format])
+        out = out[:int(lens[0])].clone()
+        return out.cpu().numpy() if to_host else out
     raw = np.ascontiguousarray(raw, dtype=np.int16).reshape(-1)
     if _check_resampler(resampler) == 'ffmpeg':
         out, off, lens = pcm_frontend_batch([raw], [channels], [src_rate], dst_rate if dst_rate is not None else src_rate,
@@ -104,15 +130,89 @@ def pcm_frontend(raw, channels, src_rate, dst_rate=None, device=None, to_host=Tr
     return out
 
 
+_GUID_TAIL = b"\x00\x00\x10\x00\x80\x00\x00\xaa\x00\x38\x9b\x71"      # KSDATAFORMAT_SUBTYPE_* after Data1
+_WAVE_PCM, _WAVE_FLOAT, _WAVE_EXTENSIBLE = 1, 3, 0xFFFE
+
+
+def _wav_format(fmt):
+    """A fmt chunk -> (AFP_PCM_* code, channels, rate).  Raises for the codings the front-ends do not
+    take, with the message the wave module gave them: 8-bit PCM, 64-bit float, A-law, mu-law, ADPCM..."""
+    if len(fmt) < 16:
+        raise EOFError
+    tag, nch, fs, _, _, bits = struct.unpack_from('<HHIIHH', fmt)
+    sub = tag
+    if tag == _WAVE_EXTENSIBLE:
+        if len(fmt) < 40:
+            raise EOFError
+        guid = fmt[24:40]
+        sub = int.from_bytes(guid[:4], 'little') if guid[4:] == _GUID_TAIL else None
+        if sub not in (_WAVE_PCM, _WAVE_FLOAT) or (sub == _WAVE_FLOAT and bits != 32):
+            import uuid
+            raise wave.Error('unknown extended format: %s' % uuid.UUID(bytes_le=guid))
+        valid = struct.unpack_from('<H', fmt, 18)[0]
+        if sub == _WAVE_PCM and bits == 32 and 0 < valid < 32:
+            # ffmpeg reads such a file as packed 24-bit samples, which it is not
+            raise IOError("32-bit PCM WAV with %d valid bits is not supported" % valid)
+    elif tag not in (_WAVE_PCM, _WAVE_FLOAT) or (tag == _WAVE_FLOAT and bits != 32):
+        raise wave.Error('unknown format: %r' % (tag,))
+    width = (bits + 7) // 8
+    if not width:
+        raise wave.Error('bad sample width')
+    if not nch:
+        raise wave.Error('bad # of channels')
+    if sub == _WAVE_FLOAT:
+        return _lib.PCM_F32, nch, fs
+    if width not in (2, 3, 4):
+        raise IOError("only 16-bit PCM WAV is supported, got %d-byte samples" % width)
+    return {2: _lib.PCM_I16, 3: _lib.PCM_S24, 4: _lib.PCM_S32}[width], nch, fs
+
+
+def _wav_parse(filename):
+    """Walk a RIFF WAVE file's chunks (padded to even sizes; unknown ones skipped) to its fmt and data
+    chunks -> (payload uint8, AFP_PCM_* code, channels, rate): the data chunk's bytes as they are, cut to
+    the whole frames present (a data size past the end of the file reads to the end).  Samples are not
+    converted: 16-bit, 24-bit and 32-bit PCM and 32-bit float, plain or WAVE_FORMAT_EXTENSIBLE.  Raises
+    for other files, with the wave module's messages."""
+    with open(filename, 'rb') as f:
+        data = f.read()
+    if len(data) < 8:
+        raise EOFError
+    if data[:4] != b'RIFF':
+        raise wave.Error('file does not start with RIFF id')
+    if data[8:12] != b'WAVE':
+        raise wave.Error('not a WAVE file')
+    pos, form = 12, None
+    while pos + 8 <= len(data):
+        cid, size = data[pos:pos + 4], int.from_bytes(data[pos + 4:pos + 8], 'little')
+        body = data[pos + 8:pos + 8 + size]
+        if cid == b'fmt ':
+            form = _wav_format(body)
+        elif cid == b'data':
+            if form is None:
+                raise wave.Error('data chunk before fmt chunk')
+            code, nch, fs = form
+            frame = _WIDTH[code] * nch
+            payload = np.frombuffer(body, np.uint8)
+            return payload[:len(payload) // frame * frame], code, nch, fs
+        pos += 8 + size + (size & 1)
+    raise wave.Error('fmt chunk and/or data chunk missing')
+
+
 def _wav_read_raw(filename):
-    """The host half of _wav_reader: parse a PCM WAV -> (int16 interleaved samples, channels, rate).
-    Raises what _wav_reader raises for a file it cannot read."""
-    with wave.open(filename, 'rb') as w:
-        nch, width, fs, n = w.getnchannels(), w.getsampwidth(), w.getframerate(), w.getnframes()
-        if width != 2:
-            raise IOError("only 16-bit PCM WAV is supported, got %d-byte samples" % width)
-        raw = np.frombuffer(w.readframes(n), dtype='<i2')
-    return raw, nch, fs
+    """The host half of _wav_reader: parse a WAV (_wav_parse) -> (interleaved samples, channels, rate).
+    The samples are the payload's bytes as they are, typed by format: int16, int32 or float32 arrays, a
+    24-bit file as uint8 (n, 3).  Raises what _wav_reader raises for a file it cannot read."""
+    payload, code, nch, fs = _wav_parse(filename)
+    if code == _lib.PCM_S24:
+        return payload.reshape(-1, 3), nch, fs
+    return payload.view({_lib.PCM_I16: '<i2', _lib.PCM_S32: '<i4', _lib.PCM_F32: '<f4'}[code]), nch, fs
+
+
+def _raw_format(raw):
+    """The sample_format name of an array _wav_read_raw returns."""
+    if raw.dtype == np.uint8:
+        return 's24'
+    return {np.dtype('<i2'): 's16', np.dtype('<i4'): 's32', np.dtype('<f4'): 'f32'}[raw.dtype]
 
 
 def _audio_read_raw(filename):
@@ -191,6 +291,13 @@ def _wav_reader(filename, sr=None, channels=None, device=None, resampler='poly')
     raw, nch, fs = _audio_read_raw(filename)
     if _check_resampler(resampler) == 'ffmpeg':
         _swr_check(filename, raw, nch, fs, fs if sr is None else sr)
+    if (isinstance(raw, np.ndarray) and raw.dtype != np.int16) or \
+            (isinstance(raw, flac.FlacStream) and resampler == 'ffmpeg' and raw.bits_per_sample > 16):
+        # 24-bit, 32-bit and float WAV, and deep FLAC at full depth: the byte form of the front-end
+        out, off, lens, status = _frontend_sources([raw], [nch], [fs], fs if sr is None else sr, device, resampler)
+        if status[0]:
+            raise flac.failure(status[0])
+        return out[:int(lens[0])].cpu().numpy(), (fs if sr is None else sr)
     if isinstance(raw, flac.FlacStream):
         raw = flac.decode(raw, device)
     if nch == 1 and (sr is None or fs == sr):
@@ -224,26 +331,48 @@ def taps_table(pairs):
     return np.array(uniq, np.int32).reshape(-1, 2), off, taps
 
 
-def pcm_frontend_batch(raws, channels, src_rates, dst_rate, device=None, resampler='poly'):
+def pcm_frontend_batch(raws, channels, src_rates, dst_rate, device=None, resampler='poly', sample_formats=None):
     """Many files' interleaved int16 PCM -> mono float32 at dst_rate in ONE device buffer
     (afp_pcm_frontend_batch: one upload of the packed PCM, one launch, one synchronise).
     Every file's samples are bit-identical to pcm_frontend on that file alone.
     Returns (out torch CUDA float32, offsets int64 [n+1], lengths int64 [n]): file i is
     out[offsets[i]:offsets[i] + lengths[i]], starting on a 16-byte boundary - the layout
     Analyzer.fingerprint_packed(out, offsets, sample_lengths=lengths) takes as it is.
-    resampler='ffmpeg': afp_swr_frontend_batch, ffmpeg's down-mix and resampler (pcm_frontend)."""
-    raws = [np.ascontiguousarray(r, dtype=np.int16).reshape(-1) for r in raws]
-    inoff = np.zeros(len(raws) + 1, np.int64)
-    inoff[1:] = np.cumsum([len(r) for r in raws])
-    nfr = [len(r) // max(1, int(c)) for r, c in zip(raws, channels)]
-    packed = np.concatenate(raws) if raws else np.zeros(0, np.int16)
-    return _frontend_packed(_lib.context(device), packed, inoff, nfr, channels, src_rates, dst_rate, resampler)
+    resampler='ffmpeg': afp_swr_frontend_batch, ffmpeg's down-mix and resampler (pcm_frontend).
+    sample_formats: None (every file int16, as always), or one pcm_frontend sample_format per file; the
+    files then go up as their payload bytes and one byte-form call (afp_*_frontend_batch_bytes) runs
+    over every format of the list."""
+    if sample_formats is None:
+        raws = [np.ascontiguousarray(r, dtype=np.int16).reshape(-1) for r in raws]
+        inoff = np.zeros(len(raws) + 1, np.int64)
+        inoff[1:] = np.cumsum([len(r) for r in raws])
+        nfr = [len(r) // max(1, int(c)) for r, c in zip(raws, channels)]
+        packed = np.concatenate(raws) if raws else np.zeros(0, np.int16)
+        return _frontend_packed(_lib.context(device), packed, inoff, nfr, channels, src_rates, dst_rate, resampler)
+    pays = [_as_payload(r, f) for r, f in zip(raws, sample_formats)]
+    packed, boff = _pack_payloads([b for b, _ in pays])
+    fmts = [k for _, k in pays]
+    nfr = [len(b) // _WIDTH[k] // max(1, int(c)) for (b, k), c in zip(pays, channels)]
+    return _frontend_packed(_lib.context(device), packed, boff, nfr, channels, src_rates, dst_rate, resampler, fmts)
 
 
-def _frontend_packed(ctx, pcm, inoff, nfr, channels, src_rates, dst_rate, resampler='poly'):
+def _pack_payloads(payloads, extra=()):
+    """Payload bytes of many files -> (one uint8 buffer, byte offset int64 [n]), every file on a 4-byte
+    boundary; `extra` byte counts get aligned places after them (filled by the caller)."""
+    sizes = [len(b) for b in payloads] + list(extra)
+    boff = np.zeros(len(sizes) + 1, np.int64)
+    boff[1:] = np.cumsum([(n + 3) // 4 * 4 for n in sizes])
+    packed = np.zeros(int(boff[-1]), np.uint8)
+    for b, o in zip(payloads, boff):
+        packed[o:o + len(b)] = b
+    return packed, boff
+
+
+def _frontend_packed(ctx, pcm, inoff, nfr, channels, src_rates, dst_rate, resampler='poly', formats=None):
     """afp_pcm_frontend_batch over files packed in `pcm`, a host int16 array or a device int16 tensor:
-    file i's nfr[i] frames of channels[i] channels start at pcm[inoff[i]].  -> (out, offsets, lengths)
-    as pcm_frontend_batch returns them."""
+    file i's nfr[i] frames of channels[i] channels start at pcm[inoff[i]].  With `formats` (AFP_PCM_* per
+    file) `pcm` is a host uint8 array or device uint8 tensor, `inoff` byte offsets, and the byte form
+    runs (afp_*_frontend_batch_bytes).  -> (out, offsets, lengths) as pcm_frontend_batch returns them."""
     import torch
     from math import gcd
     n = len(nfr)
@@ -255,14 +384,17 @@ def _frontend_packed(ctx, pcm, inoff, nfr, channels, src_rates, dst_rate, resamp
     plen = len(pcm) if isinstance(pcm, np.ndarray) else pcm.numel()
     off = np.zeros(n + 1, np.int64)
     lens = np.zeros(n, np.int64)
+    fmt = None if formats is None else np.ascontiguousarray(formats, dtype=np.int32)
+    form = [] if fmt is None else [fmt.ctypes.data]
     if _check_resampler(resampler) == 'ffmpeg':
         rates = np.array([int(fs) for fs in src_rates], np.int32)
-        args = [ctx.h, ptr if plen else None, on_host, plen, n, inoff.ctypes.data_as(P), nfr.ctypes.data_as(P),
-                ch.ctypes.data, rates.ctypes.data, int(dst_rate)]
-        ctx.check(ctx.lib.afp_swr_frontend_batch(*args, None, 0, off.ctypes.data_as(P), lens.ctypes.data_as(P)))
+        fn = ctx.lib.afp_swr_frontend_batch if fmt is None else ctx.lib.afp_swr_frontend_batch_bytes
+        args = [ctx.h, ptr if plen else None, on_host, plen, n, inoff.ctypes.data_as(P)] + form + \
+               [nfr.ctypes.data_as(P), ch.ctypes.data, rates.ctypes.data, int(dst_rate)]
+        ctx.check(fn(*args, None, 0, off.ctypes.data_as(P), lens.ctypes.data_as(P)))
         out = torch.zeros(int(off[-1]) + 4, dtype=torch.float32, device=torch.device("cuda", ctx.device))
         with ctx.after_torch(out, pcm):
-            ctx.check(ctx.lib.afp_swr_frontend_batch(*args, out.data_ptr(), out.numel(), None, None))
+            ctx.check(fn(*args, out.data_ptr(), out.numel(), None, None))
         return out, off, lens
     up, down = np.ones(n, np.int32), np.ones(n, np.int32)
     for i, fs in enumerate(src_rates):
@@ -270,14 +402,15 @@ def _frontend_packed(ctx, pcm, inoff, nfr, channels, src_rates, dst_rate, resamp
             g = gcd(int(dst_rate), int(fs))
             up[i], down[i] = int(dst_rate) // g, int(fs) // g
     rates, toff, taps = taps_table(zip(up, down))
-    args = [ctx.h, ptr if plen else None, on_host, plen, n, inoff.ctypes.data_as(P),
-            nfr.ctypes.data_as(P), ch.ctypes.data, up.ctypes.data, down.ctypes.data, len(rates), rates.ctypes.data,
+    fn = ctx.lib.afp_pcm_frontend_batch if fmt is None else ctx.lib.afp_pcm_frontend_batch_bytes
+    args = [ctx.h, ptr if plen else None, on_host, plen, n, inoff.ctypes.data_as(P)] + form + \
+           [nfr.ctypes.data_as(P), ch.ctypes.data, up.ctypes.data, down.ctypes.data, len(rates), rates.ctypes.data,
             toff.ctypes.data_as(P), taps.ctypes.data]
-    ctx.check(ctx.lib.afp_pcm_frontend_batch(*args, None, 0, off.ctypes.data_as(P), lens.ctypes.data_as(P)))
+    ctx.check(fn(*args, None, 0, off.ctypes.data_as(P), lens.ctypes.data_as(P)))
     # 16 bytes of zeros past the last file, as Analyzer._pack leaves
     out = torch.zeros(int(off[-1]) + 4, dtype=torch.float32, device=torch.device("cuda", ctx.device))
     with ctx.after_torch(out, pcm):       # the zeros (and a device pcm) land before the library's stream
-        ctx.check(ctx.lib.afp_pcm_frontend_batch(*args, out.data_ptr(), out.numel(), None, None))
+        ctx.check(fn(*args, out.data_ptr(), out.numel(), None, None))
     return out, off, lens
 
 
@@ -291,6 +424,10 @@ def _frontend_sources(sources, channels, src_rates, dst_rate, device=None, resam
     n = len(sources)
     status = np.zeros(n, np.int32)
     fl = [k for k, s in enumerate(sources) if isinstance(s, flac.FlacStream)]
+    full_depth = resampler == 'ffmpeg'
+    if any(s.dtype != np.int16 for s in sources if isinstance(s, np.ndarray)) or \
+            (full_depth and any(sources[k].bits_per_sample > 16 for k in fl)):
+        return _frontend_sources_bytes(sources, fl, channels, src_rates, dst_rate, device, resampler)
     if not fl:
         return pcm_frontend_batch(sources, channels, src_rates, dst_rate, device=device, resampler=resampler) + (status,)
     ctx = _lib.context(device)
@@ -318,6 +455,48 @@ def _frontend_sources(sources, channels, src_rates, dst_rate, device=None, resam
         if fst[j]:
             status[k], nfr[k] = fst[j], 0
     return _frontend_packed(ctx, pcm, inoff, nfr, channels, src_rates, dst_rate, resampler) + (status,)
+
+
+def _frontend_sources_bytes(sources, fl, channels, src_rates, dst_rate, device, resampler):
+    """_frontend_sources over a round that holds 24-bit, 32-bit or float WAV, or FLAC of 17-24 bits in
+    'ffmpeg' mode: every file's payload bytes in one buffer (_pack_payloads), FLAC decoded into it on the
+    device (full depth in 'ffmpeg' mode), one byte-form front-end call with a format per file."""
+    import torch
+    n = len(sources)
+    status = np.zeros(n, np.int32)
+    ctx = _lib.context(device)
+    is_flac = set(fl)
+    wav = [k for k in range(n) if k not in is_flac]
+    fmts, nfr = np.zeros(n, np.int32), np.zeros(n, np.int64)
+    pays = []
+    for k in wav:
+        b, fmts[k] = _as_payload(sources[k], _raw_format(sources[k]))
+        nfr[k] = len(b) // _WIDTH[int(fmts[k])] // max(1, int(channels[k]))
+        pays.append(b)
+    full_depth = resampler == 'ffmpeg'
+    nsamples = flac.locate(ctx, [sources[k] for k in fl])[0] if fl else []
+    extra = []
+    for j, k in enumerate(fl):
+        deep = full_depth and sources[k].bits_per_sample > 16
+        fmts[k] = _lib.PCM_S32 if deep else _lib.PCM_I16
+        nfr[k] = nsamples[j]
+        extra.append(int(nsamples[j]) * int(channels[k]) * _WIDTH[int(fmts[k])])
+    packed, boff = _pack_payloads(pays, extra)
+    inoff = np.zeros(n, np.int64)
+    inoff[wav] = boff[:len(wav)]
+    inoff[fl] = boff[len(wav):len(wav) + len(fl)]
+    if not fl:
+        return _frontend_packed(ctx, packed, inoff, nfr, channels, src_rates, dst_rate, resampler, fmts) + (status,)
+    pcm = torch.zeros(max(len(packed), 1), dtype=torch.uint8, device=torch.device("cuda", ctx.device))
+    wav_len = int(boff[len(wav)])
+    if wav_len:
+        pcm[:wav_len].copy_(torch.from_numpy(packed[:wav_len]))
+    with ctx.after_torch(pcm):            # the payload copy lands before the decode writes after it
+        fst = flac.decode_into_bytes(ctx, pcm, inoff[fl], full_depth)
+    for j, k in enumerate(fl):
+        if fst[j]:
+            status[k], nfr[k] = fst[j], 0
+    return _frontend_packed(ctx, pcm, inoff, nfr, channels, src_rates, dst_rate, resampler, fmts) + (status,)
 
 
 class _ChunkPlanner(object):
@@ -745,8 +924,8 @@ class Analyzer(object):
             return []        # the reference returns [] when there are no peaks (:401-402)
         return hashes
 
-    # bytes of raw PCM (int16 WAV samples, or a custom reader's float32) that wavfiles2hashes stages
-    # per device call
+    # bytes of raw PCM (WAV payload bytes: 2, 3 or 4 a sample; decoded FLAC: 2, or 4 for 17-24 bits in
+    # 'ffmpeg' mode; or a custom reader's float32) that wavfiles2hashes stages per device call
     max_pcm_bytes_per_call = 1 << 30
 
     def wavfiles2hashes(self, filenames):
@@ -878,7 +1057,11 @@ class Analyzer(object):
                 raw, nch, fs, nframes, nout = np.zeros(0, np.int16), 1, self.target_sr, 0, 0
             if nout == 0:
                 return 'host', (i, None, 0.0), 0, 0
-            nbytes = raw.nbytes if isinstance(raw, np.ndarray) else 2 * nframes * nch     # decoded int16
+            if isinstance(raw, np.ndarray):
+                nbytes = raw.nbytes                   # the payload as it goes up: 2, 3 or 4 bytes a sample
+            else:                                     # decoded FLAC: int16, or int32 at full depth
+                deep = self.resampler == 'ffmpeg' and raw.bits_per_sample > 16
+                nbytes = (4 if deep else 2) * nframes * nch
             return 'pcm', (i, (raw, nch, fs), nout, None), nsh * (1 + nout // self.n_hop), nbytes
         d, sr = self._read(fn)
         if len(d) == 0:

@@ -32,7 +32,7 @@ struct FlacFile {
   int64_t gframe_base;  // decode: first frame of the file in the call's frame space
   int64_t nframes;      // decode: frames of the file (0 when it failed to locate)
   int64_t nsamples;     // decode: samples per channel
-  int64_t out_off;      // decode: first int16 of the file in the output
+  int64_t out_off;      // decode: first byte of the file in the output
   int64_t scratch_off;  // decode: first int32 of the file in the scratch
   int32_t rate, channels, bps, max_bs;
   int32_t status;       // AFP_FLAC_DEPTH when the host refused it
@@ -396,7 +396,7 @@ constexpr int DECODE_THREADS = 128;
 __global__ void __launch_bounds__(DECODE_THREADS) flac_decode_kernel(const uint8_t* bytes, const FlacFile* files,
                                                                      int nfiles, const FlacFrame* frames,
                                                                      int64_t total_frames, int32_t* scratch,
-                                                                     int16_t* out, int32_t* status) {
+                                                                     uint8_t* out, int full_depth, int32_t* status) {
   __shared__ int32_t s_coef[DECODE_THREADS][33];
   const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= total_frames) return;
@@ -428,8 +428,9 @@ __global__ void __launch_bounds__(DECODE_THREADS) flac_decode_kernel(const uint8
     atomicMin(status + lo, rc);
     return;
   }
-  int16_t* o = out + f.out_off + fr.sample * nch;
   const int bps = f.bps;
+  const bool s32 = full_depth && bps > 16;          // x << (32 - bps), as FFmpeg's decoder gives it
+  uint8_t* o = out + f.out_off + fr.sample * nch * (s32 ? 4 : 2);
   for (int i = 0; i < bs; ++i) {
     for (int c = 0; c < nch; ++c) {
       int32_t v = s[(int64_t)c * bs + i];
@@ -442,7 +443,11 @@ __global__ void __launch_bounds__(DECODE_THREADS) flac_decode_kernel(const uint8
           v = c == 0 ? (mid + b) >> 1 : (mid - b) >> 1;
         }
       }
-      o[(int64_t)i * nch + c] = (int16_t)(bps <= 16 ? (int32_t)((uint32_t)v << (16 - bps)) : v >> (bps - 16));
+      if (s32)
+        reinterpret_cast<int32_t*>(o)[(int64_t)i * nch + c] = (int32_t)((uint32_t)v << (32 - bps));
+      else
+        reinterpret_cast<int16_t*>(o)[(int64_t)i * nch + c] =
+            (int16_t)(bps <= 16 ? (int32_t)((uint32_t)v << (16 - bps)) : v >> (bps - 16));
     }
   }
 }
@@ -541,8 +546,8 @@ extern "C" int afp_flac_locate_batch(afp_ctx* c, const uint8_t* bytes, int bytes
   return flac_first_failure(c, c->fl.status);
 }
 
-extern "C" int afp_flac_decode_batch(afp_ctx* c, int16_t* out, int64_t out_capacity, const int64_t* out_offsets,
-                                     int32_t* file_status) {
+extern "C" int afp_flac_decode_batch_bytes(afp_ctx* c, uint8_t* out, int64_t out_capacity, const int64_t* out_offsets,
+                                           int32_t full_depth, int32_t* file_status) {
   if (!c) return AFP_ERR_INVALID;
   if (!c->fl.valid) AFP_FAIL(c, AFP_ERR_STATE, "no located FLAC batch (afp_flac_locate_batch)");
   const int nfiles = c->fl.nfiles;
@@ -557,9 +562,11 @@ extern "C" int afp_flac_decode_batch(afp_ctx* c, int16_t* out, int64_t out_capac
     x.gframe_base = gframes;
     x.scratch_off = scratch;
     x.out_off = out_offsets[f];
-    const int64_t len = x.nsamples * x.channels;
-    if (len > 0 && (x.out_off < 0 || x.out_off > out_capacity || len > out_capacity - x.out_off))
+    const int64_t len = x.nsamples * x.channels, width = full_depth && x.bps > 16 ? 4 : 2;
+    if (len > 0 && (x.out_off < 0 || x.out_off > out_capacity || len > (out_capacity - x.out_off) / width))
       AFP_FAIL(c, AFP_ERR_INVALID, "file " + std::to_string(f) + ": output range outside the buffer");
+    if (len > 0 && (reinterpret_cast<uintptr_t>(out) + (uintptr_t)x.out_off) % (uintptr_t)width)
+      AFP_FAIL(c, AFP_ERR_INVALID, "file " + std::to_string(f) + ": output not aligned to its sample width");
     gframes += x.nframes;
     scratch += len;
   }
@@ -579,7 +586,7 @@ extern "C" int afp_flac_decode_batch(afp_ctx* c, int16_t* out, int64_t out_capac
     int rc;
     if ((rc = afp_launch(c, flac_decode_kernel, (unsigned)((gframes + DECODE_THREADS - 1) / DECODE_THREADS),
                          DECODE_THREADS, 0, c->fl.bytes, c->d_fl_file.as<FlacFile>(), nfiles,
-                         c->d_fl_frame.as<FlacFrame>(), gframes, c->d_fl_scratch.as<int32_t>(), out,
+                         c->d_fl_frame.as<FlacFrame>(), gframes, c->d_fl_scratch.as<int32_t>(), out, full_depth,
                          c->d_fl_res.as<int32_t>())) ||
         (rc = afp_read_back(c, dst.data(), c->d_fl_res.as<int32_t>(), (size_t)nfiles)))   // `d` is pageable, too
       return rc;
@@ -589,4 +596,16 @@ extern "C" int afp_flac_decode_batch(afp_ctx* c, int16_t* out, int64_t out_capac
   if (file_status)
     for (int f = 0; f < nfiles; ++f) file_status[f] = st[f];
   return flac_first_failure(c, st);
+}
+
+extern "C" int afp_flac_decode_batch(afp_ctx* c, int16_t* out, int64_t out_capacity, const int64_t* out_offsets,
+                                     int32_t* file_status) {
+  if (!c) return AFP_ERR_INVALID;
+  if (!c->fl.valid) AFP_FAIL(c, AFP_ERR_STATE, "no located FLAC batch (afp_flac_locate_batch)");
+  const int nfiles = c->fl.nfiles;
+  if (nfiles > 0 && !out_offsets) AFP_FAIL(c, AFP_ERR_INVALID, "null out_offsets");
+  if (out_capacity > INT64_MAX / 2) AFP_FAIL(c, AFP_ERR_INVALID, "output capacity too large");
+  std::vector<int64_t> boff((size_t)nfiles + 1);
+  for (int f = 0; f < nfiles; ++f) boff[f] = out_offsets[f] < 0 ? -1 : out_offsets[f] > INT64_MAX / 2 ? INT64_MAX : 2 * out_offsets[f];
+  return afp_flac_decode_batch_bytes(c, reinterpret_cast<uint8_t*>(out), 2 * out_capacity, boff.data(), 0, file_status);
 }

@@ -19,31 +19,34 @@
 // block belongs to one file (a per-file block prefix), each file's output starts on a 16-byte boundary
 // of one device buffer, laid out as afp_fingerprint_batch takes it, and every distinct (up, down)
 // design is uploaded once.  tests/test_gpu_pcm_batch.py holds it bit-equal to afp_pcm_frontend per file.
+// afp_pcm_frontend_batch_bytes is the same call over packed payload bytes with a sample format per file
+// (afp_pcm_formats.cuh): a 24-bit, 32-bit or float sample enters as the int16 `ffmpeg -ac 1` gives it at
+// the file's own rate, at the sample load, so every format runs in the same launch.
 #include <cstring>
 
 #include "afp_internal.cuh"
+#include "afp_pcm_formats.cuh"
 
 namespace {
 
-__device__ __forceinline__ float mono_at(const int16_t* pcm, int64_t j, int ch) {
-  const int16_t* p = pcm + j * ch;
+__device__ __forceinline__ float mono_at(const uint8_t* pcm, int fmt, int64_t j, int ch) {
   float s = 0.0f;
-  for (int c = 0; c < ch; ++c) s += (float)p[c] * (1.0f / 32768.0f);
+  for (int c = 0; c < ch; ++c) s += (float)pcm_s16(pcm, fmt, j * ch + c) * (1.0f / 32768.0f);
   return ch == 1 ? s : s / (float)ch;
 }
 
 // Output n of one file: the down-mix alone (up = down = 1) or the polyphase FIR over it.  The single-file
 // and the batched kernel both call this, so a file gives the same bits through either entry point.
-__device__ __forceinline__ float frontend_sample(const int16_t* pcm, int64_t nframes, int ch, int up, int down,
-                                                 const double* taps, int half, int64_t n) {
-  if (up == 1 && down == 1) return mono_at(pcm, n, ch);
+__device__ __forceinline__ float frontend_sample(const uint8_t* pcm, int fmt, int64_t nframes, int ch, int up,
+                                                 int down, const double* taps, int half, int64_t n) {
+  if (up == 1 && down == 1) return mono_at(pcm, fmt, n, ch);
   const int64_t centre = n * down + half;                 // tap index of input frame j is centre - j*up
   int64_t j_lo = (centre - 2 * (int64_t)half + up - 1) / up;            // ceil((centre - 2 half) / up)
   if (centre - 2 * (int64_t)half < 0) j_lo = 0;
   int64_t j_hi = centre / up;                                            // floor
   if (j_hi > nframes - 1) j_hi = nframes - 1;
   double acc = 0.0;
-  for (int64_t j = j_lo; j <= j_hi; ++j) acc += taps[centre - j * up] * (double)mono_at(pcm, j, ch);
+  for (int64_t j = j_lo; j <= j_hi; ++j) acc += taps[centre - j * up] * (double)mono_at(pcm, fmt, j, ch);
   return (float)acc;
 }
 
@@ -52,23 +55,23 @@ __global__ void __launch_bounds__(256) afp_pcm_frontend_kernel(const int16_t* pc
                                                                int64_t nout) {
   const int64_t n = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (n >= nout) return;
-  out[n] = frontend_sample(pcm, nframes, ch, up, down, taps, half, n);
+  out[n] = frontend_sample(reinterpret_cast<const uint8_t*>(pcm), AFP_PCM_I16, nframes, ch, up, down, taps, half, n);
 }
 
 // One file of a batched front-end call, built on the host.
 struct PcmFileDesc {
-  int64_t in_off;       // first int16 of the file in the packed PCM
+  int64_t in_off;       // first byte of the file in the packed PCM
   int64_t nframes;
   int64_t out_off;      // first output sample (a multiple of 4: 16-byte aligned)
   int64_t nout;         // ceil(nframes * up / down)
   int64_t tap_off;      // first tap of the file's (up, down) design in the packed taps
   int64_t block_base;   // first block of the file: the prefix sum of ceil(nout / 256)
-  int32_t ch, up, down, half;
+  int32_t ch, up, down, half, fmt;
 };
 
 // Block b belongs to the last file whose block_base <= b (a file without outputs has the same base as
 // the next one), found by one thread per block with a binary search over the block prefix.
-__global__ void __launch_bounds__(256) afp_pcm_frontend_batch_kernel(const int16_t* pcm, const PcmFileDesc* files,
+__global__ void __launch_bounds__(256) afp_pcm_frontend_batch_kernel(const uint8_t* pcm, const PcmFileDesc* files,
                                                                      int nfiles, const double* taps, float* out) {
   __shared__ int s_file;
   const int64_t b = blockIdx.x;
@@ -85,7 +88,8 @@ __global__ void __launch_bounds__(256) afp_pcm_frontend_batch_kernel(const int16
   const int64_t n = (b - f.block_base) * blockDim.x + threadIdx.x;
   const int64_t nout = f.nout;
   if (n >= nout) return;
-  out[f.out_off + n] = frontend_sample(pcm + f.in_off, f.nframes, f.ch, f.up, f.down, taps + f.tap_off, f.half, n);
+  out[f.out_off + n] =
+      frontend_sample(pcm + f.in_off, f.fmt, f.nframes, f.ch, f.up, f.down, taps + f.tap_off, f.half, n);
 }
 
 }  // namespace
@@ -121,14 +125,15 @@ extern "C" int afp_pcm_frontend(afp_ctx* c, const int16_t* pcm, int pcm_on_host,
   return AFP_OK;
 }
 
-extern "C" int afp_pcm_frontend_batch(afp_ctx* c, const int16_t* pcm, int pcm_on_host, int64_t pcm_len, int32_t nfiles,
-                                      const int64_t* pcm_offsets, const int64_t* nframes, const int32_t* channels,
-                                      const int32_t* up, const int32_t* down, int32_t npairs, const int32_t* pair_rates,
-                                      const int64_t* tap_offsets, const double* taps, float* out, int64_t out_capacity,
-                                      int64_t* out_offsets, int64_t* out_lengths) {
+extern "C" int afp_pcm_frontend_batch_bytes(afp_ctx* c, const uint8_t* pcm, int pcm_on_host, int64_t pcm_bytes,
+                                            int32_t nfiles, const int64_t* byte_offsets, const int32_t* formats,
+                                            const int64_t* nframes, const int32_t* channels, const int32_t* up,
+                                            const int32_t* down, int32_t npairs, const int32_t* pair_rates,
+                                            const int64_t* tap_offsets, const double* taps, float* out,
+                                            int64_t out_capacity, int64_t* out_offsets, int64_t* out_lengths) {
   if (!c) return AFP_ERR_INVALID;
-  if (nfiles < 0 || npairs < 0 || pcm_len < 0) AFP_FAIL(c, AFP_ERR_INVALID, "negative count");
-  if (nfiles > 0 && (!pcm_offsets || !nframes || !channels || !up || !down))
+  if (nfiles < 0 || npairs < 0 || pcm_bytes < 0) AFP_FAIL(c, AFP_ERR_INVALID, "negative count");
+  if (nfiles > 0 && (!byte_offsets || !formats || !nframes || !channels || !up || !down))
     AFP_FAIL(c, AFP_ERR_INVALID, "null per-file array");
   if (npairs > 0 && (!pair_rates || !tap_offsets || !taps)) AFP_FAIL(c, AFP_ERR_INVALID, "null taps table");
   // the taps table: one odd-length design per distinct (up, down), packed one after the other
@@ -140,18 +145,19 @@ extern "C" int afp_pcm_frontend_batch(afp_ctx* c, const int16_t* pcm, int pcm_on
   }
   std::vector<PcmFileDesc> d((size_t)nfiles);
   int64_t o = 0, blocks = 0;
+  int rc;
   for (int f = 0; f < nfiles; ++f) {
     PcmFileDesc& x = d[f];
     x.nframes = nframes[f];
     x.ch = channels[f];
     x.up = up[f];
     x.down = down[f];
-    x.in_off = pcm_offsets[f];
+    x.in_off = byte_offsets[f];
+    x.fmt = formats[f];
     if (x.nframes < 0) AFP_FAIL(c, AFP_ERR_INVALID, "file " + std::to_string(f) + ": negative length");
     if (x.ch < 1) AFP_FAIL(c, AFP_ERR_INVALID, "file " + std::to_string(f) + ": channels must be >= 1");
     if (x.up < 1 || x.down < 1) AFP_FAIL(c, AFP_ERR_INVALID, "file " + std::to_string(f) + ": up and down must be >= 1");
-    if (x.nframes > 0 && (x.in_off < 0 || x.in_off > pcm_len || x.nframes > (pcm_len - x.in_off) / x.ch))
-      AFP_FAIL(c, AFP_ERR_INVALID, "file " + std::to_string(f) + ": input range outside the PCM buffer");
+    if ((rc = pcm_check_input(c, f, pcm, pcm_on_host, pcm_bytes, x.in_off, x.fmt, x.nframes, x.ch))) return rc;
     if (x.nframes > (INT64_MAX - x.down) / x.up) AFP_FAIL(c, AFP_ERR_INVALID, "file " + std::to_string(f) + ": too long");
     x.tap_off = 0;
     x.half = 0;
@@ -181,9 +187,8 @@ extern "C" int afp_pcm_frontend_batch(afp_ctx* c, const int16_t* pcm, int pcm_on
     for (int f = 0; f < nfiles; ++f) out_lengths[f] = d[f].nout;
   if (!out || blocks == 0) return AFP_OK;                                 // sizing call, or nothing to compute
   AFP_CUDA(c, cudaSetDevice(c->device));
-  const int16_t* dpcm = nullptr;
-  int rc = afp_stage(c, c->d_pcm_stage, pcm, (size_t)pcm_len, pcm_on_host, &dpcm);
-  if (rc) return rc;
+  const uint8_t* dpcm = nullptr;
+  if ((rc = afp_stage(c, c->d_pcm_stage, pcm, (size_t)pcm_bytes, pcm_on_host, &dpcm))) return rc;
   if (pcm_on_host) c->batch_valid = false;   // the PCM staging buffer of the last fingerprint batch is overwritten
   // descriptors and every distinct design's taps in one upload
   const int64_t ntaps = npairs > 0 ? tap_offsets[npairs] : 0;
@@ -204,4 +209,20 @@ extern "C" int afp_pcm_frontend_batch(afp_ctx* c, const int16_t* pcm, int pcm_on
     return rc;
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));       // one synchronise for the whole list (`h` is pageable)
   return AFP_OK;
+}
+
+extern "C" int afp_pcm_frontend_batch(afp_ctx* c, const int16_t* pcm, int pcm_on_host, int64_t pcm_len, int32_t nfiles,
+                                      const int64_t* pcm_offsets, const int64_t* nframes, const int32_t* channels,
+                                      const int32_t* up, const int32_t* down, int32_t npairs, const int32_t* pair_rates,
+                                      const int64_t* tap_offsets, const double* taps, float* out, int64_t out_capacity,
+                                      int64_t* out_offsets, int64_t* out_lengths) {
+  if (!c) return AFP_ERR_INVALID;
+  if (nfiles < 0 || pcm_len < 0 || pcm_len > INT64_MAX / 2) AFP_FAIL(c, AFP_ERR_INVALID, "negative count");
+  if (nfiles > 0 && !pcm_offsets) AFP_FAIL(c, AFP_ERR_INVALID, "null per-file array");
+  std::vector<int64_t> boff;
+  std::vector<int32_t> fmt;
+  pcm_i16_layout(nfiles, pcm_offsets, &boff, &fmt);
+  return afp_pcm_frontend_batch_bytes(c, reinterpret_cast<const uint8_t*>(pcm), pcm_on_host, 2 * pcm_len, nfiles,
+                                      boff.data(), fmt.data(), nframes, channels, up, down, npairs, pair_rates,
+                                      tap_offsets, taps, out, out_capacity, out_offsets, out_lengths);
 }

@@ -11,6 +11,13 @@
 //                 Then lrintf(v * 32768), clipped to int16.  Edges: the input is mirrored around its
 //                 last sample for R samples and then around sample 0 (swr_edges).
 //
+// 24-bit, 32-bit and float input (afp_swr_frontend_batch_bytes) is read at the sample load
+// (afp_pcm_formats.cuh) as the library reads it: at equal rates a mono file's samples become int16 directly
+// (x >> 16, or the s16 rule of a float), and stereo is mixed in float32 as 0.5 l + 0.5 r of float(x) 2^-31
+// or the float itself; other rates take those floats instead of x / 32768.  Outputs of float input at
+// equal rates follow the library's buffers: its packed s16 rule, and its scalar rule for the file's last
+// n % 16 frames (tests/wide_pcm_reference.py).
+//
 // tests/swr_reference.py states the same in NumPy; tests/test_ffmpeg_frontend_cpu.py holds it to the
 // library's own output and tests/test_gpu_ffmpeg_frontend.py holds this kernel to both.  One thread
 // computes one output and reads its taps from global memory through the cache.  A design has P L
@@ -23,6 +30,7 @@
 #include <numeric>
 
 #include "afp_internal.cuh"
+#include "afp_pcm_formats.cuh"
 
 namespace {
 
@@ -108,18 +116,18 @@ const std::vector<float>& cached_design(int32_t in_rate, int32_t out_rate, const
 
 struct SwrFileDesc {
   int64_t in_off, nframes, out_off, nout, bank_off, block_base;
-  int32_t ch, P, D, L, resample;
+  int32_t ch, P, D, L, resample, fmt;
 };
 
 // sample c of extended input position e: mirrored around the end, then around 0 (the output count keeps
 // e within the reflected samples)
-__device__ __forceinline__ float swr_in(const int16_t* pcm, int64_t n, int ch, int c, int64_t e) {
+__device__ __forceinline__ float swr_in(const uint8_t* pcm, int fmt, int64_t n, int ch, int c, int64_t e) {
   if (e < 0) e = -e;
   if (e >= n) e = 2 * n - 1 - e;
-  return (float)pcm[e * ch + c] * (1.0f / 32768.0f);
+  return pcm_f32(pcm, fmt, e * ch + c);
 }
 
-__device__ __forceinline__ float swr_channel(const int16_t* pcm, const SwrFileDesc& f, const float* taps, int64_t start,
+__device__ __forceinline__ float swr_channel(const uint8_t* pcm, const SwrFileDesc& f, const float* taps, int64_t start,
                                              int c) {
   float lane[kLanes];
 #pragma unroll
@@ -127,7 +135,7 @@ __device__ __forceinline__ float swr_channel(const int16_t* pcm, const SwrFileDe
   for (int j = 0; j < f.L; j += kLanes) {
 #pragma unroll
     for (int k = 0; k < kLanes; ++k)
-      if (j + k < f.L) lane[k] = __fmaf_rn(swr_in(pcm, f.nframes, f.ch, c, start + j + k), __ldg(taps + j + k), lane[k]);
+      if (j + k < f.L) lane[k] = __fmaf_rn(swr_in(pcm, f.fmt, f.nframes, f.ch, c, start + j + k), __ldg(taps + j + k), lane[k]);
   }
   float a[4];
 #pragma unroll
@@ -135,10 +143,20 @@ __device__ __forceinline__ float swr_channel(const int16_t* pcm, const SwrFileDe
   return __fadd_rn(__fadd_rn(a[0], a[2]), __fadd_rn(a[1], a[3]));
 }
 
-__device__ __forceinline__ float swr_sample(const int16_t* pcm, const SwrFileDesc& f, const float* bank, int64_t n) {
+__device__ __forceinline__ float swr_sample(const uint8_t* pcm, const SwrFileDesc& f, const float* bank, int64_t n) {
   if (!f.resample) {
-    if (f.ch == 1) return (float)pcm[n] * (1.0f / 32768.0f);
-    const int v = (16384 * ((int)pcm[2 * n] + (int)pcm[2 * n + 1]) + 16384) >> 15;
+    int v;
+    if (f.fmt == AFP_PCM_I16 && f.ch == 2) {
+      const int16_t* p = reinterpret_cast<const int16_t*>(pcm);
+      v = (16384 * ((int)p[2 * n] + (int)p[2 * n + 1]) + 16384) >> 15;
+    } else if (f.fmt != AFP_PCM_F32 && f.ch == 1) {
+      v = pcm_s16(pcm, f.fmt, n);
+    } else {
+      float m = pcm_f32(pcm, f.fmt, f.ch * n);
+      if (f.ch == 2) m = __fadd_rn(__fmul_rn(m, 0.5f), __fmul_rn(pcm_f32(pcm, f.fmt, 2 * n + 1), 0.5f));
+      // the library's buffers of float input are 4096-byte packets, a multiple of 16 frames
+      v = n >= f.nframes - (f.nframes & 15) ? pcm_s16_scalar_rule(m) : pcm_s16_rule(m);
+    }
     return (float)v * (1.0f / 32768.0f);
   }
   const int64_t k = n * f.D;
@@ -146,11 +164,10 @@ __device__ __forceinline__ float swr_sample(const int16_t* pcm, const SwrFileDes
   const float* taps = bank + (k % f.P) * f.L;
   float v = swr_channel(pcm, f, taps, start, 0);
   if (f.ch == 2) v = __fadd_rn(__fmul_rn(v, 0.5f), __fmul_rn(swr_channel(pcm, f, taps, start, 1), 0.5f));
-  const int s = min(max(__float2int_rn(__fmul_rn(v, 32768.0f)), -32768), 32767);
-  return (float)s * (1.0f / 32768.0f);
+  return (float)pcm_s16_rule(v) * (1.0f / 32768.0f);
 }
 
-__global__ void __launch_bounds__(256) afp_swr_frontend_kernel(const int16_t* pcm, const SwrFileDesc* files, int nfiles,
+__global__ void __launch_bounds__(256) afp_swr_frontend_kernel(const uint8_t* pcm, const SwrFileDesc* files, int nfiles,
                                                               const float* banks, float* out) {
   __shared__ int s_file;
   const int64_t b = blockIdx.x;
@@ -197,29 +214,32 @@ extern "C" int afp_swr_length(int64_t nframes, int32_t in_rate, int32_t out_rate
   return AFP_OK;
 }
 
-extern "C" int afp_swr_frontend_batch(afp_ctx* c, const int16_t* pcm, int pcm_on_host, int64_t pcm_len, int32_t nfiles,
-                                      const int64_t* pcm_offsets, const int64_t* nframes, const int32_t* channels,
-                                      const int32_t* rates, int32_t out_rate, float* out, int64_t out_capacity,
-                                      int64_t* out_offsets, int64_t* out_lengths) {
+extern "C" int afp_swr_frontend_batch_bytes(afp_ctx* c, const uint8_t* pcm, int pcm_on_host, int64_t pcm_bytes,
+                                            int32_t nfiles, const int64_t* byte_offsets, const int32_t* formats,
+                                            const int64_t* nframes, const int32_t* channels, const int32_t* rates,
+                                            int32_t out_rate, float* out, int64_t out_capacity, int64_t* out_offsets,
+                                            int64_t* out_lengths) {
   if (!c) return AFP_ERR_INVALID;
-  if (nfiles < 0 || pcm_len < 0) AFP_FAIL(c, AFP_ERR_INVALID, "negative count");
+  if (nfiles < 0 || pcm_bytes < 0) AFP_FAIL(c, AFP_ERR_INVALID, "negative count");
   if (out_rate < 1) AFP_FAIL(c, AFP_ERR_INVALID, "output rate must be >= 1");
-  if (nfiles > 0 && (!pcm_offsets || !nframes || !channels || !rates)) AFP_FAIL(c, AFP_ERR_INVALID, "null per-file array");
+  if (nfiles > 0 && (!byte_offsets || !formats || !nframes || !channels || !rates))
+    AFP_FAIL(c, AFP_ERR_INVALID, "null per-file array");
   std::vector<SwrFileDesc> d((size_t)nfiles);
   std::vector<std::pair<int32_t, const std::vector<float>*>> uniq;   // distinct input rates, first use first
   int64_t o = 0, blocks = 0, nbank = 0;
+  int rc;
   for (int f = 0; f < nfiles; ++f) {
     SwrFileDesc& x = d[f];
     const std::string tag = "file " + std::to_string(f) + ": ";
     x.nframes = nframes[f];
     x.ch = channels[f];
-    x.in_off = pcm_offsets[f];
+    x.in_off = byte_offsets[f];
+    x.fmt = formats[f];
     if (x.nframes < 0) AFP_FAIL(c, AFP_ERR_INVALID, tag + "negative length");
     if (x.ch < 1) AFP_FAIL(c, AFP_ERR_INVALID, tag + "channels must be >= 1");
     if (rates[f] < 1) AFP_FAIL(c, AFP_ERR_INVALID, tag + "sample rate must be >= 1");
     if (x.ch > 2) AFP_FAIL(c, AFP_ERR_UNSUPPORTED, tag + "the ffmpeg front-end takes mono or stereo");
-    if (x.nframes > 0 && (x.in_off < 0 || x.in_off > pcm_len || x.nframes > (pcm_len - x.in_off) / x.ch))
-      AFP_FAIL(c, AFP_ERR_INVALID, tag + "input range outside the PCM buffer");
+    if ((rc = pcm_check_input(c, f, pcm, pcm_on_host, pcm_bytes, x.in_off, x.fmt, x.nframes, x.ch))) return rc;
     x.resample = rates[f] != out_rate;
     x.P = x.D = x.L = 1;
     x.bank_off = 0;
@@ -260,9 +280,8 @@ extern "C" int afp_swr_frontend_batch(afp_ctx* c, const int16_t* pcm, int pcm_on
     for (int f = 0; f < nfiles; ++f) out_lengths[f] = d[f].nout;
   if (!out || blocks == 0) return AFP_OK;                                 // sizing call, or nothing to compute
   AFP_CUDA(c, cudaSetDevice(c->device));
-  const int16_t* dpcm = nullptr;
-  int rc = afp_stage(c, c->d_pcm_stage, pcm, (size_t)pcm_len, pcm_on_host, &dpcm);
-  if (rc) return rc;
+  const uint8_t* dpcm = nullptr;
+  if ((rc = afp_stage(c, c->d_pcm_stage, pcm, (size_t)pcm_bytes, pcm_on_host, &dpcm))) return rc;
   if (pcm_on_host) c->batch_valid = false;   // the PCM staging buffer of the last fingerprint batch is overwritten
   // descriptors and every distinct rate's design in one upload
   SwrFileDesc* dd = nullptr;
@@ -285,4 +304,19 @@ extern "C" int afp_swr_frontend_batch(afp_ctx* c, const int16_t* pcm, int pcm_on
   if ((rc = afp_launch(c, afp_swr_frontend_kernel, (unsigned)blocks, 256, 0, dpcm, dd, nfiles, dbank, out))) return rc;
   AFP_CUDA(c, cudaStreamSynchronize(c->stream));       // one synchronise for the whole list (`h` is pageable)
   return AFP_OK;
+}
+
+extern "C" int afp_swr_frontend_batch(afp_ctx* c, const int16_t* pcm, int pcm_on_host, int64_t pcm_len, int32_t nfiles,
+                                      const int64_t* pcm_offsets, const int64_t* nframes, const int32_t* channels,
+                                      const int32_t* rates, int32_t out_rate, float* out, int64_t out_capacity,
+                                      int64_t* out_offsets, int64_t* out_lengths) {
+  if (!c) return AFP_ERR_INVALID;
+  if (nfiles < 0 || pcm_len < 0 || pcm_len > INT64_MAX / 2) AFP_FAIL(c, AFP_ERR_INVALID, "negative count");
+  if (nfiles > 0 && !pcm_offsets) AFP_FAIL(c, AFP_ERR_INVALID, "null per-file array");
+  std::vector<int64_t> boff;
+  std::vector<int32_t> fmt;
+  pcm_i16_layout(nfiles, pcm_offsets, &boff, &fmt);
+  return afp_swr_frontend_batch_bytes(c, reinterpret_cast<const uint8_t*>(pcm), pcm_on_host, 2 * pcm_len, nfiles,
+                                      boff.data(), fmt.data(), nframes, channels, rates, out_rate, out, out_capacity,
+                                      out_offsets, out_lengths);
 }

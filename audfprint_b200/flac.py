@@ -3,7 +3,7 @@ the device decoder (afp_flac_locate_batch / afp_flac_decode_batch, include/afp.h
 
 The host only finds where the frames start and what STREAMINFO says; locating, checking and decoding
 the frames run on the device.  Native FLAC only: Ogg-FLAC (an Ogg container) is not recognised and
-reads as an unreadable file, like any other format but 16-bit PCM WAV.  The STREAMINFO MD5 signature is
+reads as an unreadable file, like any other format but PCM and float WAV.  The STREAMINFO MD5 signature is
 not checked, as ffmpeg does not check it by default."""
 from __future__ import annotations
 
@@ -124,6 +124,20 @@ def decode_into(ctx, out, out_offsets):
     status = np.zeros(max(n, 1), np.int32)
     rc = ctx.lib.afp_flac_decode_batch(ctx.h, out.data_ptr(), out.numel(), off.ctypes.data_as(C.POINTER(C.c_int64)),
                                        status.ctypes.data)
+    _check_files(ctx, rc, status)
+    return status[:n]
+
+
+def decode_into_bytes(ctx, out, out_offsets, full_depth):
+    """afp_flac_decode_batch_bytes of the last located batch into the device uint8 tensor `out`: file i
+    at byte out_offsets[i], int16, or with full_depth a file of 17-24 bits as int32 x << (32 - bits).
+    -> status int32 [n]."""
+    off = np.ascontiguousarray(out_offsets, dtype=np.int64)
+    n = len(off)
+    status = np.zeros(max(n, 1), np.int32)
+    rc = ctx.lib.afp_flac_decode_batch_bytes(ctx.h, out.data_ptr(), out.numel(),
+                                             off.ctypes.data_as(C.POINTER(C.c_int64)), int(bool(full_depth)),
+                                             status.ctypes.data)
     _check_files(ctx, rc, status)
     return status[:n]
 

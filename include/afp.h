@@ -52,7 +52,12 @@ typedef enum {
   AFP_ERR_INDEX = -6        /* a computed index leaves its array (maps to IndexError) */
 } afp_status;
 
-enum { AFP_PCM_I16 = 0, AFP_PCM_F32 = 1 };
+/* Sample formats.  afp_fingerprint_batch takes AFP_PCM_I16 and AFP_PCM_F32 (float in [-1, 1)); the
+ * byte forms of the front-ends (afp_pcm_frontend_batch_bytes, afp_swr_frontend_batch_bytes) take all
+ * four, packed little-endian as a WAV data chunk holds them: int16, IEEE float32, 24-bit integers in 3
+ * bytes, 32-bit integers.  A 17-24-bit FLAC file decoded at full depth is AFP_PCM_S32 holding
+ * x << (32 - bits). */
+enum { AFP_PCM_I16 = 0, AFP_PCM_F32 = 1, AFP_PCM_S24 = 2, AFP_PCM_S32 = 3 };
 
 /* compiled limits */
 #define AFP_N_FFT 512
@@ -162,6 +167,22 @@ int afp_pcm_frontend_batch(afp_ctx* ctx, const int16_t* pcm, int pcm_on_host, in
                            const int32_t* up, const int32_t* down, int32_t npairs, const int32_t* pair_rates,
                            const int64_t* tap_offsets, const double* taps, float* out, int64_t out_capacity,
                            int64_t* out_offsets, int64_t* out_lengths);
+/* afp_pcm_frontend_batch over packed payload bytes with a sample format per file:
+ *   pcm            pcm_bytes bytes, HOST or DEVICE: each file's samples as its WAV data chunk holds them
+ *   byte_offsets   HOST int64 [nfiles]: file i starts at byte byte_offsets[i], a multiple of its sample's
+ *                  width for AFP_PCM_I16 (2), AFP_PCM_S32 and AFP_PCM_F32 (4) when counted from an
+ *                  aligned address; AFP_PCM_S24 takes any offset
+ *   formats        HOST int32 [nfiles]: AFP_PCM_* of each file
+ * Each sample enters the down-mix as the int16 `ffmpeg -ac 1` gives a mono file of its format at its own
+ * rate: x >> 16 of a 24-bit (x << 8) or 32-bit integer, and for a float v the packed s16 rule of the
+ * ffmpeg front-end below.  An all-AFP_PCM_I16 call is afp_pcm_frontend_batch, bit for bit, through the
+ * same kernel; files of every format share one launch.  AFP_ERR_INVALID for an unknown format or a
+ * misaligned file, otherwise as afp_pcm_frontend_batch. */
+int afp_pcm_frontend_batch_bytes(afp_ctx* ctx, const uint8_t* pcm, int pcm_on_host, int64_t pcm_bytes, int32_t nfiles,
+                                 const int64_t* byte_offsets, const int32_t* formats, const int64_t* nframes,
+                                 const int32_t* channels, const int32_t* up, const int32_t* down, int32_t npairs,
+                                 const int32_t* pair_rates, const int64_t* tap_offsets, const double* taps, float* out,
+                                 int64_t out_capacity, int64_t* out_offsets, int64_t* out_lengths);
 
 /* ---- ffmpeg front-end (audfprint_b200/csrc/afp_swr.cu) ----
  * What `ffmpeg -i F -f s16le -ac 1 -ar <out_rate> -` (the reference's reader, audio_read.py:196-203)
@@ -190,6 +211,28 @@ int afp_swr_frontend_batch(afp_ctx* ctx, const int16_t* pcm, int pcm_on_host, in
                            const int64_t* pcm_offsets, const int64_t* nframes, const int32_t* channels,
                            const int32_t* rates, int32_t out_rate, float* out, int64_t out_capacity,
                            int64_t* out_offsets, int64_t* out_lengths);
+/* afp_swr_frontend_batch over packed payload bytes with a sample format per file (the layout of
+ * afp_pcm_frontend_batch_bytes).  What FFmpeg 8.0 does with 24-bit, 32-bit and float PCM, and with
+ * 17-24-bit FLAC decoded at full depth (AFP_PCM_S32, afp_flac_decode_batch_bytes): its decoders give an
+ * integer as the int32 x << (32 - bits) and a float as it is, and libswresample then makes int16
+ *   mono, equal rates    x >> 16 of an integer; the s16 rule of a float;
+ *   stereo, equal rates  in float32: each channel as float(x) 2^-31 (or the float), 0.5 l + 0.5 r, the
+ *                        s16 rule;
+ *   other rates          the float32 resampler above, fed those floats instead of x / 32768.
+ * s16 rule: v * 32768 in float32, rounded half to even to int32, NaN, +-Inf and values outside the int32
+ * range giving INT32_MIN, then saturated to int16: so NaN, +Inf and large positive values give -32768
+ * (x86 cvtps2dq + packssdw).  The library converts the last n % 16 samples of each buffer with its scalar
+ * rule instead, av_clip_int16((int) lrintf(v * 32768)), which differs only for NaN, +-Inf and |v| >= 65536:
+ * for float input at equal rates the buffers are 4096-byte packets and the kernel takes the scalar rule
+ * for the file's last nframes % 16 outputs; at other rates the packed rule is taken for every output.
+ * An all-AFP_PCM_I16 call is afp_swr_frontend_batch, bit for bit, through the same kernel.  8-bit, 64-bit
+ * float, A-law, mu-law and other codings have no format code: the library's int16 and double engines they
+ * would go through are not stated.  AFP_ERR_INVALID for an unknown format or a misaligned file,
+ * otherwise as afp_swr_frontend_batch. */
+int afp_swr_frontend_batch_bytes(afp_ctx* ctx, const uint8_t* pcm, int pcm_on_host, int64_t pcm_bytes, int32_t nfiles,
+                                 const int64_t* byte_offsets, const int32_t* formats, const int64_t* nframes,
+                                 const int32_t* channels, const int32_t* rates, int32_t out_rate, float* out,
+                                 int64_t out_capacity, int64_t* out_offsets, int64_t* out_lengths);
 
 /* ---- FLAC decoding -----------------------------------------------------------
  * What the reference's `ffmpeg -i F -f s16le` does for a FLAC file, up to the int16 stream the PCM
@@ -260,6 +303,13 @@ int afp_flac_locate_batch(afp_ctx* ctx, const uint8_t* bytes, int bytes_on_host,
  * batch; every range is checked against out_capacity before anything is launched.  Synchronises. */
 int afp_flac_decode_batch(afp_ctx* ctx, int16_t* out_dev, int64_t out_capacity, const int64_t* out_offsets,
                           int32_t* file_status);
+/* afp_flac_decode_batch into a byte buffer: out_dev holds out_capacity bytes and file i starts at byte
+ * out_offsets[i].  With full_depth = 0 every file is int16 as above.  With full_depth = 1 a file of 17-24
+ * bits is written at full depth, AFP_PCM_S32 holding x << (32 - b) (4 bytes a sample, 4-byte aligned),
+ * the int32 FFmpeg's decoder gives it; files of 16 bits or fewer are int16 (2-byte aligned) either way.
+ * AFP_ERR_INVALID for a misaligned file; otherwise as afp_flac_decode_batch. */
+int afp_flac_decode_batch_bytes(afp_ctx* ctx, uint8_t* out_dev, int64_t out_capacity, const int64_t* out_offsets,
+                                int32_t full_depth, int32_t* file_status);
 
 /* ---- Analyzer --------------------------------------------------------------
  * Replaces stft.stft (stft.py:62-94) + Analyzer.find_peaks
