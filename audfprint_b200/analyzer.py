@@ -87,47 +87,17 @@ def _as_payload(raw, sample_format):
 
 def pcm_frontend(raw, channels, src_rate, dst_rate=None, device=None, to_host=True, resampler='poly',
                  sample_format=None):
-    """Interleaved int16 PCM -> mono float32 at dst_rate, on the device (afp_pcm_frontend:
-    channel mean, 1/32768 scaling, polyphase resampling).  Returns a NumPy array, or with
+    """Interleaved int16 PCM -> mono float32 at dst_rate, on the device: pcm_frontend_batch of one file
+    (channel mean, 1/32768 scaling, polyphase resampling).  Returns a NumPy array, or with
     to_host=False a torch CUDA tensor that Analyzer.fingerprint_packed takes as it is.
     resampler='ffmpeg' gives instead the bits `ffmpeg -ac 1 -ar dst_rate` gives, v / 32768
-    (afp_swr_frontend_batch; mono or stereo, and rates with out / gcd <= 1024).
+    (mono or stereo, and rates with out / gcd <= 1024).
     sample_format 's24', 's32' or 'f32' (or 's16') takes `raw` as a WAV data chunk's bytes of that
-    format (_as_payload) and runs the byte form of the same front-end (pcm_frontend_batch)."""
-    from math import gcd
-    if sample_format is not None:
-        out, off, lens = pcm_frontend_batch([raw], [channels], [src_rate], dst_rate if dst_rate is not None else src_rate,
-                                            device=device, resampler=resampler, sample_formats=[sample_format])
-        out = out[:int(lens[0])].clone()
-        return out.cpu().numpy() if to_host else out
-    raw = np.ascontiguousarray(raw, dtype=np.int16).reshape(-1)
-    if _check_resampler(resampler) == 'ffmpeg':
-        out, off, lens = pcm_frontend_batch([raw], [channels], [src_rate], dst_rate if dst_rate is not None else src_rate,
-                                            device=device, resampler='ffmpeg')
-        out = out[:int(lens[0])].clone()
-        return out.cpu().numpy() if to_host else out
-    nframes = len(raw) // max(1, int(channels))
-    up, down = 1, 1
-    if dst_rate is not None and int(dst_rate) != int(src_rate):
-        g = gcd(int(dst_rate), int(src_rate))
-        up, down = int(dst_rate) // g, int(src_rate) // g
-    taps = resample_taps(up, down) if (up, down) != (1, 1) else None
-    ctx = _lib.context(device)
-    nout = -(-nframes * up // down)
-    n = C.c_int64(0)
-    if to_host:
-        out = np.empty(nout, np.float32)
-        optr, on_host = out.ctypes.data, 1
-    else:
-        import torch
-        out = torch.empty(nout, dtype=torch.float32, device=torch.device("cuda", ctx.device))
-        optr, on_host = out.data_ptr(), 0
-    with ctx.after_torch(out):            # torch's pending reads of out's memory come first
-        ctx.check(ctx.lib.afp_pcm_frontend(ctx.h, raw.ctypes.data if nframes else None, 1, nframes, int(channels), up,
-                                           down, taps.ctypes.data if taps is not None else None,
-                                           len(taps) if taps is not None else 0, optr if nout else None, on_host,
-                                           C.byref(n)))
-    return out
+    format (_as_payload)."""
+    out, _, lens = pcm_frontend_batch([raw], [channels], [src_rate], src_rate if dst_rate is None else dst_rate,
+                                      device=device, resampler=resampler, sample_formats=[sample_format])
+    out = out[:int(lens[0])]
+    return out.cpu().numpy() if to_host else out
 
 
 _GUID_TAIL = b"\x00\x00\x10\x00\x80\x00\x00\xaa\x00\x38\x9b\x71"      # KSDATAFORMAT_SUBTYPE_* after Data1
@@ -283,28 +253,22 @@ def _wav_reader(filename, sr=None, channels=None, device=None, resampler='poly')
     """PCM-WAV and FLAC reader standing in for audio_read.audio_read (audio_read.py:56-68; ffmpeg
     decoding of other formats is out of scope, SURVEY §2 #9).  Returns (float32 samples in [-1,1), sr)
     like the reference reader does (audio_read.py:139-145).  A WAV is parsed on the host; a FLAC file's
-    frames are decoded on the device (flac.decode) to the int16 samples ffmpeg's decoder gives.  The
-    arithmetic the reference hands to ffmpeg - down-mix to mono, resampling to `sr` - runs on the
-    device (afp_pcm_frontend, SURVEY.md 8f-2).  No two resamplers agree bit for bit, so parity
-    statements in this repo are made on 11025 Hz PCM.  With resampler='ffmpeg' the down-mix and
-    resampling are ffmpeg's own, bit for bit (afp_swr_frontend_batch)."""
+    frames are decoded on the device to the samples ffmpeg's decoder gives.  The arithmetic the
+    reference hands to ffmpeg - down-mix to mono, resampling to `sr` - runs on the device
+    (_frontend_sources, SURVEY.md 8f-2).  No two resamplers agree bit for bit, so parity statements in
+    this repo are made on 11025 Hz PCM.  With resampler='ffmpeg' the down-mix and resampling are
+    ffmpeg's own, bit for bit (afp_swr_frontend_batch_bytes)."""
     raw, nch, fs = _audio_read_raw(filename)
+    sr = fs if sr is None else sr
     if _check_resampler(resampler) == 'ffmpeg':
-        _swr_check(filename, raw, nch, fs, fs if sr is None else sr)
-    if (isinstance(raw, np.ndarray) and raw.dtype != np.int16) or \
-            (isinstance(raw, flac.FlacStream) and resampler == 'ffmpeg' and raw.bits_per_sample > 16):
-        # 24-bit, 32-bit and float WAV, and deep FLAC at full depth: the byte form of the front-end
-        out, off, lens, status = _frontend_sources([raw], [nch], [fs], fs if sr is None else sr, device, resampler)
-        if status[0]:
-            raise flac.failure(status[0])
-        return out[:int(lens[0])].cpu().numpy(), (fs if sr is None else sr)
-    if isinstance(raw, flac.FlacStream):
-        raw = flac.decode(raw, device)
-    if nch == 1 and (sr is None or fs == sr):
-        # nothing to do but the reader's own scaling (exact in float32)
+        _swr_check(filename, raw, nch, fs, sr)
+    if isinstance(raw, np.ndarray) and raw.dtype == np.int16 and nch == 1 and fs == sr:
+        # nothing to do but the reader's own scaling (exact in float32, the bits the device gives)
         return raw.astype(np.float32) * np.float32(1.0 / 32768.0), fs
-    data = pcm_frontend(raw, nch, fs, sr, device=device, resampler=resampler)
-    return data, (fs if sr is None else sr)
+    out, _, lens, status = _frontend_sources([raw], [nch], [fs], sr, device, resampler)
+    if status[0]:
+        raise flac.failure(status[0])
+    return out[:int(lens[0])].cpu().numpy(), sr
 
 
 _TAPS = {}
@@ -333,32 +297,32 @@ def taps_table(pairs):
 
 def pcm_frontend_batch(raws, channels, src_rates, dst_rate, device=None, resampler='poly', sample_formats=None):
     """Many files' interleaved int16 PCM -> mono float32 at dst_rate in ONE device buffer
-    (afp_pcm_frontend_batch: one upload of the packed PCM, one launch, one synchronise).
-    Every file's samples are bit-identical to pcm_frontend on that file alone.
+    (_frontend_packed: one upload of the packed payloads, one launch, one synchronise).
     Returns (out torch CUDA float32, offsets int64 [n+1], lengths int64 [n]): file i is
     out[offsets[i]:offsets[i] + lengths[i]], starting on a 16-byte boundary - the layout
     Analyzer.fingerprint_packed(out, offsets, sample_lengths=lengths) takes as it is.
-    resampler='ffmpeg': afp_swr_frontend_batch, ffmpeg's down-mix and resampler (pcm_frontend).
-    sample_formats: None (every file int16, as always), or one pcm_frontend sample_format per file; the
-    files then go up as their payload bytes and one byte-form call (afp_*_frontend_batch_bytes) runs
-    over every format of the list."""
+    resampler='ffmpeg': ffmpeg's down-mix and resampler (pcm_frontend).
+    sample_formats: None (every file int16, values converted as pcm_frontend converts them), or one
+    pcm_frontend sample_format per file; files of every format share the one call."""
     if sample_formats is None:
-        raws = [np.ascontiguousarray(r, dtype=np.int16).reshape(-1) for r in raws]
-        inoff = np.zeros(len(raws) + 1, np.int64)
-        inoff[1:] = np.cumsum([len(r) for r in raws])
-        nfr = [len(r) // max(1, int(c)) for r, c in zip(raws, channels)]
-        packed = np.concatenate(raws) if raws else np.zeros(0, np.int16)
-        return _frontend_packed(_lib.context(device), packed, inoff, nfr, channels, src_rates, dst_rate, resampler)
-    pays = [_as_payload(r, f) for r, f in zip(raws, sample_formats)]
-    packed, boff = _pack_payloads([b for b, _ in pays])
-    fmts = [k for _, k in pays]
-    nfr = [len(b) // _WIDTH[k] // max(1, int(c)) for (b, k), c in zip(pays, channels)]
+        sample_formats = [None] * len(raws)
+    pays, fmts, nfr = _payloads(raws, sample_formats, channels)
+    packed, boff = _pack_payloads(pays)
     return _frontend_packed(_lib.context(device), packed, boff, nfr, channels, src_rates, dst_rate, resampler, fmts)
+
+
+def _payloads(raws, sample_formats, channels):
+    """Files' samples -> (payload bytes, AFP_PCM_* codes, frames) per file (_as_payload)."""
+    pays = [_as_payload(r, f) for r, f in zip(raws, sample_formats)]
+    nfr = [len(b) // _WIDTH[k] // max(1, int(c)) for (b, k), c in zip(pays, channels)]
+    return [b for b, _ in pays], [k for _, k in pays], nfr
 
 
 def _pack_payloads(payloads, extra=()):
     """Payload bytes of many files -> (one uint8 buffer, byte offset int64 [n]), every file on a 4-byte
     boundary; `extra` byte counts get aligned places after them (filled by the caller)."""
+    if len(payloads) == 1 and not extra:          # nothing to align: the bytes go up as they are, uncopied
+        return payloads[0], np.array([0, len(payloads[0])], np.int64)
     sizes = [len(b) for b in payloads] + list(extra)
     boff = np.zeros(len(sizes) + 1, np.int64)
     boff[1:] = np.cumsum([(n + 3) // 4 * 4 for n in sizes])
@@ -369,43 +333,39 @@ def _pack_payloads(payloads, extra=()):
 
 
 def _frontend_packed(ctx, pcm, inoff, nfr, channels, src_rates, dst_rate, resampler='poly', formats=None):
-    """afp_pcm_frontend_batch over files packed in `pcm`, a host int16 array or a device int16 tensor:
-    file i's nfr[i] frames of channels[i] channels start at pcm[inoff[i]].  With `formats` (AFP_PCM_* per
-    file) `pcm` is a host uint8 array or device uint8 tensor, `inoff` byte offsets, and the byte form
-    runs (afp_*_frontend_batch_bytes).  -> (out, offsets, lengths) as pcm_frontend_batch returns them."""
+    """The byte-form front-end (afp_pcm_frontend_batch_bytes, or afp_swr_frontend_batch_bytes for
+    'ffmpeg') over files packed in `pcm`, a host uint8 array or device uint8 tensor: file i's nfr[i]
+    frames of channels[i] channels, AFP_PCM_* formats[i], start at byte inoff[i].  formats None: `pcm`
+    is a host int16 array or device int16 tensor, `inoff` counts int16 values, and every file is
+    AFP_PCM_I16.  -> (out, offsets, lengths) as pcm_frontend_batch returns them."""
     import torch
     from math import gcd
     n = len(nfr)
+    inoff = np.ascontiguousarray(inoff, dtype=np.int64)
+    if formats is None:
+        pcm = pcm.view(np.uint8) if isinstance(pcm, np.ndarray) else pcm.view(torch.uint8)
+        inoff, formats = 2 * inoff, np.full(n, _lib.PCM_I16, np.int32)
+    fmt = np.ascontiguousarray(formats, dtype=np.int32)
     ch = np.array([int(c) for c in channels], np.int32)
     nfr = np.ascontiguousarray(nfr, dtype=np.int64)
-    inoff = np.ascontiguousarray(inoff, dtype=np.int64)
     P = C.POINTER(C.c_int64)
     ptr, on_host = _lib.ptr_of(pcm)
     plen = len(pcm) if isinstance(pcm, np.ndarray) else pcm.numel()
-    off = np.zeros(n + 1, np.int64)
-    lens = np.zeros(n, np.int64)
-    fmt = None if formats is None else np.ascontiguousarray(formats, dtype=np.int32)
-    form = [] if fmt is None else [fmt.ctypes.data]
     if _check_resampler(resampler) == 'ffmpeg':
         rates = np.array([int(fs) for fs in src_rates], np.int32)
-        fn = ctx.lib.afp_swr_frontend_batch if fmt is None else ctx.lib.afp_swr_frontend_batch_bytes
-        args = [ctx.h, ptr if plen else None, on_host, plen, n, inoff.ctypes.data_as(P)] + form + \
-               [nfr.ctypes.data_as(P), ch.ctypes.data, rates.ctypes.data, int(dst_rate)]
-        ctx.check(fn(*args, None, 0, off.ctypes.data_as(P), lens.ctypes.data_as(P)))
-        out = torch.zeros(int(off[-1]) + 4, dtype=torch.float32, device=torch.device("cuda", ctx.device))
-        with ctx.after_torch(out, pcm):
-            ctx.check(fn(*args, out.data_ptr(), out.numel(), None, None))
-        return out, off, lens
-    up, down = np.ones(n, np.int32), np.ones(n, np.int32)
-    for i, fs in enumerate(src_rates):
-        if dst_rate is not None and int(dst_rate) != int(fs):
-            g = gcd(int(dst_rate), int(fs))
-            up[i], down[i] = int(dst_rate) // g, int(fs) // g
-    rates, toff, taps = taps_table(zip(up, down))
-    fn = ctx.lib.afp_pcm_frontend_batch if fmt is None else ctx.lib.afp_pcm_frontend_batch_bytes
-    args = [ctx.h, ptr if plen else None, on_host, plen, n, inoff.ctypes.data_as(P)] + form + \
-           [nfr.ctypes.data_as(P), ch.ctypes.data, up.ctypes.data, down.ctypes.data, len(rates), rates.ctypes.data,
-            toff.ctypes.data_as(P), taps.ctypes.data]
+        fn, own = ctx.lib.afp_swr_frontend_batch_bytes, [rates.ctypes.data, int(dst_rate)]
+    else:
+        up, down = np.ones(n, np.int32), np.ones(n, np.int32)
+        for i, fs in enumerate(src_rates):
+            if dst_rate is not None and int(dst_rate) != int(fs):
+                g = gcd(int(dst_rate), int(fs))
+                up[i], down[i] = int(dst_rate) // g, int(fs) // g
+        rates, toff, taps = taps_table(zip(up, down))
+        fn, own = ctx.lib.afp_pcm_frontend_batch_bytes, [up.ctypes.data, down.ctypes.data, len(rates),
+                                                         rates.ctypes.data, toff.ctypes.data_as(P), taps.ctypes.data]
+    args = [ctx.h, ptr if plen else None, on_host, plen, n, inoff.ctypes.data_as(P), fmt.ctypes.data,
+            nfr.ctypes.data_as(P), ch.ctypes.data] + own
+    off, lens = np.zeros(n + 1, np.int64), np.zeros(n, np.int64)
     ctx.check(fn(*args, None, 0, off.ctypes.data_as(P), lens.ctypes.data_as(P)))
     # 16 bytes of zeros past the last file, as Analyzer._pack leaves
     out = torch.zeros(int(off[-1]) + 4, dtype=torch.float32, device=torch.device("cuda", ctx.device))
@@ -414,88 +374,46 @@ def _frontend_packed(ctx, pcm, inoff, nfr, channels, src_rates, dst_rate, resamp
     return out, off, lens
 
 
+def _flac_format(stream, resampler):
+    """The AFP_PCM_* format a FLAC file is decoded to for `resampler`: int16, or for 17-24 bits in
+    'ffmpeg' mode the full-depth int32 ffmpeg's decoder gives (flac.decode_into_bytes)."""
+    return _lib.PCM_S32 if resampler == 'ffmpeg' and stream.bits_per_sample > 16 else _lib.PCM_I16
+
+
 def _frontend_sources(sources, channels, src_rates, dst_rate, device=None, resampler='poly'):
-    """pcm_frontend_batch over files given as int16 PCM or as flac.FlacStream.  With FLAC files among
-    them, the round's int16 buffer is built on the device: the PCM files go up in one copy, the FLAC
-    files are located (one call) and decoded in place after them (one call), and one front-end call
-    runs over all.  -> (out, offsets, lengths, status int32 [n]): 0, or the AFP_FLAC_* code of a FLAC
-    file the device refused, which then has no samples."""
-    import torch
+    """The front-end over files given as WAV samples (what _wav_read_raw returns, or int16 PCM) or as
+    flac.FlacStream.  Without FLAC files: pcm_frontend_batch of the WAV payloads, each in its own
+    format (_raw_format).  With them, the round's buffer is built on the device: the WAV payloads go up
+    in one copy, the FLAC files are located (one call) and decoded into their places after them (one
+    call; _flac_format), and one front-end call runs over all (_frontend_packed).
+    -> (out, offsets, lengths, status int32 [n]): 0, or the AFP_FLAC_* code of a FLAC file the device
+    refused, which then has no samples."""
     n = len(sources)
     status = np.zeros(n, np.int32)
     fl = [k for k, s in enumerate(sources) if isinstance(s, flac.FlacStream)]
-    full_depth = resampler == 'ffmpeg'
-    if any(s.dtype != np.int16 for s in sources if isinstance(s, np.ndarray)) or \
-            (full_depth and any(sources[k].bits_per_sample > 16 for k in fl)):
-        return _frontend_sources_bytes(sources, fl, channels, src_rates, dst_rate, device, resampler)
     if not fl:
-        return pcm_frontend_batch(sources, channels, src_rates, dst_rate, device=device, resampler=resampler) + (status,)
-    ctx = _lib.context(device)
-    nsamples, _ = flac.locate(ctx, [sources[k] for k in fl])
-    is_flac = set(fl)
-    raws = [np.ascontiguousarray(sources[k], dtype=np.int16).reshape(-1) for k in range(n) if k not in is_flac]
-    inoff, nfr = np.zeros(n, np.int64), np.zeros(n, np.int64)
-    pos, r = 0, iter(raws)
-    for k in range(n):
-        if k not in is_flac:
-            raw = next(r)
-            inoff[k], nfr[k] = pos, len(raw) // max(1, int(channels[k]))
-            pos += len(raw)
-    wav_len, fl_off = pos, []
-    for j, k in enumerate(fl):
-        inoff[k], nfr[k] = pos, nsamples[j]
-        fl_off.append(pos)
-        pos += int(nsamples[j]) * int(channels[k])
-    pcm = torch.empty(max(pos, 1), dtype=torch.int16, device=torch.device("cuda", ctx.device))
-    if wav_len:
-        pcm[:wav_len].copy_(torch.from_numpy(np.concatenate(raws)))
-    with ctx.after_torch(pcm):            # the PCM copy lands before the decode writes after it
-        fst = flac.decode_into(ctx, pcm, fl_off)
-    for j, k in enumerate(fl):
-        if fst[j]:
-            status[k], nfr[k] = fst[j], 0
-    return _frontend_packed(ctx, pcm, inoff, nfr, channels, src_rates, dst_rate, resampler) + (status,)
-
-
-def _frontend_sources_bytes(sources, fl, channels, src_rates, dst_rate, device, resampler):
-    """_frontend_sources over a round that holds 24-bit, 32-bit or float WAV, or FLAC of 17-24 bits in
-    'ffmpeg' mode: every file's payload bytes in one buffer (_pack_payloads), FLAC decoded into it on the
-    device (full depth in 'ffmpeg' mode), one byte-form front-end call with a format per file."""
+        return pcm_frontend_batch(sources, channels, src_rates, dst_rate, device=device, resampler=resampler,
+                                  sample_formats=[_raw_format(s) for s in sources]) + (status,)
     import torch
-    n = len(sources)
-    status = np.zeros(n, np.int32)
     ctx = _lib.context(device)
-    is_flac = set(fl)
-    wav = [k for k in range(n) if k not in is_flac]
+    wav = [k for k, s in enumerate(sources) if not isinstance(s, flac.FlacStream)]
     fmts, nfr = np.zeros(n, np.int32), np.zeros(n, np.int64)
-    pays = []
-    for k in wav:
-        b, fmts[k] = _as_payload(sources[k], _raw_format(sources[k]))
-        nfr[k] = len(b) // _WIDTH[int(fmts[k])] // max(1, int(channels[k]))
-        pays.append(b)
-    full_depth = resampler == 'ffmpeg'
-    nsamples = flac.locate(ctx, [sources[k] for k in fl])[0] if fl else []
-    extra = []
+    pays, fmts[wav], nfr[wav] = _payloads([sources[k] for k in wav], [_raw_format(sources[k]) for k in wav],
+                                          [channels[k] for k in wav])
+    nsamples = flac.locate(ctx, [sources[k] for k in fl])[0]
     for j, k in enumerate(fl):
-        deep = full_depth and sources[k].bits_per_sample > 16
-        fmts[k] = _lib.PCM_S32 if deep else _lib.PCM_I16
-        nfr[k] = nsamples[j]
-        extra.append(int(nsamples[j]) * int(channels[k]) * _WIDTH[int(fmts[k])])
-    packed, boff = _pack_payloads(pays, extra)
+        fmts[k], nfr[k] = _flac_format(sources[k], resampler), nsamples[j]
+    packed, boff = _pack_payloads(pays, [int(nfr[k]) * int(channels[k]) * _WIDTH[int(fmts[k])] for k in fl])
     inoff = np.zeros(n, np.int64)
     inoff[wav] = boff[:len(wav)]
-    inoff[fl] = boff[len(wav):len(wav) + len(fl)]
-    if not fl:
-        return _frontend_packed(ctx, packed, inoff, nfr, channels, src_rates, dst_rate, resampler, fmts) + (status,)
-    pcm = torch.zeros(max(len(packed), 1), dtype=torch.uint8, device=torch.device("cuda", ctx.device))
+    inoff[fl] = boff[len(wav):n]
+    pcm = torch.empty(max(len(packed), 1), dtype=torch.uint8, device=torch.device("cuda", ctx.device))
     wav_len = int(boff[len(wav)])
     if wav_len:
         pcm[:wav_len].copy_(torch.from_numpy(packed[:wav_len]))
     with ctx.after_torch(pcm):            # the payload copy lands before the decode writes after it
-        fst = flac.decode_into_bytes(ctx, pcm, inoff[fl], full_depth)
-    for j, k in enumerate(fl):
-        if fst[j]:
-            status[k], nfr[k] = fst[j], 0
+        status[fl] = flac.decode_into_bytes(ctx, pcm, inoff[fl], resampler == 'ffmpeg')
+    nfr[status != 0] = 0
     return _frontend_packed(ctx, pcm, inoff, nfr, channels, src_rates, dst_rate, resampler, fmts) + (status,)
 
 
@@ -924,8 +842,8 @@ class Analyzer(object):
             return []        # the reference returns [] when there are no peaks (:401-402)
         return hashes
 
-    # bytes of raw PCM (WAV payload bytes: 2, 3 or 4 a sample; decoded FLAC: 2, or 4 for 17-24 bits in
-    # 'ffmpeg' mode; or a custom reader's float32) that wavfiles2hashes stages per device call
+    # bytes of raw PCM (WAV payload bytes: 2, 3 or 4 a sample; decoded FLAC at _flac_format's width; or a
+    # custom reader's float32) that wavfiles2hashes stages per device call
     max_pcm_bytes_per_call = 1 << 30
 
     def wavfiles2hashes(self, filenames):
@@ -934,10 +852,10 @@ class Analyzer(object):
         and the files' durations in `last_batch_durations`.
 
         WAVs read by the default reader are parsed on the host (_wav_read_raw); the raw PCM of a
-        chunk of files is staged once, down-mixed and resampled by ONE afp_pcm_frontend_batch call
-        into a device buffer, and fingerprinted there in place (fingerprint_packed).  FLAC files are
-        decoded on the device into the same staging buffer first (_frontend_sources); one the device
-        refuses is an unreadable file.  A custom
+        chunk of files is staged once, down-mixed and resampled by ONE front-end call into a device
+        buffer (_frontend_sources), and fingerprinted there in place (fingerprint_packed).  FLAC files
+        are decoded on the device into the same staging buffer first; one the device refuses is an
+        unreadable file.  A custom
         `reader` is called per file and its output packed as it is.  Runs of .afpk files are loaded
         on the host and hashed by ONE afp_fingerprint_from_peaks call per chunk; .afpt files are
         loaded as they are.  Chunks follow max_frames_per_call and max_pcm_bytes_per_call (a file
@@ -1059,9 +977,8 @@ class Analyzer(object):
                 return 'host', (i, None, 0.0), 0, 0
             if isinstance(raw, np.ndarray):
                 nbytes = raw.nbytes                   # the payload as it goes up: 2, 3 or 4 bytes a sample
-            else:                                     # decoded FLAC: int16, or int32 at full depth
-                deep = self.resampler == 'ffmpeg' and raw.bits_per_sample > 16
-                nbytes = (4 if deep else 2) * nframes * nch
+            else:                                     # decoded FLAC
+                nbytes = _WIDTH[_flac_format(raw, self.resampler)] * nframes * nch
             return 'pcm', (i, (raw, nch, fs), nout, None), nsh * (1 + nout // self.n_hop), nbytes
         d, sr = self._read(fn)
         if len(d) == 0:

@@ -15,15 +15,14 @@
 // scipy.signal.resample_poly cross-checks on the CPU.  ffmpeg's resampler, which the reference uses,
 // is not reproduced (§8f-2); parity statements against the reference are made on 11025 Hz PCM.
 //
-// afp_pcm_frontend_batch runs the same per-output function over a list of files in one launch: each
-// block belongs to one file (a per-file block prefix), each file's output starts on a 16-byte boundary
-// of one device buffer, laid out as afp_fingerprint_batch takes it, and every distinct (up, down)
+// afp_pcm_frontend_batch_bytes runs the same per-output function over a list of files in one launch,
+// over packed payload bytes with a sample format per file: a 24-bit, 32-bit or float sample enters as
+// the int16 `ffmpeg -ac 1` gives it at the file's own rate, at the sample load, so every format runs in
+// the same launch.  The layout, checks, upload and launch it shares with the ffmpeg front-end
+// (afp_pcm_formats.cuh); here are only the taps lookup and frontend_sample, and every distinct (up, down)
 // design is uploaded once.  tests/test_gpu_pcm_batch.py holds it bit-equal to afp_pcm_frontend per file.
-// afp_pcm_frontend_batch_bytes is the same call over packed payload bytes with a sample format per file
-// (afp_pcm_formats.cuh): a 24-bit, 32-bit or float sample enters as the int16 `ffmpeg -ac 1` gives it at
-// the file's own rate, at the sample load, so every format runs in the same launch.
-#include <cstring>
-
+// The package calls only this byte form; afp_pcm_frontend_batch (int16) forwards to it, and
+// afp_pcm_frontend keeps its single-file kernel for ABI callers and as the tests' per-file reference.
 #include "afp_internal.cuh"
 #include "afp_pcm_formats.cuh"
 
@@ -58,34 +57,16 @@ __global__ void __launch_bounds__(256) afp_pcm_frontend_kernel(const int16_t* pc
   out[n] = frontend_sample(reinterpret_cast<const uint8_t*>(pcm), AFP_PCM_I16, nframes, ch, up, down, taps, half, n);
 }
 
-// One file of a batched front-end call, built on the host.
-struct PcmFileDesc {
-  int64_t in_off;       // first byte of the file in the packed PCM
-  int64_t nframes;
-  int64_t out_off;      // first output sample (a multiple of 4: 16-byte aligned)
-  int64_t nout;         // ceil(nframes * up / down)
+// One file of a batched front-end call, built on the host; nout = ceil(nframes * up / down).
+struct PcmFileDesc : PcmFile {
   int64_t tap_off;      // first tap of the file's (up, down) design in the packed taps
-  int64_t block_base;   // first block of the file: the prefix sum of ceil(nout / 256)
-  int32_t ch, up, down, half, fmt;
+  int32_t up, down, half;
 };
 
-// Block b belongs to the last file whose block_base <= b (a file without outputs has the same base as
-// the next one), found by one thread per block with a binary search over the block prefix.
 __global__ void __launch_bounds__(256) afp_pcm_frontend_batch_kernel(const uint8_t* pcm, const PcmFileDesc* files,
                                                                      int nfiles, const double* taps, float* out) {
-  __shared__ int s_file;
-  const int64_t b = blockIdx.x;
-  if (threadIdx.x == 0) {
-    int lo = 0, hi = nfiles - 1;
-    while (lo < hi) {
-      const int mid = (lo + hi + 1) >> 1;
-      if (files[mid].block_base <= b) lo = mid; else hi = mid - 1;
-    }
-    s_file = lo;
-  }
-  __syncthreads();
-  const PcmFileDesc& f = files[s_file];
-  const int64_t n = (b - f.block_base) * blockDim.x + threadIdx.x;
+  const PcmFileDesc& f = files[pcm_block_file(files, nfiles)];
+  const int64_t n = ((int64_t)blockIdx.x - f.block_base) * blockDim.x + threadIdx.x;
   const int64_t nout = f.nout;
   if (n >= nout) return;
   out[f.out_off + n] =
@@ -132,9 +113,8 @@ extern "C" int afp_pcm_frontend_batch_bytes(afp_ctx* c, const uint8_t* pcm, int 
                                             const int64_t* tap_offsets, const double* taps, float* out,
                                             int64_t out_capacity, int64_t* out_offsets, int64_t* out_lengths) {
   if (!c) return AFP_ERR_INVALID;
-  if (nfiles < 0 || npairs < 0 || pcm_bytes < 0) AFP_FAIL(c, AFP_ERR_INVALID, "negative count");
-  if (nfiles > 0 && (!byte_offsets || !formats || !nframes || !channels || !up || !down))
-    AFP_FAIL(c, AFP_ERR_INVALID, "null per-file array");
+  if (npairs < 0) AFP_FAIL(c, AFP_ERR_INVALID, "negative count");
+  if (nfiles > 0 && (!up || !down)) AFP_FAIL(c, AFP_ERR_INVALID, "null per-file array");
   if (npairs > 0 && (!pair_rates || !tap_offsets || !taps)) AFP_FAIL(c, AFP_ERR_INVALID, "null taps table");
   // the taps table: one odd-length design per distinct (up, down), packed one after the other
   if (npairs > 0 && tap_offsets[0] != 0) AFP_FAIL(c, AFP_ERR_INVALID, "tap_offsets[0] must be 0");
@@ -143,72 +123,29 @@ extern "C" int afp_pcm_frontend_batch_bytes(afp_ctx* c, const uint8_t* pcm, int 
     if (pair_rates[2 * p] < 1 || pair_rates[2 * p + 1] < 1) AFP_FAIL(c, AFP_ERR_INVALID, "taps table: up and down must be >= 1");
     if (nt < 1 || !(nt & 1) || nt > INT32_MAX) AFP_FAIL(c, AFP_ERR_INVALID, "taps: odd length required");
   }
-  std::vector<PcmFileDesc> d((size_t)nfiles);
-  int64_t o = 0, blocks = 0;
-  int rc;
-  for (int f = 0; f < nfiles; ++f) {
-    PcmFileDesc& x = d[f];
-    x.nframes = nframes[f];
-    x.ch = channels[f];
+  std::vector<PcmFileDesc> d;
+  int64_t blocks = 0;
+  auto own = [&](int f, const std::string& tag, PcmFileDesc& x) -> int {
     x.up = up[f];
     x.down = down[f];
-    x.in_off = byte_offsets[f];
-    x.fmt = formats[f];
-    if (x.nframes < 0) AFP_FAIL(c, AFP_ERR_INVALID, "file " + std::to_string(f) + ": negative length");
-    if (x.ch < 1) AFP_FAIL(c, AFP_ERR_INVALID, "file " + std::to_string(f) + ": channels must be >= 1");
-    if (x.up < 1 || x.down < 1) AFP_FAIL(c, AFP_ERR_INVALID, "file " + std::to_string(f) + ": up and down must be >= 1");
-    if ((rc = pcm_check_input(c, f, pcm, pcm_on_host, pcm_bytes, x.in_off, x.fmt, x.nframes, x.ch))) return rc;
-    if (x.nframes > (INT64_MAX - x.down) / x.up) AFP_FAIL(c, AFP_ERR_INVALID, "file " + std::to_string(f) + ": too long");
-    x.tap_off = 0;
-    x.half = 0;
+    if (x.up < 1 || x.down < 1) AFP_FAIL(c, AFP_ERR_INVALID, tag + "up and down must be >= 1");
+    if (x.nframes > (INT64_MAX - x.down) / x.up) AFP_FAIL(c, AFP_ERR_INVALID, tag + "too long");
     if (!(x.up == 1 && x.down == 1)) {
       int p = 0;
       while (p < npairs && !(pair_rates[2 * p] == x.up && pair_rates[2 * p + 1] == x.down)) ++p;
-      if (p == npairs) AFP_FAIL(c, AFP_ERR_INVALID, "file " + std::to_string(f) + ": no taps for its (up, down)");
+      if (p == npairs) AFP_FAIL(c, AFP_ERR_INVALID, tag + "no taps for its (up, down)");
       x.tap_off = tap_offsets[p];
       x.half = (int32_t)((tap_offsets[p + 1] - tap_offsets[p] - 1) / 2);
     }
     x.nout = (x.nframes * x.up + x.down - 1) / x.down;                   // ceil, as resample_poly
-    x.out_off = o;
-    x.block_base = blocks;
-    o += (x.nout + 3) & ~(int64_t)3;
-    blocks += (x.nout + 255) / 256;
-  }
-  if (blocks > INT32_MAX) AFP_FAIL(c, AFP_ERR_INVALID, "batch too large for one launch");
-  if (out) {
-    if (o > out_capacity) AFP_FAIL(c, AFP_ERR_INVALID, "output buffer smaller than the batch's " + std::to_string(o) + " samples");
-    if (blocks > 0 && !pcm) AFP_FAIL(c, AFP_ERR_INVALID, "null pcm");
-  }
-  if (out_offsets) {
-    for (int f = 0; f < nfiles; ++f) out_offsets[f] = d[f].out_off;
-    out_offsets[nfiles] = o;
-  }
-  if (out_lengths)
-    for (int f = 0; f < nfiles; ++f) out_lengths[f] = d[f].nout;
-  if (!out || blocks == 0) return AFP_OK;                                 // sizing call, or nothing to compute
-  AFP_CUDA(c, cudaSetDevice(c->device));
-  const uint8_t* dpcm = nullptr;
-  if ((rc = afp_stage(c, c->d_pcm_stage, pcm, (size_t)pcm_bytes, pcm_on_host, &dpcm))) return rc;
-  if (pcm_on_host) c->batch_valid = false;   // the PCM staging buffer of the last fingerprint batch is overwritten
-  // descriptors and every distinct design's taps in one upload
-  const int64_t ntaps = npairs > 0 ? tap_offsets[npairs] : 0;
-  PcmFileDesc* dd = nullptr;
-  double* dtaps = nullptr;
-  size_t desc_bytes = 0;
-  if ((rc = afp_carve(c, c->d_tmp, [&](Carver& k) {
-         dd = k.take<PcmFileDesc>(nfiles);
-         desc_bytes = k.bytes;
-         dtaps = k.take<double>(ntaps);
-       })))
-    return rc;
-  std::vector<char> h(desc_bytes + sizeof(double) * (size_t)ntaps);
-  memcpy(h.data(), d.data(), sizeof(PcmFileDesc) * (size_t)nfiles);
-  if (ntaps) memcpy(h.data() + desc_bytes, taps, sizeof(double) * (size_t)ntaps);
-  AFP_CUDA(c, afp_copy_in(c, reinterpret_cast<char*>(dd), h.data(), h.size(), 1));
-  if ((rc = afp_launch(c, afp_pcm_frontend_batch_kernel, (unsigned)blocks, 256, 0, dpcm, dd, nfiles, dtaps, out)))
-    return rc;
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));       // one synchronise for the whole list (`h` is pageable)
-  return AFP_OK;
+    return AFP_OK;
+  };
+  const int rc = pcm_batch_layout(c, pcm, pcm_on_host, pcm_bytes, nfiles, byte_offsets, formats, nframes, channels, own,
+                                  out, out_capacity, out_offsets, out_lengths, &d, &blocks);
+  if (rc || !out || blocks == 0) return rc;                   // a refused call, a sizing call, or nothing to compute
+  // every distinct design's taps go up once, after the descriptors
+  return pcm_batch_launch(c, afp_pcm_frontend_batch_kernel, pcm, pcm_on_host, pcm_bytes, d, blocks,
+                          {{taps, npairs > 0 ? tap_offsets[npairs] : 0}}, out);
 }
 
 extern "C" int afp_pcm_frontend_batch(afp_ctx* c, const int16_t* pcm, int pcm_on_host, int64_t pcm_len, int32_t nfiles,

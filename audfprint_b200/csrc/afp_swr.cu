@@ -22,9 +22,12 @@
 // library's own output and tests/test_gpu_ffmpeg_frontend.py holds this kernel to both.  One thread
 // computes one output and reads its taps from global memory through the cache.  A design has P L
 // floats: 1 KB at 22050 Hz, 83 KB at 48000 Hz, up to 166 KB (32000 and 96000 Hz: 441 and 147 phases).
-// tools/ffmpeg_frontend_timing.py measures the kernel against afp_pcm_frontend_batch.
+// tools/ffmpeg_frontend_timing.py measures the kernel against the default front-end.
+//
+// The batch's layout, checks, upload and launch are the default front-end's (afp_pcm_formats.cuh); here
+// are only the geometry, the cached designs, the edges and swr_sample.  The package calls only the byte
+// form; afp_swr_frontend_batch (int16) forwards to it for ABI callers.
 #include <cmath>
-#include <cstring>
 #include <map>
 #include <mutex>
 #include <numeric>
@@ -114,9 +117,9 @@ const std::vector<float>& cached_design(int32_t in_rate, int32_t out_rate, const
   return v;
 }
 
-struct SwrFileDesc {
-  int64_t in_off, nframes, out_off, nout, bank_off, block_base;
-  int32_t ch, P, D, L, resample, fmt;
+struct SwrFileDesc : PcmFile {
+  int64_t bank_off;
+  int32_t P, D, L, resample;
 };
 
 // sample c of extended input position e: mirrored around the end, then around 0 (the output count keeps
@@ -169,19 +172,8 @@ __device__ __forceinline__ float swr_sample(const uint8_t* pcm, const SwrFileDes
 
 __global__ void __launch_bounds__(256) afp_swr_frontend_kernel(const uint8_t* pcm, const SwrFileDesc* files, int nfiles,
                                                               const float* banks, float* out) {
-  __shared__ int s_file;
-  const int64_t b = blockIdx.x;
-  if (threadIdx.x == 0) {
-    int lo = 0, hi = nfiles - 1;
-    while (lo < hi) {
-      const int mid = (lo + hi + 1) >> 1;
-      if (files[mid].block_base <= b) lo = mid; else hi = mid - 1;
-    }
-    s_file = lo;
-  }
-  __syncthreads();
-  const SwrFileDesc f = files[s_file];
-  const int64_t n = (b - f.block_base) * blockDim.x + threadIdx.x;
+  const SwrFileDesc f = files[pcm_block_file(files, nfiles)];
+  const int64_t n = ((int64_t)blockIdx.x - f.block_base) * blockDim.x + threadIdx.x;
   if (n >= f.nout) return;
   out[f.out_off + n] = swr_sample(pcm + f.in_off, f, banks + f.bank_off, n);
 }
@@ -220,90 +212,41 @@ extern "C" int afp_swr_frontend_batch_bytes(afp_ctx* c, const uint8_t* pcm, int 
                                             int32_t out_rate, float* out, int64_t out_capacity, int64_t* out_offsets,
                                             int64_t* out_lengths) {
   if (!c) return AFP_ERR_INVALID;
-  if (nfiles < 0 || pcm_bytes < 0) AFP_FAIL(c, AFP_ERR_INVALID, "negative count");
   if (out_rate < 1) AFP_FAIL(c, AFP_ERR_INVALID, "output rate must be >= 1");
-  if (nfiles > 0 && (!byte_offsets || !formats || !nframes || !channels || !rates))
-    AFP_FAIL(c, AFP_ERR_INVALID, "null per-file array");
-  std::vector<SwrFileDesc> d((size_t)nfiles);
-  std::vector<std::pair<int32_t, const std::vector<float>*>> uniq;   // distinct input rates, first use first
-  int64_t o = 0, blocks = 0, nbank = 0;
-  int rc;
-  for (int f = 0; f < nfiles; ++f) {
-    SwrFileDesc& x = d[f];
-    const std::string tag = "file " + std::to_string(f) + ": ";
-    x.nframes = nframes[f];
-    x.ch = channels[f];
-    x.in_off = byte_offsets[f];
-    x.fmt = formats[f];
-    if (x.nframes < 0) AFP_FAIL(c, AFP_ERR_INVALID, tag + "negative length");
-    if (x.ch < 1) AFP_FAIL(c, AFP_ERR_INVALID, tag + "channels must be >= 1");
+  if (nfiles > 0 && !rates) AFP_FAIL(c, AFP_ERR_INVALID, "null per-file array");
+  std::vector<SwrFileDesc> d;
+  std::vector<int32_t> uniq;                               // distinct input rates, first use first
+  std::vector<std::pair<const float*, int64_t>> banks;     // and their designs
+  int64_t blocks = 0;
+  auto own = [&](int f, const std::string& tag, SwrFileDesc& x) -> int {
     if (rates[f] < 1) AFP_FAIL(c, AFP_ERR_INVALID, tag + "sample rate must be >= 1");
     if (x.ch > 2) AFP_FAIL(c, AFP_ERR_UNSUPPORTED, tag + "the ffmpeg front-end takes mono or stereo");
-    if ((rc = pcm_check_input(c, f, pcm, pcm_on_host, pcm_bytes, x.in_off, x.fmt, x.nframes, x.ch))) return rc;
     x.resample = rates[f] != out_rate;
     x.P = x.D = x.L = 1;
-    x.bank_off = 0;
     x.nout = x.nframes;
-    if (x.resample) {
-      SwrGeometry g;
-      if (!swr_geometry(rates[f], out_rate, &g))
-        AFP_FAIL(c, AFP_ERR_UNSUPPORTED, tag + std::to_string(rates[f]) + " Hz needs interpolated phases or more than 528 taps");
-      if (x.nframes > (INT64_MAX / 2 - g.L) / g.P) AFP_FAIL(c, AFP_ERR_INVALID, tag + "too long");
-      x.P = g.P;
-      x.D = g.D;
-      x.L = g.L;
-      x.nout = swr_edges(g, x.nframes);
-      size_t u = 0;
-      int64_t off = 0;
-      while (u < uniq.size() && uniq[u].first != rates[f]) off += (int64_t)uniq[u++].second->size();
-      if (u == uniq.size()) {
-        uniq.push_back({rates[f], &cached_design(rates[f], out_rate, g)});
-        nbank += (int64_t)g.P * g.L;
-      }
-      x.bank_off = off;
+    if (!x.resample) return AFP_OK;
+    SwrGeometry g;
+    if (!swr_geometry(rates[f], out_rate, &g))
+      AFP_FAIL(c, AFP_ERR_UNSUPPORTED, tag + std::to_string(rates[f]) + " Hz needs interpolated phases or more than 528 taps");
+    if (x.nframes > (INT64_MAX / 2 - g.L) / g.P) AFP_FAIL(c, AFP_ERR_INVALID, tag + "too long");
+    x.P = g.P;
+    x.D = g.D;
+    x.L = g.L;
+    x.nout = swr_edges(g, x.nframes);
+    size_t u = 0;
+    while (u < uniq.size() && uniq[u] != rates[f]) x.bank_off += banks[u++].second;
+    if (u == uniq.size()) {
+      const std::vector<float>& bank = cached_design(rates[f], out_rate, g);
+      uniq.push_back(rates[f]);
+      banks.push_back({bank.data(), (int64_t)bank.size()});
     }
-    x.out_off = o;
-    x.block_base = blocks;
-    o += (x.nout + 3) & ~(int64_t)3;
-    blocks += (x.nout + 255) / 256;
-  }
-  if (blocks > INT32_MAX) AFP_FAIL(c, AFP_ERR_INVALID, "batch too large for one launch");
-  if (out) {
-    if (o > out_capacity) AFP_FAIL(c, AFP_ERR_INVALID, "output buffer smaller than the batch's " + std::to_string(o) + " samples");
-    if (blocks > 0 && !pcm) AFP_FAIL(c, AFP_ERR_INVALID, "null pcm");
-  }
-  if (out_offsets) {
-    for (int f = 0; f < nfiles; ++f) out_offsets[f] = d[f].out_off;
-    out_offsets[nfiles] = o;
-  }
-  if (out_lengths)
-    for (int f = 0; f < nfiles; ++f) out_lengths[f] = d[f].nout;
-  if (!out || blocks == 0) return AFP_OK;                                 // sizing call, or nothing to compute
-  AFP_CUDA(c, cudaSetDevice(c->device));
-  const uint8_t* dpcm = nullptr;
-  if ((rc = afp_stage(c, c->d_pcm_stage, pcm, (size_t)pcm_bytes, pcm_on_host, &dpcm))) return rc;
-  if (pcm_on_host) c->batch_valid = false;   // the PCM staging buffer of the last fingerprint batch is overwritten
-  // descriptors and every distinct rate's design in one upload
-  SwrFileDesc* dd = nullptr;
-  float* dbank = nullptr;
-  size_t desc_bytes = 0;
-  if ((rc = afp_carve(c, c->d_tmp, [&](Carver& k) {
-         dd = k.take<SwrFileDesc>(nfiles);
-         desc_bytes = k.bytes;
-         dbank = k.take<float>(nbank);
-       })))
-    return rc;
-  std::vector<char> h(desc_bytes + sizeof(float) * (size_t)nbank);
-  memcpy(h.data(), d.data(), sizeof(SwrFileDesc) * (size_t)nfiles);
-  size_t pos = desc_bytes;
-  for (auto& u : uniq) {
-    memcpy(h.data() + pos, u.second->data(), sizeof(float) * u.second->size());
-    pos += sizeof(float) * u.second->size();
-  }
-  AFP_CUDA(c, afp_copy_in(c, reinterpret_cast<char*>(dd), h.data(), h.size(), 1));
-  if ((rc = afp_launch(c, afp_swr_frontend_kernel, (unsigned)blocks, 256, 0, dpcm, dd, nfiles, dbank, out))) return rc;
-  AFP_CUDA(c, cudaStreamSynchronize(c->stream));       // one synchronise for the whole list (`h` is pageable)
-  return AFP_OK;
+    return AFP_OK;
+  };
+  const int rc = pcm_batch_layout(c, pcm, pcm_on_host, pcm_bytes, nfiles, byte_offsets, formats, nframes, channels, own,
+                                  out, out_capacity, out_offsets, out_lengths, &d, &blocks);
+  if (rc || !out || blocks == 0) return rc;                   // a refused call, a sizing call, or nothing to compute
+  // every distinct rate's design goes up once, after the descriptors
+  return pcm_batch_launch(c, afp_swr_frontend_kernel, pcm, pcm_on_host, pcm_bytes, d, blocks, banks, out);
 }
 
 extern "C" int afp_swr_frontend_batch(afp_ctx* c, const int16_t* pcm, int pcm_on_host, int64_t pcm_len, int32_t nfiles,

@@ -1,5 +1,5 @@
 """FLAC input: the host half (recognising a FLAC file, reading its metadata blocks) and the calls of
-the device decoder (afp_flac_locate_batch / afp_flac_decode_batch, include/afp.h).
+the device decoder (afp_flac_locate_batch / afp_flac_decode_batch_bytes, include/afp.h).
 
 The host only finds where the frames start and what STREAMINFO says; locating, checking and decoding
 the frames run on the device.  Native FLAC only: Ogg-FLAC (an Ogg container) is not recognised and
@@ -117,21 +117,16 @@ def locate(ctx, streams):
 
 
 def decode_into(ctx, out, out_offsets):
-    """afp_flac_decode_batch of the last located batch into the device int16 tensor `out` (the caller
-    orders it against torch with ctx.after_torch): file i at out[out_offsets[i]:].  -> status int32 [n]."""
-    off = np.ascontiguousarray(out_offsets, dtype=np.int64)
-    n = len(off)
-    status = np.zeros(max(n, 1), np.int32)
-    rc = ctx.lib.afp_flac_decode_batch(ctx.h, out.data_ptr(), out.numel(), off.ctypes.data_as(C.POINTER(C.c_int64)),
-                                       status.ctypes.data)
-    _check_files(ctx, rc, status)
-    return status[:n]
+    """decode_into_bytes of the last located batch into the device int16 tensor `out`, every file int16:
+    file i at out[out_offsets[i]:].  -> status int32 [n]."""
+    import torch
+    return decode_into_bytes(ctx, out.view(torch.uint8), 2 * np.asarray(out_offsets, dtype=np.int64), False)
 
 
 def decode_into_bytes(ctx, out, out_offsets, full_depth):
-    """afp_flac_decode_batch_bytes of the last located batch into the device uint8 tensor `out`: file i
-    at byte out_offsets[i], int16, or with full_depth a file of 17-24 bits as int32 x << (32 - bits).
-    -> status int32 [n]."""
+    """afp_flac_decode_batch_bytes of the last located batch into the device uint8 tensor `out` (the
+    caller orders it against torch with ctx.after_torch): file i at byte out_offsets[i], int16, or with
+    full_depth a file of 17-24 bits as int32 x << (32 - bits).  -> status int32 [n]."""
     off = np.ascontiguousarray(out_offsets, dtype=np.int64)
     n = len(off)
     status = np.zeros(max(n, 1), np.int32)
