@@ -10,7 +10,6 @@ spectrogram, a peak or a hash on the CPU.
 """
 from __future__ import annotations
 
-import contextlib
 import ctypes as C
 import os
 import struct
@@ -713,17 +712,12 @@ class Analyzer(object):
         """Waveform -> list of (time_frame, freq_bin) (audfprint_analyze.py:255-308)."""
         if len(d) == 0:
             return []
-        return self._fetch_peaks(self._fingerprint_one(d, 1), 0, 1)[0]
-
-    def _fingerprint_one(self, d, shifts):
-        """Fingerprint one signal in one device call at `shifts`; the results stay in the workspace.
-        Returns the context."""
         a, dtype = _as_pcm(d)
-        ctx = self._configure(shifts)
+        ctx = self._configure(1)
         off = np.array([0, len(a)], np.int64)
         ctx.check(ctx.lib.afp_fingerprint_batch(ctx.h, a.ctypes.data, dtype, 1, 1,
                                                 off.ctypes.data_as(C.POINTER(C.c_int64)), None, None))
-        return ctx
+        return self._fetch_peaks(ctx, 0, 1)[0]
 
     def _fetch_peaks(self, ctx, shift, nfiles):
         poff = np.empty(nfiles + 1, np.int64)
@@ -781,15 +775,17 @@ class Analyzer(object):
             raise IOError(message)
         print(message, "skipping")
 
-    @contextlib.contextmanager
-    def _counters_restored_on_error(self):
-        """Leave soundfiledur / soundfiletotaldur / soundfilecount as they were if the body raises."""
+    def _list_form(self, run):
+        """A list form's bookkeeping around run() -> (results, durations): the durations go to
+        `last_batch_durations`, and if run() raises, soundfiledur / soundfiletotaldur / soundfilecount
+        are left as they were.  The per-file calls run the same drivers on one file without it."""
         saved = (self.soundfiledur, self.soundfiletotaldur, self.soundfilecount)
         try:
-            yield
+            results, self.last_batch_durations = run()
         except BaseException:
             self.soundfiledur, self.soundfiletotaldur, self.soundfilecount = saved
             raise
+        return results
 
     def _account(self, dur):
         self.soundfiledur = dur
@@ -798,49 +794,14 @@ class Analyzer(object):
 
     def wavfile2peaks(self, filename, shifts=None):
         """Soundfile -> peaks, or list of peak lists when shifts > 1
-        (audfprint_analyze.py:345-383)."""
-        ext = os.path.splitext(filename)[1]
-        if ext == PRECOMPPKEXT:
-            peaks = peaks_load(filename)
-            dur = np.max(peaks, axis=0)[0] * self.n_hop / self.target_sr
-        else:
-            d, sr = self._read(filename)
-            dur = len(d) / sr
-            if shifts is None or shifts < 2:
-                peaks = self.find_peaks(d, sr)
-            elif len(d) == 0:
-                peaks = [[] for _ in range(shifts)]
-            else:
-                # NB the reference takes the offsets from self.shifts (:375)
-                ctx = self._fingerprint_one(d, self.shifts)
-                peaks = [self._fetch_peaks(ctx, s, 1)[0] for s in range(min(shifts, self.shifts))]
-        self._account(dur)
-        return peaks
+        (audfprint_analyze.py:345-383): the driver of wavfiles2peaks run on the one file."""
+        return self._peaks_of_files([filename], shifts)[0][0]
 
     def wavfile2hashes(self, filename):
-        """Soundfile -> int32 (U,2) [time, hash] rows (audfprint_analyze.py:385-426)."""
-        ext = os.path.splitext(filename)[1]
-        if ext == PRECOMPEXT:
-            hashes = hashes_load(filename)
-            dur = np.max(hashes, axis=0)[0] * self.n_hop / self.target_sr
-            self._account(dur)
-            return hashes
-        if ext == PRECOMPPKEXT:
-            peaks = self.wavfile2peaks(filename, self.shifts)
-            if len(peaks) == 0:
-                return []
-            results = [None]
-            self._fingerprint_peaks([_peak_rows(peaks)])
-            self._collect_hashes([0], results, False, False)
-            return results[0]
-        d, sr = self._read(filename)
-        self._account(len(d) / sr)
-        if len(d) == 0:
-            return []
-        hashes = self.fingerprint_batch([d], self.shifts)[0]
-        if self.shifts < 2 and len(hashes) == 0:
-            return []        # the reference returns [] when there are no peaks (:401-402)
-        return hashes
+        """Soundfile -> int32 (U,2) [time, hash] rows (audfprint_analyze.py:385-426): the driver of
+        wavfiles2hashes run on the one file, so a malformed .afpk file stays counted when it raises,
+        as in the reference."""
+        return self._hashes_of_files([filename])[0][0]
 
     # bytes of raw PCM (WAV payload bytes: 2, 3 or 4 a sample; decoded FLAC at _flac_format's width; or a
     # custom reader's float32) that wavfiles2hashes stages per device call
@@ -862,48 +823,46 @@ class Analyzer(object):
         over a cap goes alone); the results do not depend on where they fall.
 
         Files are read in list order.  With fail_on_error, the first unreadable file raises the
-        IOError _read raises, and nothing is returned: unlike the per-file loop, which has already
-        returned the earlier files' hashes by then, the counters are left as they were.  A malformed
-        precomputed file raises what wavfile2hashes raises for it, the same way."""
-        return self._hashes_of_files(filenames, rows_on_device=False)
+        IOError wavfile2hashes raises, and nothing is returned: unlike the per-file loop, which has
+        already returned the earlier files' hashes by then, the counters are left as they were.  A
+        malformed precomputed file raises what wavfile2hashes raises for it, the same way."""
+        return self._list_form(lambda: self._hashes_of_files(filenames))
 
     def _hashes_of_files(self, filenames, rows_on_device=False):
-        """wavfiles2hashes; with rows_on_device the fingerprinted files' hashes stay on the device
-        (afp_fetch_hashes into a torch tensor) as DeviceHashes."""
+        """The driver of wavfile2hashes and wavfiles2hashes -> (hashes, durations) per file; with
+        rows_on_device the fingerprinted files' hashes stay on the device (afp_fetch_hashes into a
+        torch tensor) as DeviceHashes."""
         def collect(kind, idx, results):
             # the reference returns [] when a WAV has no peaks (:401-402)
             self._collect_hashes(idx, results, rows_on_device, kind == 'pcm' and self.shifts < 2)
         return self._analyse_files(filenames, False, max(1, int(self.shifts)), collect, list)
 
     def _analyse_files(self, filenames, peaks_mode, nsh, collect, empty):
-        """The list forms' driver: read `filenames` in rounds (_file_rounds), run each device round at
-        nsh shifts and hand it to `collect(kind, indices, results)`, which puts the round's results at
+        """The file driver: read `filenames` in rounds (_file_rounds), run each device round at nsh
+        shifts and hand it to `collect(kind, indices, results)`, which puts the round's results at
         their indices.  A file whose result is known on the host takes it as it is, or `empty()` when
-        it has no samples.  The counters end as the per-file loop leaves them, or as they were if
-        anything raises; the files' durations go to `last_batch_durations`."""
+        it has no samples.  -> (results, durations).  The files are counted after the last round.
+        When a file raises nothing is counted, except a malformed .afpk file, which the reference
+        counts before it raises (_peaks_round); the list forms then restore the counters (_list_form)."""
         n = len(filenames)
         results, durs = [None] * n, [0.0] * n
-        with self._counters_restored_on_error():
-            for kind, items in self._file_rounds(filenames, peaks_mode, nsh, False):
-                if kind == 'host':
-                    for i, value, dur in items:
-                        results[i], durs[i] = (empty() if value is None else value), dur
-                    continue
-                refused = []
-                if kind == 'pcm':
-                    refused = self._fingerprint_pcm(items, nsh, durs)
-                    self._refuse(filenames, items, refused)
-                else:
-                    self._fingerprint_peaks([it[1] for it in items])
-                    for i, _, dur in items:
-                        durs[i] = dur
-                collect(kind, [it[0] for it in items], results)
-                for k, _ in refused:
-                    results[items[k][0]] = empty()      # what the per-file call gives an unreadable file
+        for kind, items in self._file_rounds(filenames, peaks_mode, nsh, False):
+            if kind == 'host':
+                for i, value, dur in items:
+                    results[i], durs[i] = (empty() if value is None else value), dur
+                continue
+            refused = []
+            if kind == 'pcm':
+                refused = self._fingerprint_pcm(items, nsh, durs)
+                self._refuse(filenames, items, refused)
+            else:
+                self._peaks_round(items, durs)
+            collect(kind, [it[0] for it in items], results)
+            for k, _ in refused:
+                results[items[k][0]] = empty()          # an unreadable file has no samples
         for dur in durs:
             self._account(dur)
-        self.last_batch_durations = durs
-        return results
+        return results, durs
 
     def _file_rounds(self, filenames, peaks_mode, nsh, in_order):
         """Read `filenames` in list order and group them into rounds of one kind, each one device call:
@@ -945,8 +904,8 @@ class Analyzer(object):
             yield kind, items
 
     def _read_item(self, i, fn, nsh, peaks_mode):
-        """One file of _file_rounds -> (kind, item, frames, bytes).  Raises what the per-file call
-        raises for a file it cannot read (fail_on_error), before anything is counted."""
+        """One file of _file_rounds -> (kind, item, frames, bytes).  Raises for a file it cannot read
+        (_read_failed, fail_on_error), before anything is counted."""
         ext = os.path.splitext(fn)[1]
         if ext == PRECOMPEXT and not peaks_mode:
             hashes = hashes_load(fn)
@@ -962,7 +921,7 @@ class Analyzer(object):
             try:
                 raw, nch, fs = _audio_read_raw(fn)
                 if fs < 1:
-                    # the per-file reader fails here in the device front-end (down < 1)
+                    # no rate to resample from: the device front-end would refuse it (down < 1)
                     raise ValueError("%s: sample rate %d" % (fn, fs))
                 nframes = len(raw) // nch if isinstance(raw, np.ndarray) else self._flac_frames(raw)
                 if _check_resampler(self.resampler) == 'ffmpeg':
@@ -1045,6 +1004,24 @@ class Analyzer(object):
                     e.file_index = int(np.flatnonzero(status)[0])
                 raise
 
+    def _peaks_round(self, items, durs, before=None):
+        """Fingerprint one 'peaks' round of _file_rounds (_fingerprint_peaks); file i's duration goes
+        to durs[i].  A malformed file raises, counted first as the per-file call counts it: the
+        reference's wavfile2peaks counts the file before its peaks are hashed.  `before(k)`, when
+        given, finishes the k files before it ahead of that count."""
+        for i, _, dur in items:
+            durs[i] = dur
+        try:
+            self._fingerprint_peaks([it[1] for it in items])
+        except Exception as e:
+            k = getattr(e, 'file_index', None)
+            if k is None:
+                raise
+            if before is not None:
+                before(k)
+            self._account(durs[items[k][0]])
+            raise
+
     def _collect_hashes(self, idx, results, rows_on_device, empty_as_list):
         """Put the hashes of the last device call's files at their indices `idx` of `results`; with
         empty_as_list a file without hashes gets []."""
@@ -1077,10 +1054,15 @@ class Analyzer(object):
 
         Audio goes through the batched front-end and ONE fingerprint call per chunk, at 1 shift when
         `shifts` is None or < 2, else at self.shifts with min(shifts, self.shifts) peak lists per
-        file (the per-file call's rule); one afp_fetch_peaks per shift serves the whole chunk.
-        .afpk files are loaded on the host; .afpt files are read as audio, as the per-file call
-        reads them.  Failures behave as in wavfiles2hashes."""
+        file (`shifts` empty lists for audio without samples); one afp_fetch_peaks per shift serves
+        the whole chunk.  .afpk files are loaded on the host; .afpt files are read as audio, as the
+        reference reads them.  Failures behave as in wavfiles2hashes."""
+        return self._list_form(lambda: self._peaks_of_files(filenames, shifts))
+
+    def _peaks_of_files(self, filenames, shifts):
+        """The driver of wavfile2peaks and wavfiles2peaks -> (peaks, durations) per file."""
         multi = not (shifts is None or shifts < 2)
+        # NB the reference takes the offsets from self.shifts (audfprint_analyze.py:375)
         nsh = max(1, int(self.shifts)) if multi else 1
 
         def collect(kind, idx, results):
@@ -1147,21 +1129,13 @@ class Analyzer(object):
                         finish()
                     self._refuse(filenames, items, refused)
                 else:
-                    for i, _, dur in items:
-                        durs[i] = dur
-                    try:
-                        self._fingerprint_peaks([it[1] for it in items])
-                    except Exception as e:
-                        k = getattr(e, 'file_index', None)
-                        if k is None:
-                            raise
-                        # the loop stores the files before the malformed one, and has counted it
+                    def before(k):
+                        # the loop stores the files before the malformed one
                         if k:
                             self._fingerprint_peaks([it[1] for it in items[:k]])
                             begin(idx[:k], None)
                         finish()
-                        self._account(durs[idx[k]])
-                        raise e
+                    self._peaks_round(items, durs, before)
                 begin(idx, None)
             finish()
         except BaseException:

@@ -608,7 +608,8 @@ def match_files_sharded(matcher, analyzer, ht, filenames, root=0, group=None):
     idx = shard_indices(n, rank, ws)
     err, mine = None, []
     try:
-        mine = matcher._files_msgs(analyzer, ht, [filenames[i] for i in idx], [int(i) for i in idx])
+        mine = analyzer._list_form(lambda: matcher._files_msgs(analyzer, ht, [filenames[i] for i in idx],
+                                                               [int(i) for i in idx]))
     except Exception as e:          # raised on every rank after the status exchange
         err = e
     _raise_if_failed(err, gather_objects(_status_code(err), group), "match_files_sharded", group)

@@ -467,16 +467,8 @@ class Matcher(object):
 
     def match_file(self, analyzer, ht, filename, number=None):
         """Read, fingerprint and match one file -> (rows[:max_returns], duration in s, #hashes)
-        (audfprint_match.py:354-379)."""
-        query = analyzer.wavfile2hashes(filename)
-        nhashes = len(query)
-        seconds = analyzer.n_hop * query[-1][0] / analyzer.target_sr if nhashes else 0.0
-        if self.verbose:
-            self._print_analyzed(filename, number, seconds, nhashes)
-        rows = self.match_hashes(ht, query)
-        if self.sort_by_time:
-            rows = rows[(-rows[:, 2]).argsort(), :]
-        return rows[:self.max_returns, :], seconds, nhashes
+        (audfprint_match.py:354-379): match_files' driver over the one file."""
+        return self._match_files(analyzer, ht, [filename], [number])[0][0]
 
     @staticmethod
     def _print_analyzed(filename, number, seconds, nhashes):
@@ -497,31 +489,31 @@ class Matcher(object):
         With analyzer.fail_on_error, an unreadable file raises the IOError match_file raises and
         leaves the analyzer's counters as they were; nothing is returned (the per-file loop would
         have matched the earlier files by then)."""
-        return self._match_files(analyzer, ht, filenames, range(start, start + len(filenames)))
+        return analyzer._list_form(lambda: self._match_files(analyzer, ht, filenames,
+                                                             range(start, start + len(filenames))))
 
     def _match_files(self, analyzer, ht, filenames, numbers):
+        """The driver of match_file and match_files -> (match_file's tuple, duration) per file."""
         self._params()                     # illustrate raises before any file is read
         durs = []
         on_device = hasattr(ht, "_sync_device") and _lib.context(ht.device) is _lib.context(analyzer.device)
         out = []
-        with analyzer._counters_restored_on_error():
-            for c0 in range(0, len(filenames), max(1, int(self.max_files_per_call))):
-                names = filenames[c0:c0 + max(1, int(self.max_files_per_call))]
-                queries = analyzer._hashes_of_files(names, rows_on_device=on_device)
-                durs += analyzer.last_batch_durations
-                secs = []
-                for fn, num, q in zip(names, numbers[c0:c0 + len(names)], queries):
-                    nh = len(q)
-                    last = q.last_time if isinstance(q, DeviceHashes) else (q[-1][0] if nh else None)
-                    secs.append(analyzer.n_hop * last / analyzer.target_sr if nh else 0.0)
-                    if self.verbose:
-                        self._print_analyzed(fn, num, secs[-1], nh)
-                for q, sec, rows in zip(queries, secs, self.match_batch(ht, self._pack_queries(queries, on_device))):
-                    if self.sort_by_time:
-                        rows = rows[(-rows[:, 2]).argsort(), :]
-                    out.append((rows[:self.max_returns, :], sec, len(q)))
-        analyzer.last_batch_durations = durs
-        return out
+        for c0 in range(0, len(filenames), max(1, int(self.max_files_per_call))):
+            names = filenames[c0:c0 + max(1, int(self.max_files_per_call))]
+            queries, round_durs = analyzer._hashes_of_files(names, rows_on_device=on_device)
+            durs += round_durs
+            secs = []
+            for fn, num, q in zip(names, numbers[c0:c0 + len(names)], queries):
+                nh = len(q)
+                last = q.last_time if isinstance(q, DeviceHashes) else (q[-1][0] if nh else None)
+                secs.append(analyzer.n_hop * last / analyzer.target_sr if nh else 0.0)
+                if self.verbose:
+                    self._print_analyzed(fn, num, secs[-1], nh)
+            for q, sec, rows in zip(queries, secs, self.match_batch(ht, self._pack_queries(queries, on_device))):
+                if self.sort_by_time:
+                    rows = rows[(-rows[:, 2]).argsort(), :]
+                out.append((rows[:self.max_returns, :], sec, len(q)))
+        return out, durs
 
     @staticmethod
     def _pack_queries(queries, on_device):
@@ -549,11 +541,13 @@ class Matcher(object):
     def files_match_to_msgs(self, analyzer, ht, filenames, start=0):
         """List form of file_match_to_msgs (match_files, file i numbered start + i): one list of
         report lines per file, in list order."""
-        return self._files_msgs(analyzer, ht, filenames, range(start, start + len(filenames)))
+        return analyzer._list_form(lambda: self._files_msgs(analyzer, ht, filenames,
+                                                            range(start, start + len(filenames))))
 
     def _files_msgs(self, analyzer, ht, filenames, numbers):
-        res = self._match_files(analyzer, ht, filenames, numbers)
-        return [self._msgs(analyzer, ht, fn, *r) for fn, r in zip(filenames, res)]
+        """The driver of files_match_to_msgs -> (report lines, duration) per file."""
+        res, durs = self._match_files(analyzer, ht, filenames, numbers)
+        return [self._msgs(analyzer, ht, fn, *r) for fn, r in zip(filenames, res)], durs
 
     def _msgs(self, analyzer, ht, qry, rows, seconds, nhashes):
         frame_s = analyzer.n_hop / analyzer.target_sr

@@ -177,6 +177,30 @@ def test_wavfiles2hashes_equals_wavfile2hashes(indir):
         assert sum(isinstance(g, list) and g == [] for g in got) >= 3      # empty.wav, broken.wav, rate0.wav
 
 
+def test_per_file_results_and_bookkeeping(indir, table):
+    """The per-file calls' own results, whatever the list forms return: [] for audio without
+    samples, for an unreadable file and, at shifts < 2, for a WAV without hashes (at shifts >= 2 an
+    empty (0, 2) array); `shifts` empty peak lists for audio without samples; .afpt hashes and .afpk
+    peaks as loaded, and an .afpt read as audio by wavfile2peaks.  Each call counts its file once and
+    leaves `last_batch_durations`, which is list-form output, as it was."""
+    def empty_list(x):
+        return type(x) is list and x == []
+    for shifts in (1, 4):
+        an = _analyzer(shifts)
+        an.last_batch_durations = mark = [7.0]
+        with contextlib.redirect_stdout(io.StringIO()):
+            assert all(empty_list(an.wavfile2hashes(f)) for f in ("empty.wav", "broken.wav", "rate0.wav"))
+            tiny = an.wavfile2hashes("tiny.wav")
+            assert empty_list(tiny) if shifts < 2 else (type(tiny) is np.ndarray and tiny.shape == (0, 2))
+            assert an.wavfile2hashes("q.afpt") == an_mod.hashes_load("q.afpt")
+            assert an.wavfile2peaks("q.afpk", shifts) == an_mod.peaks_load("q.afpk")
+            assert an.wavfile2peaks("empty.wav", shifts) == ([[]] * shifts if shifts >= 2 else [])
+            assert an.wavfile2peaks("q.afpt", 3) == [[], [], []]
+            rows, sec, nh = make_matcher().match_file(an, table, "empty.wav")
+            assert rows.shape == (0, 7) and sec == 0.0 and nh == 0
+        assert an.soundfilecount == 9 and an.last_batch_durations is mark
+
+
 def test_tiny_caps_give_the_same_result(indir, table):
     mt = make_matcher(**MATCH_CONFIGS["exact_range_time"])
     want, out_w = _batch(mt, _analyzer(4), table, indir)

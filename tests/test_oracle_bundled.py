@@ -110,10 +110,11 @@ def test_bundled_query_is_found_in_full_circle(gb):
         assert str(gb[tag + "/query_s4/default/msgs"][0]).startswith("Matched query.mp3 5.6 sec")
 
 
-def test_mirror_report_lines_from_the_reference_rows(gb):
+def test_mirror_report_lines_from_the_reference_hashes_and_rows(gb):
     """Host half of Matcher.file_match_to_msgs / match_file (sort_by_time, max_returns, the -R
-    line, terse form) with the device calls replaced by the reference's own rows: the mirror
-    prints the reference's lines (audfprint_match.py:354-420)."""
+    line, terse form) with the device calls (the hashes of the file, the match of its query)
+    replaced by the reference's own hashes and rows: the mirror prints the reference's lines
+    (audfprint_match.py:354-420)."""
     from audfprint_b200 import Analyzer, Matcher
     overrides = {"default": {}, "top5": {"max_returns": 5}, "exact": {"max_returns": 5, "exact_count": True},
                  "range": {"max_returns": 5, "find_time_range": True},
@@ -137,8 +138,8 @@ def test_mirror_report_lines_from_the_reference_rows(gb):
             for k, v in overrides[cfg].items():
                 setattr(mt, k, v)
             an = Analyzer()
-            an.wavfile2hashes = lambda fn, h=gb["%s/%s/hashes" % (tag, qkey)]: h
-            mt.match_hashes = lambda ht, q, r=gb[key + "/rows"].astype(np.int32): r
+            an._hashes_of_files = lambda names, rows_on_device=False, h=gb["%s/%s/hashes" % (tag, qkey)]: ([h], [0.0])
+            mt.match_batch = lambda ht, queries, r=gb[key + "/rows"].astype(np.int32): [r]
             assert mt.file_match_to_msgs(an, Table, qname) == [str(x) for x in gb[key + "/msgs"]], key
             if key + "/msgs_terse" in gb.files:
                 mt.verbose = False
